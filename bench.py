@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- training rays/sec of the EmerNeRF per-ray-batch hot path on B200.
+"""bench.py -- training rays/sec of the EmerNeRF per-ray-batch hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            (torchrun for N > 1)
     python bench.py --impl reference ...                      (the reference's algorithm on host cores)
@@ -13,7 +13,8 @@ collective is the gradient all-reduce.
 One JSON line on stdout (rank 0): metric/value/unit/..., plus
   e2e          same metric through the public API with HOST (pinned) input batches copied H2D inside
                every step and the loss read back D2H
-  roofline     the dominant kernel of the step vs the measured peak in MEASURED_PEAKS.json
+  roofline     the dominant kernel of the step vs the measured peak in MEASURED_PEAKS.json (if present; else the
+               H100 SXM data-sheet figures)
   cpu_baseline the CPU oracle (restatement of the reference, oracle/) timed on this box's host cores
                on a bounded sample of the same workload
 """
@@ -63,6 +64,8 @@ def parse():
                     help="weak: --rays per GPU; strong: --rays in total, split over the GPUs (BASELINE configs[3,4])")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of replaying "
                     "the captured CUDA graphs of the step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (see dump_outputs)")
     return ap.parse_args()
 
 
@@ -158,7 +161,7 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-# ----------------------------------------------------------------------------- the B200 arm
+# ----------------------------------------------------------------------------- the GPU arm
 class Trainer:
     def __init__(self, args, rank, world, device):
         from emernerf_b200 import configs, synthetic
@@ -211,7 +214,7 @@ class Trainer:
     # ---- CUDA graphs: the step is ~10^2 small launches; capture it once per schedule branch
     def build_graphs(self):
         self.static = {k: torch.empty_like(v) for k, v in self.dev[0].items()}
-        self.graphs, self.static_loss = {}, {}
+        self.graphs, self.static_loss, self.static_out = {}, {}, {}
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -227,6 +230,7 @@ class Trainer:
             n0 = _lib.LAUNCHES
             with torch.cuda.graph(g):
                 self.static_loss[prg] = self._step_body(self.static, prg)
+            self.static_out[prg] = self.last_out                # graph-owned: refreshed by every replay
             self.graph_launches[prg] = _lib.LAUNCHES - n0      # library kernels inside this graph
             self.graphs[prg] = g
 
@@ -288,6 +292,7 @@ class Trainer:
                 v.copy_(src[k], non_blocking=True)
             self.graphs[prg].replay()
             self.replayed_launches = getattr(self, "replayed_launches", 0) + self.graph_launches[prg]
+            self.last_out, self.last_loss = self.static_out[prg], self.static_loss[prg]
             return self.static_loss[prg]
         if from_host:
             batch = {k: v.to(self.device, non_blocking=True) for k, v in self.host[i % 8].items()}
@@ -310,7 +315,49 @@ class Trainer:
         self.opt.zero_grad()
         (loss * 1024.0).backward()                # GradScaler(2**10).scale(loss), never unscaled (Q17)
         self.sync_and_step(self.opt, self.params)
+        # detached (same memory): a held autograd graph would break the next graph capture
+        self.last_out, self.last_loss = _detached(out), loss.detach()
         return loss
+
+
+def _detached(d):
+    return {k: _detached(v) if isinstance(v, dict) else (v.detach() if torch.is_tensor(v) else v) for k, v in d.items()}
+
+
+DUMP_TABLE_SAMPLE = 1 << 18          # entries of a hash table written by --dump-outputs (fixed seeded sample)
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(tr, out_dir):
+    """What the last timed step computed, as float32 ``out_dir/<name>.npy``: its render outputs (``out.*``), loss, and the
+    parameters its optimizer step left (``param.*``; tensors above 2^20 elements as a fixed seeded sample of 2^18)."""
+    import numpy as np
+
+    torch.cuda.synchronize()
+    arrays = {"loss": tr.last_loss}
+
+    def walk(prefix, d):
+        for k, v in d.items():
+            if isinstance(v, dict):
+                walk(f"{prefix}{k}.", v)
+            elif torch.is_tensor(v) and v.is_floating_point():
+                arrays[prefix + k] = v
+
+    walk("out.", tr.last_out)
+    g = torch.Generator().manual_seed(0)
+    for tag, m in [("field", tr.field)] + [(f"prop{i}", p) for i, p in enumerate(tr.props)]:
+        for k, v in m.named_parameters():
+            flat = v.detach().reshape(-1)
+            if flat.numel() > (1 << 20):
+                flat = flat[torch.randint(0, flat.numel(), (DUMP_TABLE_SAMPLE,), generator=g).to(flat.device)]
+            arrays[f"param.{tag}.{k}"] = flat
+    host = {k: v.detach().float().cpu().numpy() for k, v in arrays.items()}
+    total = sum(a.nbytes for a in host.values())
+    assert total <= DUMP_LIMIT_BYTES, f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES} byte budget"
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in host.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
+    return total
 
 
 def timed(trainer, steps, from_host, sync):
@@ -399,7 +446,7 @@ def run_ours(args):
     local = int(os.environ.get("LOCAL_RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (no CPU fallback for the B200 arm)")
+        raise SystemExit("bench.py needs a CUDA device (no CPU fallback for the GPU arm)")
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     if world > 1:
@@ -427,6 +474,8 @@ def run_ours(args):
     tr.replayed_launches = 0
     ms = timed(tr, args.steps, False, sync)
     launches = (_lib.LAUNCHES - launches0) + tr.replayed_launches
+    if args.dump_outputs and rank == 0:
+        dump_outputs(tr, args.dump_outputs)
 
     e2e = None
     if not args.no_e2e:
@@ -441,7 +490,7 @@ def run_ours(args):
 
     # per-kernel device times: CUDA events around every library launch over 3 eager steps, same
     # process / inputs / clocks, right after the timed region (a replayed graph cannot be event-timed
-    # per kernel).  The ncu launch list under profiles/ must agree on the kernel's SHARE.
+    # per kernel).
     table = kernel_table(tr, sync, steps=3)          # every rank runs it (the steps all-reduce)
 
     # a whole reference training iteration: pixel pass + lidar pass, two (three) optimizer steps
@@ -494,8 +543,8 @@ def run_ours(args):
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peaks = json.load(open(pk))
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
 
     tot_ms = sum(v[1] for v in table.values())
     per_launch = {k: v[1] / v[0] for k, v in table.items()}
@@ -507,17 +556,6 @@ def run_ours(args):
             print(f"# {k[0]:26s} {k[1]:32s} n={v[0]:3d} {v[1] / 3:8.3f} ms/step {100 * v[1] / tot_ms:5.1f}%",
                   file=sys.stderr)
         print(f"# library kernels: {tot_ms / 3:.3f} ms/step of {ms / args.steps:.3f} ms/step", file=sys.stderr)
-
-    # DRAM bytes per launch and tensor-pipe activity measured by `ncu --set full` on this build's kernels
-    # (profiles/r2_dram_traffic.json, extracted from the reports summarised in profiles/r2_*_ncu_summary.md)
-    try:
-        NCU = json.load(open(os.path.join(ROOT, "profiles", "r2_dram_traffic.json")))
-    except Exception:
-        NCU = {}
-
-    def measured(name, tag):
-        e = NCU.get(f"{name}[{tag}]") or NCU.get(name) or {}
-        return e.get("traffic"), e.get("tensor_pipe_active_pct")
 
     def layer_bytes(name, tag):
         """Algorithmic HBM bytes of one dense-layer launch: rows * (inputs + outputs) * 4."""
@@ -532,7 +570,6 @@ def run_ours(args):
     def roofline_of(key):
         name, tag = key
         avg_ms = per_launch[key]
-        traffic = measured(name, tag)[0]
         if name == "emer_grid_fwd":
             nbytes = _lib.algorithmic_bytes(tag)
         elif name == "emer_grid_bwd":
@@ -550,10 +587,7 @@ def run_ours(args):
             return None
         ach = nbytes / (avg_ms / 1e3) / 1e9
         return {"kernel": f"{name}[{tag}]", "bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                "frac": ach / hbm_peak, "traffic": traffic,
-                # what actually crossed the DRAM pins (ncu) over the same time: the L2 serves the rest of the algorithmic bytes
-                "dram_frac": (traffic / (avg_ms / 1e3) / 1e9 / hbm_peak) if traffic else None,
-                "tensor_pipe_active_pct": measured(name, tag)[1], "peak_source": peak_src,
+                "frac": ach / hbm_peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": nbytes, "avg_launch_ms": avg_ms, "launches_timed": table[key][0],
                 "share_of_library_kernel_time": table[key][1] / tot_ms,
                 "timing": "CUDA events around each launch, 3 eager steps after the timed region"}
@@ -570,23 +604,22 @@ def run_ours(args):
         m = re.match(r"k(\d+)_f(\d+)_N(\d+)(_save)?", key[1])
         k_enc, nf, n = int(m.group(1)), int(m.group(2)), int(m.group(3))
         if name == "emer_field_fwd":
-            macs = k_enc * 64 + 64 * nf + 64 * 128 + 64 * 64 + 64 * 16
+            macs = k_enc * 64 + 64 * nf + 64 * 128 + 64 * 64 + 64 * 8
             nbytes = n * 4 * (k_enc + 4 + (256 if m.group(4) else 0) + (64 if nf == 128 else 0))
         else:
-            macs = 8 * 64 + 64 * 128 + 64 * 64 + nf * 64 + 64 * ((k_enc + 15) // 16 * 16)
+            macs = 8 * 64 + 64 * 128 + 64 * 64 + nf * 64 + 64 * k_enc
             nbytes = n * 4 * (8 + 256 + 64 + 128 + 64 + k_enc)     # d_rgb, rgb, sigmas | saved activations | dz1, d1, dzb, d_enc
         avg_ms = per_launch[key]
-        tf32_peak = float(peaks.get("bf16_tflops", 1590.0)) / 2.0
+        tf32_peak = float(peaks.get("bf16_tflops", 989.0)) / 2.0
         executed = 3 * 2 * macs * n / (avg_ms / 1e3) / 1e12
         return {"kernel": f"{name}[{key[1]}]", "bound": "tensor", "achieved": executed, "peak": tf32_peak, "unit": "TFLOP/s",
                 "frac": executed / tf32_peak,
-                "peak_source": ("measured bf16 (MEASURED_PEAKS.json) / 2: tf32 tcgen05.mma runs at half the bf16 rate"
-                                if "bf16_tflops" in peaks else "fallback 1590 / 2"),
+                "peak_source": ("measured bf16 (MEASURED_PEAKS.json) / 2: tf32 wgmma runs at half the bf16 rate"
+                                if "bf16_tflops" in peaks else "H100 SXM data sheet, dense bf16 989 / 2"),
                 "algorithmic_tflops": 2 * macs * n / (avg_ms / 1e3) / 1e12,
                 "executed_over_algorithmic": 3, "hbm_gbs": nbytes / (avg_ms / 1e3) / 1e9, "hbm_frac": nbytes / (avg_ms / 1e3) / 1e9 / hbm_peak,
                 "algorithmic_bytes_per_launch": nbytes, "avg_launch_ms": avg_ms, "launches_timed": table[key][0],
-                "share_of_library_kernel_time": table[key][1] / tot_ms, "traffic": measured(name, key[1])[0],
-                "tensor_pipe_active_pct_ncu": measured(name, key[1])[1]}
+                "share_of_library_kernel_time": table[key][1] / tot_ms}
 
     roof = roofline_of(dom)                                  # the kernel with the largest share of the step
     roof_grid = roofline_of(grid_dom) if grid_dom is not None else None   # the hash-grid gather (north star)
@@ -598,7 +631,7 @@ def run_ours(args):
         "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None, "dtype": "f32",
         "data": "synthetic Waymo-shape rays (3 cams, 640x960, 200 timesteps), random-init MLPs, N(0,0.3) tables",
         "config": dict(workload_config(args, world),
-                       l2="no explicit flush: each step streams > 1 GB of tables+activations through the 126 MB L2",
+                       l2="no explicit flush: each step streams > 1 GB of tables+activations through the 50 MB L2",
                        optimizer=args.optimizer,
                        gradient_exchange=("none (1 GPU)" if world == 1 else
                                           (f"{args.dp_mode}: one flat NCCL collective per optimizer group, "
@@ -683,7 +716,7 @@ def cpu_baseline(args, steps, warmup):
 
 
 def parity_vs_oracle(tr, args, at_start=True):
-    """PSNR (datasets/metrics.py:31-46: -10 log10 mse) and max relative errors of the B200 render against the CPU
+    """PSNR (datasets/metrics.py:31-46: -10 log10 mse) and max relative errors of the GPU render against the CPU
     oracle -- the reference's algorithm -- on the SAME weights (the benchmark's starting state; and, for the record, the
     trainer's after the timed steps) and the same ``--cpu-rays`` Waymo-shape rays, evaluation mode (deterministic: no
     jitter, unit temporal-aggregation noise).

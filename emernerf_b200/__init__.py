@@ -1,4 +1,4 @@
-"""emernerf_b200 -- B200-native (sm_100a) volumetric renderer for EmerNeRF's per-ray-batch hot path.
+"""emernerf_b200 -- H100-native (sm_90a) volumetric renderer for EmerNeRF's per-ray-batch hot path.
 
 Drop-in for the reference's ``radiance_fields`` package and ``third_party.nerfacc_prop_net`` /
 ``third_party.tcnn_modules`` modules: same class names, constructor arguments, ``forward`` /
@@ -20,7 +20,7 @@ __version__ = "0.1.0"
 
 def install_dropin() -> None:
     """Alias the reference's module names to this package in ``sys.modules`` so that
-    ``train_emernerf.py`` / ``builders.py`` import the B200 path without modification."""
+    ``train_emernerf.py`` / ``builders.py`` import the GPU path without modification."""
     import importlib
     import importlib.util
     import os

@@ -20,12 +20,12 @@ from .grid_desc import GridDesc
 import os
 
 ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
-# Dense layers run on the tcgen05 tensor-core kernels (3xTF32, fp32-accurate).  "simt" selects the
-# fp32 CUDA-core kernels of linear_simt.cu (the bit-faithful checker); both are sm_100a code in the
+# Dense layers run on the wgmma tensor-core kernels (3xTF32, fp32-accurate).  "simt" selects the
+# fp32 CUDA-core kernels of linear_simt.cu (the bit-faithful checker); both are sm_90a code in the
 # same library -- this is a debugging switch, not a backend dispatch.
 LINEAR_IMPL = os.environ.get("EMER_LINEAR", "tc")
-LINEAR_WGRAD_IMPL = os.environ.get("EMER_LINEAR_WGRAD", "mn")      # "mn": MN-major operands (csrc/wgrad_mn.cu) where the shape
-                                                                   # allows, else "tc" (transposing, linear_tc.cu); "simt"
+LINEAR_WGRAD_IMPL = os.environ.get("EMER_LINEAR_WGRAD", "mn")      # "mn" / "tc": the tensor-core weight gradient (csrc/wgrad_mn.cu,
+                                                                   # through either entry point); "simt"
 SKIP_BWD_IMPL = os.environ.get("EMER_SKIP_BWD", "stack")   # "stack": one stacked product; "add": two + add
 TC_MIN_ROWS = int(os.environ.get("EMER_TC_MIN_ROWS", "1024"))   # below: the FP32-FMA kernels (tiny per-ray heads are launch-bound either way)
 STOT_KINDS = {"uniform": 0, "lindisp": 1, "sqrt": 2, "log": 3, "uniform_lindisp": 4, "uniform_lindisp_0": 5}
@@ -201,12 +201,6 @@ class _GridEncode(torch.autograd.Function):
         sink = _grad_sink(params) if need_p else None
         if sink is not None:
             dparams = sink[0]                     # the optimizer's pre-zeroed slice: scatter straight into it
-            if sink[2] is not None and not sink[2]():
-                # first gradient of this step: the slice is all zeros (the optimizer cleared it a step ago) but no longer
-                # in L2, and a red.add on a missing line is a DRAM read-modify-write.  Re-writing the zeros write-allocates
-                # the lines in the 126 MB L2 right before the scatter: measured 0.38 -> 0.29 ms for the 122 MB table
-                # against 0.03 ms for the fill (what torch.zeros_like did for the plain autograd path, by accident)
-                dparams.zero_()
         else:
             dparams = torch.zeros_like(params) if need_p else None
         dx = torch.empty_like(x) if need_x else None
@@ -328,16 +322,15 @@ _SMEM_MAX = 227 * 1024
 
 def _tc_fits(kred: int, ncols: int) -> bool:
     """Whether tc_linear_kernel can take a layer with reduction width ``kred`` and output width ``ncols``
-    (csrc/linear_tc.cu, launch<>): one MMA spans the padded output width, and the resident hi/lo weight panels
-    plus the smallest operand ring must fit shared memory.  Wider layers run on the CUDA-core kernels."""
-    n_pad, kred_pad = _round_up(ncols, 16), _round_up(kred, 8)
-    w_bytes = 2 * (kred_pad // 4) * n_pad * 16
-    return n_pad <= 256 and w_bytes + 128 * 68 * 4 + (256 * 4 + 6 * 8 + 16) <= _SMEM_MAX
+    (csrc/linear_tc.cu, launch<>): the output width padded to 16 is at most 256, and the resident hi/lo weight panels
+    (reduction width padded to 32) plus the bias fit shared memory.  Wider layers run on the CUDA-core kernels."""
+    n_pad, kred_pad = _round_up(ncols, 16), _round_up(kred, 32)
+    return n_pad <= 256 and 2 * (kred_pad // 4) * n_pad * 16 + n_pad * 4 <= _SMEM_MAX
 
 
 def _tc_wgrad_fits(k: int, n_out: int) -> bool:
-    """Same for tc_wgrad_kernel (emer_linear_tc_bwd_weight): TMEM columns for dW^T and one of its tile configurations
-    in shared memory."""
+    """Same for the tensor-core weight gradient (emer_linear_tc_bwd_weight): the layer widths it is used for.  (The
+    kernel takes any k <= 256, n_out <= 128; this keeps the routing the library has always had.)"""
     if n_out > 128 or k > 256:
         return False
     k_pad4, n_pad, m_blocks = _round_up(k, 4), _round_up(n_out, 16), (k + 127) // 128
@@ -409,7 +402,7 @@ def _layer_bwd_weight(x2: Tensor, ldx: int, dz: Tensor, lddz: int, w: Tensor, ha
         _lib.call("emer_linear_narrow_bwd_weight", _ptr(x2), ldx, _ptr(dz), lddz, _ptr(dw), _ptr(db), n, k, n_out,
                   _stream())
     elif tc and LINEAR_WGRAD_IMPL == "mn" and n_out == 64 and 4 <= k <= 128:
-        # operands as they lie in memory (MN-major, csrc/wgrad_mn.cu): no transposition while staging
+        # the field chain's 64-wide layers (csrc/wgrad_mn.cu)
         _lib.call("emer_linear_tc_bwd_weight_mn", _ptr(x2), ldx, _ptr(dz), lddz, _ptr(dw), _ptr(db), n, k, n_out,
                   _stream())
     elif tc:
@@ -1046,7 +1039,7 @@ def interlevel_loss(s: Tensor, cdf: Tensor, prop_s: Tensor, prop_cdf: Tensor, pu
 class _GatherRows(torch.autograd.Function):
     """``table[idx]`` for a small table hit by many repeated indices (the appearance embedding: 8192 rays over a few
     hundred rows).  The backward of torch's advanced indexing / nn.Embedding sorts the indices first -- a 64-bit radix
-    sort, ~12 launches and 0.09 ms of a 2.6 ms step; one pass of atomic adds needs neither."""
+    sort, ~12 launches; one pass of atomic adds needs neither."""
 
     @staticmethod
     def forward(ctx, table: Tensor, idx: Tensor):

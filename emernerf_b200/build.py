@@ -1,7 +1,7 @@
-"""Build libemer_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libemer_b200.so (sm_90a only) in-tree with nvcc.
 
-The shared library is the product: ``emernerf_b200/lib/libemer_b200.so`` is git-ignored but
-travels to the GPU box with the gpurun snapshot.  ``python -m emernerf_b200.build`` (re)builds it;
+The shared library is the product: ``emernerf_b200/lib/libemer_b200.so`` is git-ignored and built in
+the checkout.  ``python -m emernerf_b200.build`` (re)builds it;
 ``__graft_entry__.build()`` calls :func:`build_library`.
 """
 from __future__ import annotations
@@ -21,17 +21,12 @@ LIB_PATH = os.path.join(LIB_DIR, "libemer_b200.so")
 OBJ_DIR = os.path.join(PKG, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-fmad=false",                     # FMAs are explicit (fmaf); see csrc/common.cuh
     "-Xcompiler", "-fPIC",
     "-I", os.path.join(ROOT, "include"), "-I", CSRC,
 ]
-# compile-time experiment switches of the kernels (see the comment at each #ifndef in csrc/): passed through
-# from the environment so that an A/B build is one command; the default build defines none of them
-for _flag in ("EMER_TC_ELECT_ONE", "EMER_WARP_ARRIVE", "EMER_CHAIN_STAGE"):
-    if os.environ.get(_flag):
-        NVCC_FLAGS.append(f"-D{_flag}={os.environ[_flag]}")
 
 
 def _nvcc() -> str:

@@ -1,4 +1,4 @@
-// Shared helpers for libemer_b200 (sm_100a).  Compiled with -fmad=false: every fused
+// Shared helpers for libemer_b200 (sm_90a).  Compiled with -fmad=false: every fused
 // multiply-add in this library is written explicitly (fmaf), everything else rounds per
 // operation exactly like the fp32 torch ops of the reference, which is what makes sample
 // offsets / grid indices reproducible bit for bit against the CPU oracle.
@@ -25,6 +25,20 @@ inline int check_launch(const char* what) {
 }
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// CTAs of `kernel` resident per SM, queried once per device into `cache[device]`, never inside a graph capture (1 until then)
+template <typename Kernel>
+int resident_ctas(Kernel kernel, int threads, size_t smem, cudaStream_t stream, int* cache) {
+    int& c = cache[current_device()];
+    if (c == 0) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        int v = 0;
+        if (cudaStreamIsCapturing(stream, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) return 1;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kernel, threads, smem) != cudaSuccess || v < 1) v = 1;
+        c = v;
+    }
+    return c;
+}
 
 #define EMER_REQUIRE(cond, ...)          \
     do {                                 \

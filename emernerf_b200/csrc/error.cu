@@ -23,7 +23,7 @@ int sm_count() {
     const int dev = current_device();
     if (g_sm_count[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;   // H100 SXM
         g_sm_count[dev] = n;
     }
     return g_sm_count[dev];

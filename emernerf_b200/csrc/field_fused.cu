@@ -1,5 +1,5 @@
-// The fused field chain on tcgen05: hash-grid features -> base MLP -> density + colour head, ONE persistent kernel,
-// activations never leave the SM.
+// The fused field chain on Hopper warpgroup MMA: hash-grid features -> base MLP -> density + colour head, ONE persistent
+// kernel, activations never leave the registers.
 //
 // Replaces, for one [N, k_enc] block of hash-grid features (reference: radiance_fields/radiance_field.py)
 //     feats = base_mlp(enc)                       Linear(k_enc,64)-ReLU-Linear(64, 64 [+64 semantic])     :74-80,314-318
@@ -14,25 +14,8 @@
 //     h1 = relu(h0 W1h^T + geo W1g^T + ray_bias1[ray]) 128 -> 64
 // and the [N, 113] / [N, 177] concatenations of the reference never exist.
 //
-// Tensor-core mapping (3xTF32, fp32-accurate, see linear_tc.cu): a tile is 128 points = the 128 TMEM lanes.  Weights
-// (B operands) are resident in shared memory as tf32 hi / lo panels.  ACTIVATIONS LIVE IN TENSOR MEMORY: the epilogue of
-// layer i reads its accumulator with tcgen05.ld, applies bias / ReLU, splits into tf32 hi + lo and writes them back with
-// tcgen05.st as the A operand of layer i+1 (tcgen05.mma with A in TMEM), so no activation ever touches shared memory.
-// Two tiles are in flight (256 TMEM columns each: 128 operand + 128 accumulator), each served by two warpgroups that take
-// the two 32-column halves of every 64-column block (the per-stage TMEM -> registers -> TMEM round trip is the serial part
-// of a tile's chain: with one thread per whole row the tensor pipe sat idle 70 % of the time); one warp issues the MMAs for
-// both tiles, alternating, so one tile's MMAs run under the other tile's epilogue.
-//
-//   stage  A (TMEM)        B (smem)          D (TMEM)                epilogue
-//   0      enc hi/lo       Wb0 [64 x k_enc]  [0,64)                  +bb0, relu            -> Hb
-//   1      Hb              Wb1 [nf x 64]     [0,nf)                  +bb1; sigma; geo      -> G   (sem -> HBM)
-//   2      G               [W0g;W1g] N=128   [0,64) pre-h0 | [64,128) partial h1   +ray_bias0, relu -> H0
-//   3      H0              W1h               [64,128) accumulate     +ray_bias1, relu      -> H1
-//   4      H1              W2 (3 -> N=16)    [0,16)                  +b2, sigmoid          -> rgb
-//
-// Roofline: per point 3 x (k_enc*64 + 64*nf + 64*128 + 64*64 + 64*16) MACs = 3 x 19 968 (k_enc = 40, nf = 64) on the
-// tensor pipe (2048 tf32 MAC / clk / SM -> 29.3 clk per point, 0.053 ms for 524 288 points on 148 SMs) against
-// (k_enc + 4) * 4 B = 176 B per point of HBM traffic without the training saves (0.014 ms) or + 1 KB with them.
+// Tensor-core mapping (3xTF32, tc_common.cuh; DESIGN.md §5.1): each warpgroup walks its own 64-point tiles through all
+// five layers; the weights are resident in shared memory, and the accumulator of layer i is the A operand of layer i+1.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -41,11 +24,9 @@ namespace ff {
 
 using namespace emer::tc;
 
-constexpr int ROWS = 128;
-constexpr int EPI_THREADS = 512;              // two tiles in flight x two warpgroups per tile (each takes half of the columns);
-                                              // warp w owns TMEM lanes 32 (w % 4) .. of its tile
-constexpr int THREADS = EPI_THREADS + 32;     // + the MMA-issuing warp
-constexpr int TILE_THREADS = EPI_THREADS / 2; // epilogue threads per tile (arrivals per operand barrier)
+constexpr int ROWS = 64;                      // points per tile = M of one wgmma
+constexpr int WGS = 3;                        // warpgroups per CTA, each on its own tiles
+constexpr int THREADS = WGS * 128;
 constexpr int H = 64;                         // hidden / geometry / head width this kernel is specialised for
 
 struct FwdParams {
@@ -58,483 +39,270 @@ struct FwdParams {
     float *sigma, *rgb;                                           // [N], [N, 3]
     float *save_hb, *save_hg, *save_h1, *save_sem;                // training saves: [N,64], [N,128]=[h0|geo], [N,64], [N,64]
     int64_t n;
-    int stg_off;                                                  // byte offset of the staging tiles in shared memory, 0 = none
 };
 
-// shared-memory map (bytes): B operands as K-major SWIZZLE_NONE panels, offset(row, k) = (k/4)*rows*16 + row*16 + (k%4)*4
+// shared-memory map (bytes): B operands as K-major panels (tc::b_off), hi and lo
 struct Smem {
-    int wb0_hi, wb0_lo, wb1_hi, wb1_lo, wg_hi, wg_lo, w1h_hi, w1h_lo, w2_hi, w2_lo, bias, bars, total;
+    int wb0_hi, wb0_lo, wb1_hi, wb1_lo, wg_hi, wg_lo, w1h_hi, w1h_lo, w2_hi, w2_lo, bias, total;
 };
 __host__ __device__ inline Smem smem_map(int k_enc, int n_feat) {
     Smem m;
     int o = 0;
     const int wb0 = (k_enc / 4) * H * 16, wb1 = (H / 4) * n_feat * 16, wg = (H / 4) * 128 * 16, w1h = (H / 4) * H * 16,
-              w2 = (H / 4) * 16 * 16;
+              w2 = (H / 4) * 8 * 16;
     m.wb0_hi = o; o += wb0; m.wb0_lo = o; o += wb0;
     m.wb1_hi = o; o += wb1; m.wb1_lo = o; o += wb1;
     m.wg_hi = o; o += wg; m.wg_lo = o; o += wg;
     m.w1h_hi = o; o += w1h; m.w1h_lo = o; o += w1h;
     m.w2_hi = o; o += w2; m.w2_lo = o; o += w2;
     m.bias = o; o += (64 + 128 + 4) * 4;          // bb0 | bb1 | b2
-    m.bars = o; o += 8 * 8;
     m.total = o;
     return m;
 }
 
-// stage one weight matrix w[rows_valid, k_valid] (row stride ld) into hi / lo panels of `rows` x `kpad`
+// B operand (n = row0 + r, k) = w[r, k] for a weight w[rows_valid, k_valid] (row stride ld), panels of `rows` rows
 __device__ __forceinline__ void stage_weight(uint8_t* hi, uint8_t* lo, const float* __restrict__ w, int64_t ld, int rows,
-                                             int rows_valid, int kpad, int k_valid, int row0, int tid, int nthreads) {
-    const int panel = rows * 16;
-    for (int e = tid; e < rows_valid * kpad; e += nthreads) {
-        const int r = e / kpad, k = e - r * kpad;
-        float v = 0.0f;
-        if (k < k_valid) v = __ldg(w + (int64_t)r * ld + k);
+                                             int rows_valid, int k_valid, int row0, int tid) {
+    for (int e = tid; e < rows_valid * k_valid; e += THREADS) {
+        const int r = e / k_valid, k = e - r * k_valid;
         float h, l;
-        split(v, h, l);
-        const int off = (k >> 2) * panel + (row0 + r) * 16 + (k & 3) * 4;
+        split(__ldg(w + (int64_t)r * ld + k), h, l);
+        const int off = b_off(row0 + r, k, rows);
+        *reinterpret_cast<float*>(hi + off) = h;
+        *reinterpret_cast<float*>(lo + off) = l;
+    }
+}
+// B operand (n = row0 + j, k = o) = w[o, j]: the transposed weight of a data gradient
+__device__ __forceinline__ void stage_weight_t(uint8_t* hi, uint8_t* lo, const float* __restrict__ w, int64_t ld, int rows,
+                                               int rows_valid, int k_valid, int row0, int tid) {
+    for (int e = tid; e < rows_valid * k_valid; e += THREADS) {
+        const int o = e / rows_valid, j = e - o * rows_valid;        // consecutive threads: consecutive j (coalesced)
+        float h, l;
+        split(__ldg(w + (int64_t)o * ld + j), h, l);
+        const int off = b_off(row0 + j, o, rows);
         *reinterpret_cast<float*>(hi + off) = h;
         *reinterpret_cast<float*>(lo + off) = l;
     }
 }
 
-__device__ __forceinline__ void split16(const float (&v)[16], uint32_t (&hi)[16], uint32_t (&lo)[16]) {
+__device__ __forceinline__ float2 ld2(const float* p, bool ok) {
+    return ok ? __ldg(reinterpret_cast<const float2*>(p)) : make_float2(0.f, 0.f);
+}
+__device__ __forceinline__ void st2(float* p, float a, float b, bool ok) {
+    if (ok) *reinterpret_cast<float2*>(p) = make_float2(a, b);
+}
+
+// dZ = acc * (saved > 0) on this thread's rows (saved and dst have row stride ld), stored, and split into the next A
+__device__ __forceinline__ void relu_back(float (&acc)[32], const float* saved, float* dst, int64_t ld, int64_t row0,
+                                          int64_t row1, bool ok0, bool ok1, int q, uint32_t (&ahi)[8][4],
+                                          uint32_t (&alo)[8][4]) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-        float h, l;
-        split(v[j], h, l);
-        hi[j] = __float_as_uint(h);
-        lo[j] = __float_as_uint(l);
+    for (int j = 0; j < 8; ++j) {
+        const int c = 8 * j + 2 * q;
+        const float2 m0 = ld2(saved + row0 * ld + c, ok0), m1 = ld2(saved + row1 * ld + c, ok1);
+        acc[4 * j] = m0.x > 0.f ? acc[4 * j] : 0.f;
+        acc[4 * j + 1] = m0.y > 0.f ? acc[4 * j + 1] : 0.f;
+        acc[4 * j + 2] = m1.x > 0.f ? acc[4 * j + 2] : 0.f;
+        acc[4 * j + 3] = m1.y > 0.f ? acc[4 * j + 3] : 0.f;
+        st2(dst + row0 * ld + c, acc[4 * j], acc[4 * j + 1], ok0);
+        st2(dst + row1 * ld + c, acc[4 * j + 2], acc[4 * j + 3], ok1);
+        frag_split(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], ahi[j], alo[j]);
     }
 }
 
-// 256-bit global accesses (sm_100: LDG / STG .256).  A thread owns a ROW here (its TMEM lane), so every 16-byte access of a
-// warp lands in a different 32-byte sector and the L1 data pipe -- one wavefront per sector -- was 71-74 % busy in both
-// kernels with HALF-used sectors (34 M store sectors for 503 MB in the forward, profiles/r2_chain_ncu_summary.md).
-// 32 bytes per instruction fills a sector per wavefront: half the wavefronts, no staging latency.  Addresses must be
-// 32-byte aligned (the entry points check the buffers; row strides and column offsets are multiples of 8 floats).
-__device__ __forceinline__ void st8(float* dst, float a0, float a1, float a2, float a3, float a4, float a5, float a6, float a7) {
-    asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 :: "l"(dst), "f"(a0), "f"(a1), "f"(a2), "f"(a3), "f"(a4), "f"(a5), "f"(a6), "f"(a7) : "memory");
-}
-__device__ __forceinline__ void ld8(const float* src, float (&v)[8]) {
-    asm volatile("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(src));
-}
-
-__device__ __forceinline__ void store16(float* dst, const float (&v)[16]) {
-    st8(dst, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-    st8(dst + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
-}
-
-// bit j of the result: x[j] > 0 for 32 floats of one saved activation row
-__device__ __forceinline__ uint32_t relu_mask32(const float* __restrict__ row, bool ok) {
-    uint32_t m = 0;
-    if (ok) {
+// Adds the column sums over the warp's 16 rows of a 64-column accumulator block to dst[0, 64).
+__device__ __forceinline__ void ray_colsum(const float (&v)[32], float* dst, int lane, bool live) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            float t[8];
-            ld8(row + 8 * q, t);
+    for (int j = 0; j < 8; ++j) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) m |= (uint32_t)(t[j] > 0.f) << (8 * q + j);
+        for (int e = 0; e < 2; ++e) {
+            float s = v[4 * j + e] + v[4 * j + 2 + e];
+            s += __shfl_xor_sync(0xffffffffu, s, 4);
+            s += __shfl_xor_sync(0xffffffffu, s, 8);
+            s += __shfl_xor_sync(0xffffffffu, s, 16);
+            if (lane < 4 && live) atomicAdd(dst + 8 * j + 2 * lane + e, s);
         }
     }
-    return m;
 }
 
-// ---- coalesced row I/O through shared memory (EMER_CHAIN_STAGE=1; measured, NOT the default) --------------------------
-// Each epilogue warp owns a 32 x 16-float tile in shared memory: rows go in one per lane and come out 8 rows x 64 bytes
-// per instruction; saved activations come IN 4 rows x 128 bytes per instruction and only their sign bits are exchanged.
-// Row stride 80 B: 8 consecutive lanes hit 8 different 16-byte bank groups both as "lane = row" and as "8 lanes = one
-// 16-byte piece of 8 rows".  A/B on one box (GPU suite green on both): forward 0.315 ms with, 0.260 ms without; backward
-// 0.334 / 0.353 ms -- the two __syncwarp + shared-memory round trips sit on the serial path of every stage, and the
-// data pipe counts SECTORS, which 64-byte pieces only halve.  The 256-bit row accesses above halve them for free.
-#ifndef EMER_CHAIN_STAGE
-#define EMER_CHAIN_STAGE 0
-#endif
-constexpr int STG_LD = 20;
-constexpr int STG_BYTES = 32 * STG_LD * 4;                 // per epilogue warp
-constexpr int STG_TOTAL = (EPI_THREADS / 32) * STG_BYTES;
-
-// v = 16 columns of this lane's row; dst = address of (the warp's first row, first of the 16 columns)
-__device__ __forceinline__ void put16(float* stg, int lane, const float (&v)[16], float* dst, int64_t ld, int rows_valid) {
-    if (stg == nullptr) {
-        if (lane < rows_valid) store16(dst + (int64_t)lane * ld, v);
-        return;
-    }
-    __syncwarp();                                            // the tile's previous use is over
-    float* mine = stg + lane * STG_LD;
-#pragma unroll
-    for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(mine + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-    __syncwarp();
-    const int rr = lane & 7, q = lane >> 3;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int r = i * 8 + rr;
-        const float4 t = *reinterpret_cast<const float4*>(stg + r * STG_LD + q * 4);
-        if (r < rows_valid) *reinterpret_cast<float4*>(dst + (int64_t)r * ld + q * 4) = t;
-    }
-}
-
-// 8 columns (the last product's rows are k_enc wide: 8-column chunks)
-__device__ __forceinline__ void put8(float* stg, int lane, const float (&v)[8], float* dst, int64_t ld, int rows_valid) {
-    if (stg == nullptr) {
-        if (lane < rows_valid) st8(dst + (int64_t)lane * ld, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-        return;
-    }
-    __syncwarp();
-    float* mine = stg + lane * STG_LD;
-    *reinterpret_cast<float4*>(mine) = make_float4(v[0], v[1], v[2], v[3]);
-    *reinterpret_cast<float4*>(mine + 4) = make_float4(v[4], v[5], v[6], v[7]);
-    __syncwarp();
-    const int rr = lane & 15, q = lane >> 4;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const int r = i * 16 + rr;
-        const float4 t = *reinterpret_cast<const float4*>(stg + r * STG_LD + q * 4);
-        if (r < rows_valid) *reinterpret_cast<float4*>(dst + (int64_t)r * ld + q * 4) = t;
-    }
-}
-
-// bit j of the result: x[j] > 0 for the 32 floats at src + lane * ld (src = the warp's first row).  Staged form: the warp
-// reads 4 rows x 128 B per instruction, every lane turns its 16-byte piece into 4 sign bits, and the row's owner collects
-// its 8 nibbles from shared memory.
-__device__ __forceinline__ uint32_t get_mask32(float* stg, int lane, const float* __restrict__ src, int64_t ld, int rows_valid) {
-    if (stg == nullptr) return relu_mask32(src + (int64_t)lane * ld, lane < rows_valid);
-    uint8_t* nib = reinterpret_cast<uint8_t*>(stg);         // [32 rows][8 pieces]
-    const int piece = lane & 7, r0 = lane >> 3;
-    float4 t[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + r0;
-        t[i] = r < rows_valid ? __ldg(reinterpret_cast<const float4*>(src + (int64_t)r * ld) + piece) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + r0;
-        nib[r * 8 + piece] = (uint8_t)((t[i].x > 0.f) | ((t[i].y > 0.f) << 1) | ((t[i].z > 0.f) << 2) | ((t[i].w > 0.f) << 3));
-    }
-    __syncwarp();
-    const uint2 b = *reinterpret_cast<const uint2*>(nib + lane * 8);
-    // bytes b0..b7 hold one nibble each: mask = sum nibble_p << 4p
-    uint32_t m = 0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        m |= ((b.x >> (8 * k)) & 0xFu) << (4 * k);
-        m |= ((b.y >> (8 * k)) & 0xFu) << (16 + 4 * k);
-    }
-    return m;
-}
-
-template <int K_ENC>
+template <int K_ENC, int NF>
 __global__ void __launch_bounds__(THREADS, 1) field_fwd_kernel(const FwdParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
-    const Smem m = smem_map(K_ENC, p.n_feat);
+    const Smem m = smem_map(K_ENC, NF);
     float* bias_s = reinterpret_cast<float*>(smem + m.bias);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + m.bars);
-    uint64_t* a_full = bars;              // [2] epilogue warpgroup -> issuer: operand of the next layer is in TMEM
-    uint64_t* d_full = bars + 2;          // [2] issuer (tcgen05.commit) -> epilogue warpgroup: accumulator complete
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-
     const int tid = threadIdx.x;
-    const int warp = tid >> 5;
-    const bool is_issuer = warp == EPI_THREADS / 32;
 
-    if (tid == 0) {
-        mbar_init(&a_full[0], arrivals(TILE_THREADS));
-        mbar_init(&a_full[1], arrivals(TILE_THREADS));
-        mbar_init(&d_full[0], 1);
-        mbar_init(&d_full[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        __syncwarp();
-        tmem_alloc(tmem_slot, 512u);
-    }
-    // ---- resident weights (all threads): zero the padded rows first (W2: rows 3..15), then split and scatter
+    // ---- resident weights: zero the padded rows first (W2: rows 3..7), then split and scatter
     for (int i = tid * 16; i < m.bias; i += THREADS * 16) *reinterpret_cast<float4*>(smem + i) = make_float4(0.f, 0.f, 0.f, 0.f);
     __syncthreads();
-    stage_weight(smem + m.wb0_hi, smem + m.wb0_lo, p.wb0, K_ENC, H, H, K_ENC, K_ENC, 0, tid, THREADS);
-    stage_weight(smem + m.wb1_hi, smem + m.wb1_lo, p.wb1, H, p.n_feat, p.n_feat, H, H, 0, tid, THREADS);
-    stage_weight(smem + m.wg_hi, smem + m.wg_lo, p.w0g, p.ld_w0, 128, H, H, H, 0, tid, THREADS);
-    stage_weight(smem + m.wg_hi, smem + m.wg_lo, p.w1g, p.ld_w1, 128, H, H, H, H, tid, THREADS);
-    stage_weight(smem + m.w1h_hi, smem + m.w1h_lo, p.w1h, p.ld_w1, H, H, H, H, 0, tid, THREADS);
-    stage_weight(smem + m.w2_hi, smem + m.w2_lo, p.w2, H, 16, 3, H, H, 0, tid, THREADS);
+    stage_weight(smem + m.wb0_hi, smem + m.wb0_lo, p.wb0, K_ENC, H, H, K_ENC, 0, tid);
+    stage_weight(smem + m.wb1_hi, smem + m.wb1_lo, p.wb1, H, NF, NF, H, 0, tid);
+    stage_weight(smem + m.wg_hi, smem + m.wg_lo, p.w0g, p.ld_w0, 128, H, H, 0, tid);
+    stage_weight(smem + m.wg_hi, smem + m.wg_lo, p.w1g, p.ld_w1, 128, H, H, H, tid);
+    stage_weight(smem + m.w1h_hi, smem + m.w1h_lo, p.w1h, p.ld_w1, H, H, H, 0, tid);
+    stage_weight(smem + m.w2_hi, smem + m.w2_lo, p.w2, H, 8, 3, H, 0, tid);
     for (int e = tid; e < 64 + 128 + 4; e += THREADS) {
         float v = 0.0f;
         if (e < 64) v = __ldg(p.bb0 + e);
-        else if (e < 64 + 128) { if (e - 64 < p.n_feat) v = __ldg(p.bb1 + e - 64); }
+        else if (e < 64 + 128) { if (e - 64 < NF) v = __ldg(p.bb1 + e - 64); }
         else if (e - 192 < 3) v = __ldg(p.b2 + e - 192);
         bias_s[e] = v;
     }
     fence_async_proxy();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
+    const uint32_t sb = smem_u32(smem);
+    const int wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+    const float* bb0_s = bias_s;
+    const float* bb1_s = bias_s + 64;
+    const float* b2_s = bias_s + 192;
     const int64_t n_tiles = (p.n + ROWS - 1) / ROWS;
-    const int64_t pair_stride = (int64_t)gridDim.x * 2;
-    const int iters = (int)((n_tiles + pair_stride - 1) / pair_stride);
-    constexpr int ksteps0 = K_ENC / 8;
 
-    if (is_issuer) {
-        // ================= MMA issuer: stage s of warpgroup 0, stage s of warpgroup 1, stage s+1 of warpgroup 0, ...
-        const uint32_t sbase = smem_u32(smem);
-        const uint64_t d64 = make_desc(0, H * 16, 128), dnf = make_desc(0, p.n_feat * 16, 128),
-                       d128 = make_desc(0, 128 * 16, 128), d16 = make_desc(0, 16 * 16, 128);
-        const uint32_t id64 = make_idesc(128, 64), idnf = make_idesc(128, p.n_feat), id128 = make_idesc(128, 128),
-                       id16 = make_idesc(128, 16);
-        uint32_t ph[2] = {0, 0};
-        for (int it = 0; it < iters; ++it) {
-            for (int stage = 0; stage < 5; ++stage) {
-                for (int wg = 0; wg < 2; ++wg) {
-                    const int64_t tile = ((int64_t)it * gridDim.x + blockIdx.x) * 2 + wg;
-                    if (tile >= n_tiles) continue;
-                    mbar_wait(&a_full[wg], ph[wg]);
-                    ph[wg] ^= 1u;
-                    tc_fence_after();
-                    if (mma_issue_lane(tid)) {
-                        const uint32_t a_hi = tmem_base + (uint32_t)(wg * 256);
-                        const uint32_t a_lo = a_hi + 64u;
-                        uint32_t d = a_hi + 128u;
-                        uint64_t desc;
-                        uint32_t idesc, b_hi, b_lo, panel, acc0 = 0u;
-                        int ksteps = H / 8;
-                        if (stage == 0) { desc = d64; idesc = id64; b_hi = m.wb0_hi; b_lo = m.wb0_lo; panel = H * 16; ksteps = ksteps0; }
-                        else if (stage == 1) { desc = dnf; idesc = idnf; b_hi = m.wb1_hi; b_lo = m.wb1_lo; panel = p.n_feat * 16; }
-                        else if (stage == 2) { desc = d128; idesc = id128; b_hi = m.wg_hi; b_lo = m.wg_lo; panel = 128 * 16; }
-                        else if (stage == 3) { desc = d64; idesc = id64; b_hi = m.w1h_hi; b_lo = m.w1h_lo; panel = H * 16; d += 64u; acc0 = 1u; }
-                        else { desc = d16; idesc = id16; b_hi = m.w2_hi; b_lo = m.w2_lo; panel = 16 * 16; }
-                        const uint32_t bh = (sbase + b_hi) >> 4, bl = (sbase + b_lo) >> 4;
-                        for (int ks = 0; ks < ksteps; ++ks) {
-                            const uint32_t bo = (uint32_t)(ks * 2 * panel) >> 4;
-                            const uint64_t db_hi = desc | (uint64_t)(bh + bo), db_lo = desc | (uint64_t)(bl + bo);
-                            const uint32_t ah = a_hi + (uint32_t)(ks * 8), al = a_lo + (uint32_t)(ks * 8);
-                            mma_tf32_ts(d, ah, db_hi, idesc, (ks > 0) ? 1u : acc0);
-                            mma_tf32_ts(d, al, db_hi, idesc, 1u);
-                            mma_tf32_ts(d, ah, db_lo, idesc, 1u);
-                        }
-                        tc_commit(&d_full[wg]);
-                    }
-                    __syncwarp();
-                }
+    for (int64_t tile = (int64_t)blockIdx.x * WGS + wg; tile < n_tiles; tile += (int64_t)gridDim.x * WGS) {
+        const int64_t row0 = tile * ROWS + 16 * w + (lane >> 2), row1 = row0 + 8;
+        const bool ok0 = row0 < p.n, ok1 = row1 < p.n;
+        uint32_t ahi[8][4], alo[8][4];
+
+        // ---- stage 0: Hb = relu(enc Wb0^T + bb0)
+#pragma unroll
+        for (int j = 0; j < K_ENC / 8; ++j) {
+            const float2 x0 = ld2(p.enc + row0 * p.ld_enc + 8 * j + 2 * q, ok0);
+            const float2 x1 = ld2(p.enc + row1 * p.ld_enc + 8 * j + 2 * q, ok1);
+            frag_split(x0.x, x0.y, x1.x, x1.y, ahi[j], alo[j]);
+        }
+        float acc[32];
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < K_ENC / 8; ++ks)
+            mma3<64>(acc, ahi[ks], alo[ks], b_desc(sb + m.wb0_hi, H, ks, 0), b_desc(sb + m.wb0_lo, H, ks, 0), ks > 0);
+        wg_commit();
+        wg_wait0();
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + 2 * q;
+            const float v0 = fmaxf(acc[4 * j] + bb0_s[c], 0.0f), v1 = fmaxf(acc[4 * j + 1] + bb0_s[c + 1], 0.0f);
+            const float v2 = fmaxf(acc[4 * j + 2] + bb0_s[c], 0.0f), v3 = fmaxf(acc[4 * j + 3] + bb0_s[c + 1], 0.0f);
+            if (p.save_hb) {
+                st2(p.save_hb + row0 * H + c, v0, v1, ok0);
+                st2(p.save_hb + row1 * H + c, v2, v3, ok1);
+            }
+            frag_split(v0, v1, v2, v3, ahi[j], alo[j]);
+        }
+
+        // ---- stage 1: feats = Hb Wb1^T + bb1; sigma = exp(feats[0] - 1); geo -> operand; semantic half -> HBM
+        float geo[32], sem[NF > H ? 32 : 1];
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks) {
+            mma3<64>(geo, ahi[ks], alo[ks], b_desc(sb + m.wb1_hi, NF, ks, 0), b_desc(sb + m.wb1_lo, NF, ks, 0), ks > 0);
+            if constexpr (NF > H)
+                mma3<64>(sem, ahi[ks], alo[ks], b_desc(sb + m.wb1_hi, NF, ks, H), b_desc(sb + m.wb1_lo, NF, ks, H), ks > 0);
+        }
+        wg_commit();
+        wg_wait0();
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + 2 * q;
+            const float v0 = geo[4 * j] + bb1_s[c], v1 = geo[4 * j + 1] + bb1_s[c + 1];
+            const float v2 = geo[4 * j + 2] + bb1_s[c], v3 = geo[4 * j + 3] + bb1_s[c + 1];
+            if (j == 0 && q == 0) {
+                if (ok0) p.sigma[row0] = expf(v0 - 1.0f);
+                if (ok1) p.sigma[row1] = expf(v2 - 1.0f);
+            }
+            if (p.save_hg) {
+                st2(p.save_hg + row0 * 128 + H + c, v0, v1, ok0);
+                st2(p.save_hg + row1 * 128 + H + c, v2, v3, ok1);
+            }
+            frag_split(v0, v1, v2, v3, ahi[j], alo[j]);
+        }
+        if constexpr (NF > H) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int c = 8 * j + 2 * q;
+                st2(p.save_sem + row0 * H + c, sem[4 * j] + bb1_s[H + c], sem[4 * j + 1] + bb1_s[H + c + 1], ok0);
+                st2(p.save_sem + row1 * H + c, sem[4 * j + 2] + bb1_s[H + c], sem[4 * j + 3] + bb1_s[H + c + 1], ok1);
             }
         }
-    } else {
-        // ================= epilogue warpgroups: a point's row is its thread's TMEM lane; the two warpgroups of a tile take
-        // the two 32-column halves of every 64-column block (16-column chunks 2 half, 2 half + 1), so a stage's
-        // TMEM -> registers -> TMEM round trip is half as long as with one thread per whole row
-        const int wg = tid >> 8;                 // tile slot
-        const int half = (tid >> 7) & 1;         // column half
-        const int r_in = tid & 127;
-        const int lane = tid & 31;
-#if EMER_CHAIN_STAGE
-        float* stg = p.stg_off ? reinterpret_cast<float*>(smem + p.stg_off + warp * STG_BYTES) : nullptr;
-#else
-        constexpr float* stg = nullptr;
-#endif
-        const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-        const uint32_t a_hi = tmem_base + lane_base + (uint32_t)(wg * 256);
-        const uint32_t a_lo = a_hi + 64u;
-        const uint32_t d_addr = a_hi + 128u;
-        const float* bb0_s = bias_s;
-        const float* bb1_s = bias_s + 64;
-        const float* b2_s = bias_s + 192;
-        uint32_t ph = 0;
 
-        float x_next[K_ENC / 8][8];              // this thread's 8-column chunks of the NEXT tile's enc row (prefetched)
-        auto load_enc = [&](int64_t tile) {
-            const int64_t row = tile * ROWS + r_in;
-            const bool ok = tile < n_tiles && row < p.n;
-            const float* src = p.enc + (ok ? row : 0) * p.ld_enc;
+        // ---- stage 2: [pre-h0 | partial h1] = G [W0g; W1g]^T;  H0 = relu(pre-h0 + ray_bias0)
+        float d0[32], d1[32];
+        wg_fence();
 #pragma unroll
-            for (int c = 0; c < K_ENC / 8; ++c) {
-                if ((c & 1) != half) continue;
-                if (ok) ld8(src + c * 8, x_next[c]);
-                else {
+        for (int ks = 0; ks < 8; ++ks) {
+            mma3<64>(d0, ahi[ks], alo[ks], b_desc(sb + m.wg_hi, 128, ks, 0), b_desc(sb + m.wg_lo, 128, ks, 0), ks > 0);
+            mma3<64>(d1, ahi[ks], alo[ks], b_desc(sb + m.wg_hi, 128, ks, H), b_desc(sb + m.wg_lo, 128, ks, H), ks > 0);
+        }
+        wg_commit();
+        wg_wait0();
+        const float* rb0 = p.ray_bias + ((ok0 ? row0 : p.n - 1) / p.samples) * 128;
+        const float* rb1 = p.ray_bias + ((ok1 ? row1 : p.n - 1) / p.samples) * 128;
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) x_next[c][j] = 0.0f;
-                }
+        for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + 2 * q;
+            const float2 b0 = __ldg(reinterpret_cast<const float2*>(rb0 + c)), b1 = __ldg(reinterpret_cast<const float2*>(rb1 + c));
+            const float v0 = fmaxf(d0[4 * j] + b0.x, 0.0f), v1 = fmaxf(d0[4 * j + 1] + b0.y, 0.0f);
+            const float v2 = fmaxf(d0[4 * j + 2] + b1.x, 0.0f), v3 = fmaxf(d0[4 * j + 3] + b1.y, 0.0f);
+            if (p.save_hg) {
+                st2(p.save_hg + row0 * 128 + c, v0, v1, ok0);
+                st2(p.save_hg + row1 * 128 + c, v2, v3, ok1);
             }
-        };
-        load_enc((int64_t)blockIdx.x * 2 + wg);
+            frag_split(v0, v1, v2, v3, ahi[j], alo[j]);
+        }
 
-        for (int it = 0; it < iters; ++it) {
-            const int64_t tile = ((int64_t)it * gridDim.x + blockIdx.x) * 2 + wg;
-            if (tile >= n_tiles) break;
-            const int64_t row = tile * ROWS + r_in;
-            const bool row_ok = row < p.n;
-            const int64_t ray = (row_ok ? row : (p.n - 1)) / p.samples;
-            const int64_t wrow0 = tile * ROWS + (r_in & ~31);                 // the warp's first row
-            const int rows_valid = (int)(p.n - wrow0 < 32 ? (p.n - wrow0 < 0 ? 0 : p.n - wrow0) : 32);
+        // ---- stage 3: H1 = relu(partial h1 + H0 W1h^T + ray_bias1)
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+            mma3<64>(d1, ahi[ks], alo[ks], b_desc(sb + m.w1h_hi, H, ks, 0), b_desc(sb + m.w1h_lo, H, ks, 0), 1);
+        wg_commit();
+        wg_wait0();
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + 2 * q;
+            const float2 b0 = __ldg(reinterpret_cast<const float2*>(rb0 + H + c));
+            const float2 b1 = __ldg(reinterpret_cast<const float2*>(rb1 + H + c));
+            const float v0 = fmaxf(d1[4 * j] + b0.x, 0.0f), v1 = fmaxf(d1[4 * j + 1] + b0.y, 0.0f);
+            const float v2 = fmaxf(d1[4 * j + 2] + b1.x, 0.0f), v3 = fmaxf(d1[4 * j + 3] + b1.y, 0.0f);
+            if (p.save_h1) {
+                st2(p.save_h1 + row0 * H + c, v0, v1, ok0);
+                st2(p.save_h1 + row1 * H + c, v2, v3, ok1);
+            }
+            frag_split(v0, v1, v2, v3, ahi[j], alo[j]);
+        }
 
-            // ---- stage 0 operand: enc row -> tf32 hi / lo in TMEM
+        // ---- stage 4: rgb = sigmoid(H1 W2^T + b2)   (columns 2q, 2q + 1: quads 0 and 1 hold the three outputs)
+        float d2[4];
+        wg_fence();
 #pragma unroll
-            for (int c = 0; c < K_ENC / 8; ++c) {
-                if ((c & 1) == half) {
-                    uint32_t hi[8], lo[8];
+        for (int ks = 0; ks < 8; ++ks)
+            mma3<8>(d2, ahi[ks], alo[ks], b_desc(sb + m.w2_hi, 8, ks, 0), b_desc(sb + m.w2_lo, 8, ks, 0), ks > 0);
+        wg_commit();
+        wg_wait0();
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float h, l;
-                        split(x_next[c][j], h, l);
-                        hi[j] = __float_as_uint(h);
-                        lo[j] = __float_as_uint(l);
-                    }
-                    tmem_st8(a_hi + (uint32_t)(c * 8), hi);
-                    tmem_st8(a_lo + (uint32_t)(c * 8), lo);
-                }
+        for (int e = 0; e < 2; ++e) {
+            const int c = 2 * q + e;
+            if (c < 3) {
+                if (ok0) p.rgb[row0 * 3 + c] = 1.0f / (1.0f + expf(-(d2[e] + b2_s[c])));
+                if (ok1) p.rgb[row1 * 3 + c] = 1.0f / (1.0f + expf(-(d2[2 + e] + b2_s[c])));
             }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-            load_enc(tile + pair_stride);        // next tile's row: in flight under this tile's five layers
-
-            // ---- stage 1: Hb = relu(D + bb0)
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + (uint32_t)(c * 16), r);
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(__uint_as_float(r[j]) + bb0_s[c * 16 + j], 0.0f);
-                if (p.save_hb) put16(stg, lane, v, p.save_hb + wrow0 * H + c * 16, H, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 2: feats = D + bb1; sigma = exp(feats[0] - 1); geo -> operand; semantic half -> HBM
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + (uint32_t)(c * 16), r);
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]) + bb1_s[c * 16 + j];
-                if (c == 0 && row_ok) p.sigma[row] = expf(v[0] - 1.0f);
-                if (p.save_hg) put16(stg, lane, v, p.save_hg + wrow0 * 128 + H + c * 16, 128, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-            }
-            if (p.n_feat > H) {
-#pragma unroll
-                for (int c = 4 + 2 * half; c < 6 + 2 * half; ++c) {
-                    uint32_t r[16];
-                    tmem_ld16(d_addr + (uint32_t)(c * 16), r);
-                    tmem_ld_wait();
-                    float v[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]) + bb1_s[c * 16 + j];
-                    if (p.save_sem) put16(stg, lane, v, p.save_sem + wrow0 * H + (c - 4) * 16, H, rows_valid);
-                }
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 3: H0 = relu(D[0,64) + ray_bias0)
-            const float* rb = p.ray_bias + ray * 128;
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + (uint32_t)(c * 16), r);
-                float b[16];
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) {
-                    const float4 t = __ldg(reinterpret_cast<const float4*>(rb + c * 16 + j));
-                    b[j] = t.x; b[j + 1] = t.y; b[j + 2] = t.z; b[j + 3] = t.w;
-                }
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(__uint_as_float(r[j]) + b[j], 0.0f);
-                if (p.save_hg) put16(stg, lane, v, p.save_hg + wrow0 * 128 + c * 16, 128, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 4: H1 = relu(D[64,128) + ray_bias1)
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + 64u + (uint32_t)(c * 16), r);
-                float b[16];
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) {
-                    const float4 t = __ldg(reinterpret_cast<const float4*>(rb + 64 + c * 16 + j));
-                    b[j] = t.x; b[j + 1] = t.y; b[j + 2] = t.z; b[j + 3] = t.w;
-                }
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(__uint_as_float(r[j]) + b[j], 0.0f);
-                if (p.save_h1) put16(stg, lane, v, p.save_h1 + wrow0 * H + c * 16, H, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 5: rgb = sigmoid(D[0,3) + b2)
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-            if (half == 0) {
-                uint32_t r[4];
-                tmem_ld4(d_addr, r);
-                tmem_ld_wait();
-                if (row_ok) {
-#pragma unroll
-                    for (int j = 0; j < 3; ++j)
-                        p.rgb[row * 3 + j] = 1.0f / (1.0f + expf(-(__uint_as_float(r[j]) + b2_s[j])));
-                }
-            }
-            tc_fence_before();               // the next tile's operand stores follow these loads in program order
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, 512u);
 }
 
 
 // ------------------------------------------------------------------------------------------------------------------
-// Backward, data path: the gradient walks the same chain, again with every intermediate in tensor memory.
+// Backward, data path: the gradient walks the same chain, again with every intermediate in registers.
 //
 //   dZ2 = d_rgb * rgb (1 - rgb)                                        (registers)
 //   s0  dH1 = dZ2 W2                 A = dZ2 [.. x 8]   B = W2^T   [64 x 8]     dZ1 = dH1 * (h1 > 0)      -> HBM, operand
 //   s1  [dH0 | dG] = dZ1 [W1h | W1g] A = dZ1            B = W1hg^T [128 x 64]   dZ0 = dH0 * (h0 > 0)      -> HBM, operand
 //   s2  dG += dZ0 W0g                A = dZ0            B = W0g^T  [64 x 64]    dF = dG + d_geo, dF[0] += d_sigma * min(sigma, e^15)
 //   s3  dHb = dF Wb1 (+ d_sem Wb1s)  A = dF (, d_sem)   B = Wb1^T  [64 x nf]    dZb = dHb * (hb > 0)      -> HBM, operand
-//   s4  d_enc = dZb Wb0              A = dZb            B = Wb0^T  [k_enc+ x 64]                          -> HBM
+//   s4  d_enc = dZb Wb0              A = dZb            B = Wb0^T  [k_enc x 64]                           -> HBM
 //
-// dZ1, [dZ0 | dF], dZb are written out because the weight gradients (X^T dZ over ALL rows, linear_tc.cu) read them; the
+// dZ1, [dZ0 | dF], dZb are written out because the weight gradients (X^T dZ over ALL rows, wgrad_mn.cu) read them; the
 // per-ray sums of dZ0 / dZ1 -- the gradient of the per-ray bias, i.e. of the direction / embedding columns of the head --
-// are reduced here with warp shuffles (a warp = 32 consecutive samples of one ray) and added to d_ray_bias[R, 128].
+// are reduced here with warp shuffles (a warp's 16 rows are consecutive samples of one ray) and added to d_ray_bias[R, 128].
 struct BwdParams {
     const float *d_rgb, *rgb, *d_sigma, *sigma, *d_geo, *d_sem;      // [N,3] [N,3] [N] [N] [N,64]|null [N,64]|null
     const float *hb, *hg, *h1;                                       // saved activations [N,64] [N,128] [N,64]
@@ -543,381 +311,159 @@ struct BwdParams {
     float *dz2, *dz1, *d1, *dzb, *d_enc; int64_t ld_denc;            // [N,3], [N,64], [N,128] = [dZ0 | dF], [N,64], [N, k_enc]
     float* d_ray_bias; int samples;                                  // [R,128] += ; ray sums only when samples % 32 == 0
     int64_t n;
-    int stg_off;                                                     // staging tiles (see put16), 0 = none
 };
 
 struct BSmem {
-    int w2_hi, w2_lo, w1_hi, w1_lo, w0_hi, w0_lo, wb1_hi, wb1_lo, wb0_hi, wb0_lo, bars, total;
+    int w2_hi, w2_lo, w1_hi, w1_lo, w0_hi, w0_lo, wb1_hi, wb1_lo, wb0_hi, wb0_lo, total;
 };
 __host__ __device__ inline BSmem bsmem_map(int k_enc, int n_feat) {
     BSmem m;
     int o = 0;
-    const int kpad = (k_enc + 15) / 16 * 16;                         // N of the last product: a multiple of 16
     const int w2 = (8 / 4) * H * 16, w1 = (H / 4) * 128 * 16, w0 = (H / 4) * H * 16, wb1 = (n_feat / 4) * H * 16,
-              wb0 = (H / 4) * kpad * 16;
+              wb0 = (H / 4) * k_enc * 16;
     m.w2_hi = o; o += w2; m.w2_lo = o; o += w2;
     m.w1_hi = o; o += w1; m.w1_lo = o; o += w1;
     m.w0_hi = o; o += w0; m.w0_lo = o; o += w0;
     m.wb1_hi = o; o += wb1; m.wb1_lo = o; o += wb1;
     m.wb0_hi = o; o += wb0; m.wb0_lo = o; o += wb0;
-    m.bars = o; o += 8 * 8;
     m.total = o;
     return m;
 }
 
-// B = W^T for a data gradient: operand row j (input feature), reduction index o (output feature): element w[o, j]
-__device__ __forceinline__ void stage_weight_t(uint8_t* hi, uint8_t* lo, const float* __restrict__ w, int64_t ld, int rows,
-                                               int rows_valid, int kpad, int k_valid, int row0, int k0, int tid,
-                                               int nthreads) {
-    const int panel = rows * 16;
-    for (int e = tid; e < rows_valid * k_valid; e += nthreads) {
-        const int o = e / rows_valid, j = e - o * rows_valid;        // consecutive threads: consecutive j (coalesced)
-        float h, l;
-        split(__ldg(w + (int64_t)o * ld + j), h, l);
-        const int k = k0 + o;
-        const int off = (k >> 2) * panel + (row0 + j) * 16 + (k & 3) * 4;
-        *reinterpret_cast<float*>(hi + off) = h;
-        *reinterpret_cast<float*>(lo + off) = l;
-    }
-    (void)kpad;
-}
-
-// Column sums over the 32 lanes of a warp of v[16] (recursive halving: 15 + 1 shuffles).  Afterwards every lane holds the
-// total of ONE column: col = 8 b4 + 4 b3 + 2 b2 + b1 of its lane index (lanes l and l ^ 1 hold the same column).
-__device__ __forceinline__ float warp_colsum16(const float (&v)[16], int lane, int& col) {
-    float a[8];
-    const bool b4 = lane & 16;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const float send = b4 ? v[j] : v[j + 8];
-        const float keep = b4 ? v[j + 8] : v[j];
-        a[j] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-    float b[4];
-    const bool b3 = lane & 8;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const float send = b3 ? a[j] : a[j + 4];
-        const float keep = b3 ? a[j + 4] : a[j];
-        b[j] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-    }
-    float c[2];
-    const bool b2 = lane & 4;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        const float send = b2 ? b[j] : b[j + 2];
-        const float keep = b2 ? b[j + 2] : b[j];
-        c[j] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-    }
-    const bool b1 = lane & 2;
-    float d = (b1 ? c[1] : c[0]) + __shfl_xor_sync(0xffffffffu, b1 ? c[0] : c[1], 2);
-    d += __shfl_xor_sync(0xffffffffu, d, 1);
-    col = (b4 ? 8 : 0) + (b3 ? 4 : 0) + (b2 ? 2 : 0) + (b1 ? 1 : 0);
-    return d;
-}
-
-template <int K_ENC>
+template <int K_ENC, int NF>
 __global__ void __launch_bounds__(THREADS, 1) field_bwd_kernel(const BwdParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
-    constexpr int KPAD = (K_ENC + 15) / 16 * 16;
-    const BSmem m = bsmem_map(K_ENC, p.n_feat);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + m.bars);
-    uint64_t* a_full = bars;
-    uint64_t* d_full = bars + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-
+    const BSmem m = bsmem_map(K_ENC, NF);
     const int tid = threadIdx.x;
-    const int warp = tid >> 5;
-    const int lane = tid & 31;
-    const bool is_issuer = warp == EPI_THREADS / 32;
-
-    if (tid == 0) {
-        mbar_init(&a_full[0], arrivals(TILE_THREADS));
-        mbar_init(&a_full[1], arrivals(TILE_THREADS));
-        mbar_init(&d_full[0], 1);
-        mbar_init(&d_full[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        __syncwarp();
-        tmem_alloc(tmem_slot, 512u);
-    }
-    for (int i = tid * 16; i < m.bars; i += THREADS * 16) *reinterpret_cast<float4*>(smem + i) = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = tid * 16; i < m.total; i += THREADS * 16) *reinterpret_cast<float4*>(smem + i) = make_float4(0.f, 0.f, 0.f, 0.f);
     __syncthreads();
-    stage_weight_t(smem + m.w2_hi, smem + m.w2_lo, p.w2, H, H, H, 8, 3, 0, 0, tid, THREADS);                 // [64 x 8]
-    stage_weight_t(smem + m.w1_hi, smem + m.w1_lo, p.w1h, p.ld_w1, 128, H, H, H, 0, 0, tid, THREADS);       // rows 0..63
-    stage_weight_t(smem + m.w1_hi, smem + m.w1_lo, p.w1g, p.ld_w1, 128, H, H, H, H, 0, tid, THREADS);       // rows 64..127
-    stage_weight_t(smem + m.w0_hi, smem + m.w0_lo, p.w0g, p.ld_w0, H, H, H, H, 0, 0, tid, THREADS);
-    stage_weight_t(smem + m.wb1_hi, smem + m.wb1_lo, p.wb1, H, H, H, p.n_feat, p.n_feat, 0, 0, tid, THREADS);  // [64 x nf]
-    stage_weight_t(smem + m.wb0_hi, smem + m.wb0_lo, p.wb0, K_ENC, KPAD, K_ENC, H, H, 0, 0, tid, THREADS);  // [kpad x 64]
+    stage_weight_t(smem + m.w2_hi, smem + m.w2_lo, p.w2, H, H, H, 3, 0, tid);                  // [64 x 8]
+    stage_weight_t(smem + m.w1_hi, smem + m.w1_lo, p.w1h, p.ld_w1, 128, H, H, 0, tid);         // rows 0..63
+    stage_weight_t(smem + m.w1_hi, smem + m.w1_lo, p.w1g, p.ld_w1, 128, H, H, H, tid);         // rows 64..127
+    stage_weight_t(smem + m.w0_hi, smem + m.w0_lo, p.w0g, p.ld_w0, H, H, H, 0, tid);
+    stage_weight_t(smem + m.wb1_hi, smem + m.wb1_lo, p.wb1, H, H, H, NF, 0, tid);               // [64 x nf]
+    stage_weight_t(smem + m.wb0_hi, smem + m.wb0_lo, p.wb0, K_ENC, K_ENC, K_ENC, H, 0, tid);    // [k_enc x 64]
     fence_async_proxy();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
+    const uint32_t sb = smem_u32(smem);
+    const int wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+    const bool ray_sums = p.d_ray_bias != nullptr && (p.samples % 32 == 0);
     const int64_t n_tiles = (p.n + ROWS - 1) / ROWS;
-    const int64_t pair_stride = (int64_t)gridDim.x * 2;
-    const int iters = (int)((n_tiles + pair_stride - 1) / pair_stride);
-    const int n_stages = p.n_feat > H ? 6 : 5;           // (with a semantic half, stage 3 takes its operand in two pieces)
 
-    if (is_issuer) {
-        const uint32_t sbase = smem_u32(smem);
-        const uint64_t d64 = make_desc(0, H * 16, 128), d128 = make_desc(0, 128 * 16, 128), dkp = make_desc(0, KPAD * 16, 128);
-        const uint32_t id64 = make_idesc(128, 64), id128 = make_idesc(128, 128), idkp = make_idesc(128, KPAD);
-        uint32_t ph[2] = {0, 0};
-        for (int it = 0; it < iters; ++it) {
-            for (int st = 0; st < n_stages; ++st) {
-                // stage ids: 0 dZ2 W2 | 1 dZ1 W1hg | 2 dZ0 W0g | 3 dF Wb1 | (5: d_sem Wb1[:, 64:]) | 4 dZb Wb0
-                const int stage = (n_stages == 6) ? (st < 4 ? st : (st == 4 ? 5 : 4)) : st;
-                for (int wg = 0; wg < 2; ++wg) {
-                    const int64_t tile = ((int64_t)it * gridDim.x + blockIdx.x) * 2 + wg;
-                    if (tile >= n_tiles) continue;
-                    mbar_wait(&a_full[wg], ph[wg]);
-                    ph[wg] ^= 1u;
-                    tc_fence_after();
-                    if (mma_issue_lane(tid)) {
-                        const uint32_t a_hi = tmem_base + (uint32_t)(wg * 256);
-                        const uint32_t a_lo = a_hi + 64u;
-                        uint32_t d = a_hi + 128u;
-                        uint64_t desc = d64;
-                        uint32_t idesc = id64, b_hi, b_lo, panel = H * 16, acc0 = 0u, koff = 0u;
-                        int ksteps = H / 8;
-                        if (stage == 0) { b_hi = m.w2_hi; b_lo = m.w2_lo; ksteps = 1; }
-                        else if (stage == 1) { desc = d128; idesc = id128; b_hi = m.w1_hi; b_lo = m.w1_lo; panel = 128 * 16; }
-                        else if (stage == 2) { b_hi = m.w0_hi; b_lo = m.w0_lo; d += 64u; acc0 = 1u; }
-                        else if (stage == 3) { b_hi = m.wb1_hi; b_lo = m.wb1_lo; }
-                        else if (stage == 5) { b_hi = m.wb1_hi; b_lo = m.wb1_lo; acc0 = 1u; koff = (uint32_t)(16 * panel) >> 4; }
-                        else { desc = dkp; idesc = idkp; b_hi = m.wb0_hi; b_lo = m.wb0_lo; panel = KPAD * 16; }
-                        const uint32_t bh = ((sbase + b_hi) >> 4) + koff, bl = ((sbase + b_lo) >> 4) + koff;
-                        for (int ks = 0; ks < ksteps; ++ks) {
-                            const uint32_t bo = (uint32_t)(ks * 2 * panel) >> 4;
-                            const uint64_t db_hi = desc | (uint64_t)(bh + bo), db_lo = desc | (uint64_t)(bl + bo);
-                            const uint32_t ah = a_hi + (uint32_t)(ks * 8), al = a_lo + (uint32_t)(ks * 8);
-                            mma_tf32_ts(d, ah, db_hi, idesc, (ks > 0) ? 1u : acc0);
-                            mma_tf32_ts(d, al, db_hi, idesc, 1u);
-                            mma_tf32_ts(d, ah, db_lo, idesc, 1u);
-                        }
-                        tc_commit(&d_full[wg]);
-                    }
-                    __syncwarp();
+    for (int64_t tile = (int64_t)blockIdx.x * WGS + wg; tile < n_tiles; tile += (int64_t)gridDim.x * WGS) {
+        const int64_t wrow0 = tile * ROWS + 16 * w;                     // the warp's first row
+        const int64_t row0 = wrow0 + (lane >> 2), row1 = row0 + 8;
+        const bool ok0 = row0 < p.n, ok1 = row1 < p.n;
+        // the warp's 16 rows belong to one ray (samples % 32 == 0); rows past the end contribute zeros
+        const bool warp_live = wrow0 < p.n;
+        float* rbias = ray_sums ? p.d_ray_bias + (wrow0 / p.samples) * 128 : nullptr;
+        uint32_t ahi[8][4], alo[8][4];
+
+        // ---- stage 0 operand: dZ2 = d_rgb * rgb (1 - rgb), columns 2q, 2q + 1 of one 8-wide k step
+        {
+            float v[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int c = 2 * q + (e & 1);
+                const int64_t row = (e < 2) ? row0 : row1;
+                if (c < 3 && (e < 2 ? ok0 : ok1) && p.d_rgb) {
+                    const float y = __ldg(p.rgb + row * 3 + c);
+                    v[e] = __ldg(p.d_rgb + row * 3 + c) * (y * (1.0f - y));
+                    if (p.dz2) p.dz2[row * 3 + c] = v[e];
                 }
+            }
+            frag_split(v[0], v[1], v[2], v[3], ahi[0], alo[0]);
+        }
+        float acc[32];
+        wg_fence();
+        mma3<64>(acc, ahi[0], alo[0], b_desc(sb + m.w2_hi, H, 0, 0), b_desc(sb + m.w2_lo, H, 0, 0), 0);
+        wg_commit();
+        wg_wait0();
+
+        // ---- stage 0 result: dZ1 = dH1 * (h1 > 0)
+        relu_back(acc, p.h1, p.dz1, H, row0, row1, ok0, ok1, q, ahi, alo);
+        if (ray_sums) ray_colsum(acc, rbias + H, lane, warp_live);
+
+        // ---- stage 1: [dH0 | dG] = dZ1 [W1h | W1g];  dZ0 = dH0 * (h0 > 0)   (dG stays in its accumulator)
+        float dg[32];
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks) {
+            mma3<64>(acc, ahi[ks], alo[ks], b_desc(sb + m.w1_hi, 128, ks, 0), b_desc(sb + m.w1_lo, 128, ks, 0), ks > 0);
+            mma3<64>(dg, ahi[ks], alo[ks], b_desc(sb + m.w1_hi, 128, ks, H), b_desc(sb + m.w1_lo, 128, ks, H), ks > 0);
+        }
+        wg_commit();
+        wg_wait0();
+        relu_back(acc, p.hg, p.d1, 128, row0, row1, ok0, ok1, q, ahi, alo);
+        if (ray_sums) ray_colsum(acc, rbias, lane, warp_live);
+
+        // ---- stage 2: dG += dZ0 W0g;  dF = dG (+ d_geo); dF[0] += d_sigma * exp(min(x, 15)), exp(x) = sigma (nerf_utils.py:72-75)
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+            mma3<64>(dg, ahi[ks], alo[ks], b_desc(sb + m.w0_hi, H, ks, 0), b_desc(sb + m.w0_lo, H, ks, 0), 1);
+        wg_commit();
+        wg_wait0();
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + 2 * q;
+            float v0 = dg[4 * j], v1 = dg[4 * j + 1], v2 = dg[4 * j + 2], v3 = dg[4 * j + 3];
+            if (p.d_geo) {
+                const float2 g0 = ld2(p.d_geo + row0 * H + c, ok0), g1 = ld2(p.d_geo + row1 * H + c, ok1);
+                v0 += g0.x; v1 += g0.y; v2 += g1.x; v3 += g1.y;
+            }
+            if (j == 0 && q == 0 && p.d_sigma) {
+                if (ok0) v0 += __ldg(p.d_sigma + row0) * fminf(__ldg(p.sigma + row0), 3269017.25f);
+                if (ok1) v2 += __ldg(p.d_sigma + row1) * fminf(__ldg(p.sigma + row1), 3269017.25f);
+            }
+            st2(p.d1 + row0 * 128 + H + c, v0, v1, ok0);
+            st2(p.d1 + row1 * 128 + H + c, v2, v3, ok1);
+            frag_split(v0, v1, v2, v3, ahi[j], alo[j]);
+        }
+
+        // ---- stage 3: dHb = dF Wb1[:64] (+ d_sem Wb1[64:]);  dZb = dHb * (hb > 0)
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+            mma3<64>(acc, ahi[ks], alo[ks], b_desc(sb + m.wb1_hi, H, ks, 0), b_desc(sb + m.wb1_lo, H, ks, 0), ks > 0);
+        wg_commit();
+        wg_wait0();
+        if constexpr (NF > H) {
+            if (p.d_sem) {                           // the second operand piece: the gradient of the semantic half
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int c = 8 * j + 2 * q;
+                    const float2 s0 = ld2(p.d_sem + row0 * H + c, ok0), s1 = ld2(p.d_sem + row1 * H + c, ok1);
+                    frag_split(s0.x, s0.y, s1.x, s1.y, ahi[j], alo[j]);
+                }
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < 8; ++ks)
+                    mma3<64>(acc, ahi[ks], alo[ks], b_desc(sb + m.wb1_hi, H, 8 + ks, 0), b_desc(sb + m.wb1_lo, H, 8 + ks, 0), 1);
+                wg_commit();
+                wg_wait0();
             }
         }
-    } else {
-        const int wg = tid >> 8;                 // tile slot
-        const int half = (tid >> 7) & 1;         // column half (see field_fwd_kernel)
-        const int r_in = tid & 127;
-        const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-        const uint32_t a_hi = tmem_base + lane_base + (uint32_t)(wg * 256);
-        const uint32_t a_lo = a_hi + 64u;
-        const uint32_t d_addr = a_hi + 128u;
-        const bool ray_sums = p.d_ray_bias != nullptr && (p.samples % 32 == 0);
-#if EMER_CHAIN_STAGE
-        float* stg = p.stg_off ? reinterpret_cast<float*>(smem + p.stg_off + warp * STG_BYTES) : nullptr;
-#else
-        constexpr float* stg = nullptr;
-#endif
-        uint32_t ph = 0;
+        relu_back(acc, p.hb, p.dzb, H, row0, row1, ok0, ok1, q, ahi, alo);
 
-        for (int it = 0; it < iters; ++it) {
-            const int64_t tile = ((int64_t)it * gridDim.x + blockIdx.x) * 2 + wg;
-            if (tile >= n_tiles) break;
-            const int64_t row = tile * ROWS + r_in;
-            const bool row_ok = row < p.n;
-            const int64_t wrow0 = tile * ROWS + (r_in & ~31);                 // the warp's first row
-            const int rows_valid = (int)(p.n - wrow0 < 32 ? (p.n - wrow0 < 0 ? 0 : p.n - wrow0) : 32);
-            // the warp's 32 rows belong to one ray (samples % 32 == 0); rows past the end contribute zeros
-            const int64_t ray = wrow0 / p.samples;
-            const bool warp_live = wrow0 < p.n;
-
-            // ---- stage 0 operand: dZ2 = d_rgb * rgb (1 - rgb), 3 columns of an 8-wide k step (written by half 0)
-            if (half == 0) {
-                uint32_t hi[8], lo[8];
+        // ---- stage 4: d_enc = dZb Wb0
+        if (p.d_enc) {
+            float de[K_ENC / 2];
+            wg_fence();
 #pragma unroll
-                for (int j = 0; j < 8; ++j) hi[j] = lo[j] = 0u;
-                if (row_ok && p.d_rgb) {
+            for (int ks = 0; ks < 8; ++ks)
+                mma3<K_ENC>(de, ahi[ks], alo[ks], b_desc(sb + m.wb0_hi, K_ENC, ks, 0), b_desc(sb + m.wb0_lo, K_ENC, ks, 0), ks > 0);
+            wg_commit();
+            wg_wait0();
 #pragma unroll
-                    for (int j = 0; j < 3; ++j) {
-                        const float y = __ldg(p.rgb + row * 3 + j);
-                        const float g = __ldg(p.d_rgb + row * 3 + j) * (y * (1.0f - y));
-                        if (p.dz2) p.dz2[row * 3 + j] = g;
-                        float h, l;
-                        split(g, h, l);
-                        hi[j] = __float_as_uint(h);
-                        lo[j] = __float_as_uint(l);
-                    }
-                }
-                tmem_st8(a_hi, hi);
-                tmem_st8(a_lo, lo);
+            for (int j = 0; j < K_ENC / 8; ++j) {
+                const int c = 8 * j + 2 * q;
+                st2(p.d_enc + row0 * p.ld_denc + c, de[4 * j], de[4 * j + 1], ok0);
+                st2(p.d_enc + row1 * p.ld_denc + c, de[4 * j + 2], de[4 * j + 3], ok1);
             }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 0 result: dZ1 = dH1 * (h1 > 0)
-            uint32_t mask = get_mask32(stg, lane, p.h1 + wrow0 * H + half * 32, H, rows_valid);   // columns 32 half .. 32 half + 31
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + (uint32_t)(c * 16), r);
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = ((mask >> ((c & 1) * 16 + j)) & 1u) ? __uint_as_float(r[j]) : 0.0f;
-                put16(stg, lane, v, p.dz1 + wrow0 * H + c * 16, H, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-                if (ray_sums) {
-                    int col;
-                    const float sum = warp_colsum16(v, lane, col);
-                    if (!(lane & 1) && warp_live) atomicAdd(p.d_ray_bias + ray * 128 + H + c * 16 + col, sum);
-                }
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 1 result: dZ0 = dH0 * (h0 > 0)   (dG stays in the accumulator's upper half)
-            mask = get_mask32(stg, lane, p.hg + wrow0 * 128 + half * 32, 128, rows_valid);
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + (uint32_t)(c * 16), r);
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = ((mask >> ((c & 1) * 16 + j)) & 1u) ? __uint_as_float(r[j]) : 0.0f;
-                put16(stg, lane, v, p.d1 + wrow0 * 128 + c * 16, 128, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-                if (ray_sums) {
-                    int col;
-                    const float sum = warp_colsum16(v, lane, col);
-                    if (!(lane & 1) && warp_live) atomicAdd(p.d_ray_bias + ray * 128 + c * 16 + col, sum);
-                }
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 2 result: dF = dG (+ d_geo); dF[0] += d_sigma * exp(min(x, 15)), exp(x) = sigma (nerf_utils.py:72-75)
-            float ds = 0.0f;
-            if (row_ok && p.d_sigma) ds = __ldg(p.d_sigma + row) * fminf(__ldg(p.sigma + row), 3269017.25f);
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + 64u + (uint32_t)(c * 16), r);
-                float g[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) g[j] = 0.0f;
-                if (p.d_geo && row_ok) {
-#pragma unroll
-                    for (int j = 0; j < 16; j += 4) {
-                        const float4 t = __ldg(reinterpret_cast<const float4*>(p.d_geo + row * H + c * 16 + j));
-                        g[j] = t.x; g[j + 1] = t.y; g[j + 2] = t.z; g[j + 3] = t.w;
-                    }
-                }
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]) + g[j];
-                if (c == 0) v[0] += ds;
-                put16(stg, lane, v, p.d1 + wrow0 * 128 + H + c * 16, 128, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            if (p.n_feat > H) {
-                // ---- second operand piece of stage 3: the gradient of the semantic half
-                mbar_wait(&d_full[wg], ph); ph ^= 1u;           // (the first piece's MMAs have read the operand)
-                tc_fence_after();
-#pragma unroll
-                for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                    float v[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] = 0.0f;
-                    if (p.d_sem && row_ok) {
-#pragma unroll
-                        for (int j = 0; j < 16; j += 4) {
-                            const float4 t = __ldg(reinterpret_cast<const float4*>(p.d_sem + row * H + c * 16 + j));
-                            v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
-                        }
-                    }
-                    uint32_t hi[16], lo[16];
-                    split16(v, hi, lo);
-                    tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                    tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-                }
-                tmem_st_wait();
-                tc_fence_before();
-                mbar_arrive_warp(&a_full[wg]);
-            }
-
-            // ---- stage 3 result: dZb = dHb * (hb > 0)
-            mask = get_mask32(stg, lane, p.hb + wrow0 * H + half * 32, H, rows_valid);
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-#pragma unroll
-            for (int c = 2 * half; c < 2 * half + 2; ++c) {
-                uint32_t r[16];
-                tmem_ld16(d_addr + (uint32_t)(c * 16), r);
-                tmem_ld_wait();
-                float v[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = ((mask >> ((c & 1) * 16 + j)) & 1u) ? __uint_as_float(r[j]) : 0.0f;
-                put16(stg, lane, v, p.dzb + wrow0 * H + c * 16, H, rows_valid);
-                uint32_t hi[16], lo[16];
-                split16(v, hi, lo);
-                tmem_st16(a_hi + (uint32_t)(c * 16), hi);
-                tmem_st16(a_lo + (uint32_t)(c * 16), lo);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive_warp(&a_full[wg]);
-
-            // ---- stage 4 result: d_enc
-            mbar_wait(&d_full[wg], ph); ph ^= 1u;
-            tc_fence_after();
-            if (p.d_enc) {
-                // half 0 takes the first ceil(nc / 2) 8-column chunks, half 1 the rest (contiguous ranges per thread)
-                constexpr int NC = K_ENC / 8, C_SPLIT = (NC + 1) / 2;
-#pragma unroll
-                for (int c = 0; c < NC; ++c) {
-                    if ((c < C_SPLIT) != (half == 0)) continue;
-                    uint32_t r[8];
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                                 : "r"(d_addr + (uint32_t)(c * 8))
-                                 : "memory");
-                    tmem_ld_wait();
-                    float v[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(r[j]);
-                    put8(stg, lane, v, p.d_enc + wrow0 * p.ld_denc + c * 8, p.ld_denc, rows_valid);
-                }
-            }
-            tc_fence_before();
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, 512u);
 }
 
 }  // namespace ff
@@ -937,7 +483,7 @@ extern "C" int emer_field_fwd(const float* enc, int64_t ld_enc, int k_enc, const
     EMER_REQUIRE(k_enc == 32 || k_enc == 40 || k_enc == 64, "emer_field_fwd: k_enc=%d (L*F of the grid) must be 32, 40 or 64", k_enc);
     EMER_REQUIRE(n_feat == 64 || n_feat == 128, "emer_field_fwd: n_feat=%d must be 64 or 128", n_feat);
     EMER_REQUIRE(samples > 0, "emer_field_fwd: samples per ray must be positive");
-    EMER_REQUIRE(ld_enc % 8 == 0 && ((uintptr_t)enc & 31) == 0, "emer_field_fwd: enc rows must be 32-byte aligned (256-bit row loads)");
+    EMER_REQUIRE(ld_enc % 8 == 0 && ((uintptr_t)enc & 31) == 0, "emer_field_fwd: enc rows must be 32-byte aligned");
     EMER_REQUIRE(((uintptr_t)ray_bias & 15) == 0, "emer_field_fwd: ray_bias must be 16-byte aligned");
     EMER_REQUIRE((((uintptr_t)save_hb | (uintptr_t)save_hg | (uintptr_t)save_h1 | (uintptr_t)save_sem) & 31) == 0,
                  "emer_field_fwd: save buffers must be 32-byte aligned");
@@ -950,15 +496,9 @@ extern "C" int emer_field_fwd(const float* enc, int64_t ld_enc, int k_enc, const
     const Smem m = smem_map(k_enc, n_feat);
     size_t smem = (size_t)m.total;
     EMER_REQUIRE(smem <= 227 * 1024, "emer_field_fwd: %zu B of shared memory needed", smem);
-#if EMER_CHAIN_STAGE
-    {   // staging tiles for coalesced row stores, when they fit beside the weights (n_feat = 64: 157 + 40 KB)
-        const size_t off = (smem + 127) / 128 * 128;
-        if (off + STG_TOTAL <= 227 * 1024) { p.stg_off = (int)off; smem = off + STG_TOTAL; }
-    }
-#endif
     const int64_t n_tiles = ceil_div(n, ROWS);
     int64_t grid = sm_count();
-    if (grid > ceil_div(n_tiles, 2)) grid = ceil_div(n_tiles, 2);
+    if (grid > ceil_div(n_tiles, WGS)) grid = ceil_div(n_tiles, WGS);
     auto launch = [&](auto kernel, size_t& configured) -> int {
         if (smem > configured) {
             cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -971,12 +511,18 @@ extern "C" int emer_field_fwd(const float* enc, int64_t ld_enc, int k_enc, const
         kernel<<<(unsigned)grid, THREADS, smem, (cudaStream_t)stream>>>(p);
         return 0;
     };
-    static size_t configured_dev[3][64] = {{0}};          // the attribute is per kernel and per device
+    static size_t configured_dev[6][64] = {{0}};          // the attribute is per kernel and per device
     const int dev = current_device();
     int rc;
-    if (k_enc == 32) rc = launch(field_fwd_kernel<32>, configured_dev[0][dev]);
-    else if (k_enc == 40) rc = launch(field_fwd_kernel<40>, configured_dev[1][dev]);
-    else rc = launch(field_fwd_kernel<64>, configured_dev[2][dev]);
+    if (n_feat == 64) {
+        if (k_enc == 32) rc = launch(field_fwd_kernel<32, 64>, configured_dev[0][dev]);
+        else if (k_enc == 40) rc = launch(field_fwd_kernel<40, 64>, configured_dev[1][dev]);
+        else rc = launch(field_fwd_kernel<64, 64>, configured_dev[2][dev]);
+    } else {
+        if (k_enc == 32) rc = launch(field_fwd_kernel<32, 128>, configured_dev[3][dev]);
+        else if (k_enc == 40) rc = launch(field_fwd_kernel<40, 128>, configured_dev[4][dev]);
+        else rc = launch(field_fwd_kernel<64, 128>, configured_dev[5][dev]);
+    }
     if (rc) return rc;
     return check_launch("emer_field_fwd");
 }
@@ -997,7 +543,7 @@ extern "C" int emer_field_bwd(const float* d_rgb, const float* rgb, const float*
     EMER_REQUIRE(!d_enc || (ld_denc % 8 == 0 && ld_denc >= k_enc), "emer_field_bwd: d_enc rows must be 32-byte aligned");
     EMER_REQUIRE((((uintptr_t)hb | (uintptr_t)hg | (uintptr_t)h1 | (uintptr_t)dz1 | (uintptr_t)d1 | (uintptr_t)dzb |
                    (uintptr_t)d_enc | (uintptr_t)d_geo | (uintptr_t)d_sem) & 31) == 0,
-                 "emer_field_bwd: row buffers must be 32-byte aligned (256-bit row accesses)");
+                 "emer_field_bwd: row buffers must be 32-byte aligned");
     EMER_REQUIRE(!d_ray_bias || samples % 32 == 0, "emer_field_bwd: per-ray sums need samples %% 32 == 0 (got %d)", samples);
     BwdParams p{};
     p.d_rgb = d_rgb; p.rgb = rgb; p.d_sigma = d_sigma; p.sigma = sigma; p.d_geo = d_geo; p.d_sem = d_sem;
@@ -1008,15 +554,9 @@ extern "C" int emer_field_bwd(const float* d_rgb, const float* rgb, const float*
     const BSmem m = bsmem_map(k_enc, n_feat);
     size_t smem = (size_t)m.total;
     EMER_REQUIRE(smem <= 227 * 1024, "emer_field_bwd: %zu B of shared memory needed", smem);
-#if EMER_CHAIN_STAGE
-    {
-        const size_t off = (smem + 127) / 128 * 128;
-        if (off + STG_TOTAL <= 227 * 1024) { p.stg_off = (int)off; smem = off + STG_TOTAL; }
-    }
-#endif
     const int64_t n_tiles = ceil_div(n, ROWS);
     int64_t grid = sm_count();
-    if (grid > ceil_div(n_tiles, 2)) grid = ceil_div(n_tiles, 2);
+    if (grid > ceil_div(n_tiles, WGS)) grid = ceil_div(n_tiles, WGS);
     auto launch = [&](auto kernel, size_t& configured) -> int {
         if (smem > configured) {
             cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1029,12 +569,18 @@ extern "C" int emer_field_bwd(const float* d_rgb, const float* rgb, const float*
         kernel<<<(unsigned)grid, THREADS, smem, (cudaStream_t)stream>>>(p);
         return 0;
     };
-    static size_t configured_dev[3][64] = {{0}};
+    static size_t configured_dev[6][64] = {{0}};          // the attribute is per kernel and per device
     const int dev = current_device();
     int rc;
-    if (k_enc == 32) rc = launch(field_bwd_kernel<32>, configured_dev[0][dev]);
-    else if (k_enc == 40) rc = launch(field_bwd_kernel<40>, configured_dev[1][dev]);
-    else rc = launch(field_bwd_kernel<64>, configured_dev[2][dev]);
+    if (n_feat == 64) {
+        if (k_enc == 32) rc = launch(field_bwd_kernel<32, 64>, configured_dev[0][dev]);
+        else if (k_enc == 40) rc = launch(field_bwd_kernel<40, 64>, configured_dev[1][dev]);
+        else rc = launch(field_bwd_kernel<64, 64>, configured_dev[2][dev]);
+    } else {
+        if (k_enc == 32) rc = launch(field_bwd_kernel<32, 128>, configured_dev[3][dev]);
+        else if (k_enc == 40) rc = launch(field_bwd_kernel<40, 128>, configured_dev[4][dev]);
+        else rc = launch(field_bwd_kernel<64, 128>, configured_dev[5][dev]);
+    }
     if (rc) return rc;
     return check_launch("emer_field_bwd");
 }

@@ -1,4 +1,4 @@
-// Multi-resolution hash-grid encoding for sm_100a: forward gather, backward scatter (+ input
+// Multi-resolution hash-grid encoding for sm_90a: forward gather, backward scatter (+ input
 // gradient).  Replaces tiny-cuda-nn's GridEncoding as reached through
 // third_party/tcnn_modules.py:122 (fwd) and :161 (bwd) of the reference.
 //
@@ -198,8 +198,7 @@ __global__ void grid_indices_kernel(const GridDescDev gd, const float* __restric
 // (red.global.add.v4.f32 for F=4: one 16-byte L2 atomic per corner); dx is summed in registers.
 //
 // Ray-coherent batches put consecutive samples of a ray in consecutive lanes, and at the coarse
-// levels those samples share a cell: measured on B200, the level-0 scatter of the 10x4 static grid
-// cost 945 us against 24 us for incoherent points (same-address L2 reductions serialise).  So each
+// levels those samples share a cell, and same-address L2 reductions serialise.  So each
 // warp first looks for runs of adjacent lanes in the SAME cell; where there are any, the 2^D*F
 // partial sums of a run are combined with a segmented shuffle reduction and only the run's first
 // lane issues the reductions.

@@ -4,7 +4,7 @@
 // (radiance_fields/mlp.py:38-46, radiance_fields/radiance_field.py:74-198,808-812).  The layers
 // are skinny: N = rays*samples rows (524 288 at 8192x64), inner/outer widths <= 192.  This file is
 // the bit-faithful fp32 implementation (FFMA, fp32 accumulate, same rounding class as the fp32
-// SGEMM of the reference) and the checker for the tcgen05 path in mlp_tc.cu.
+// SGEMM of the reference) and the checker for the tensor-core path in linear_tc.cu.
 //
 //   emer_linear_fwd        Y  = act(X W^T + b)          [N,k] x [n_out,k] -> [N,n_out]
 //   emer_linear_bwd_data   dX (=|+=) (dY*act'(Y)) W     [N,n_out] x [n_out,k] -> [N,k]
@@ -357,8 +357,8 @@ __global__ void __launch_bounds__(256) narrow_wgrad_kernel(const float* __restri
 #pragma unroll
     for (int o = 0; o < NARROW_MAX_OUT; ++o) acc[o] = bacc[o] = 0.0f;
     if (rl < lanes) {
-        // four rows per trip: the loads of a trip are independent, so four row fetches are in flight per thread (the
-        // one-row loop was latency-bound: 0.10 ms for 64 -> 3 over 524 288 rows against 0.02 ms of HBM time)
+        // four rows per trip: the loads of a trip are independent, so four row fetches are in flight per thread (a
+        // one-row loop is latency-bound on these shapes)
         constexpr int U = 4;
         for (int64_t row = r0 + rl; row < r1; row += (int64_t)lanes * U) {
             float xv[U], g[U][NARROW_MAX_OUT];
@@ -406,8 +406,7 @@ __global__ void __launch_bounds__(256) narrow_wgrad_kernel(const float* __restri
 
 // The same product for the shapes the field produces (k % 4 == 0, rows of X and dZ 16-byte aligned, n_out <= 4): a
 // thread owns FOUR columns and reads X and dZ rows as 16-byte vectors -- per 4 x 4 elements 2 loads + 16 FMAs instead of
-// 4 x (1 + n_out) loads + 4 x 8 FMAs; the scalar kernel was instruction-bound at 129 us for 64 -> 3 over 524 288 rows
-// (21 us of HBM time).
+// 4 x (1 + n_out) loads + 4 x 8 FMAs (the scalar kernel is instruction-bound on these shapes, far from the HBM time).
 template <int U, bool DZ_VEC>
 __global__ void __launch_bounds__(256) narrow_wgrad_vec4_kernel(const float* __restrict__ x, int64_t ldx,
                                                                 const float* __restrict__ dz, int64_t lddz,

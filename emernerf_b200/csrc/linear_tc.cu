@@ -1,49 +1,24 @@
-// Dense layers of the MLP heads on the 5th-generation tensor cores (tcgen05 + TMEM), fp32-accurate.
+// Dense layers of the MLP heads on Hopper warpgroup MMA (wgmma), fp32-accurate.
 //
-// The reference runs every head as fp32 nn.Linear (SURVEY.md F5), so a single-pass TF32 MMA
-// (10-bit mantissa) is not accurate enough for the 1e-4 parity bar.  Each fp32 operand is split
-// into tf32 hi + tf32 lo (x = hi + lo to ~2^-21) and a product is accumulated in TMEM as
-//     A_hi*B_hi  +  (A_lo*B_hi + A_hi*B_lo)          ("3xTF32", error ~1e-6 relative)
-// by three tcgen05.mma.kind::tf32 per 8-wide k step, into two independent TMEM accumulators
-// (two dependency chains for the tensor pipe) that the epilogue adds.
+// The reference runs every head as fp32 nn.Linear (SURVEY.md F5), so a single-pass TF32 MMA (10-bit mantissa) is not
+// accurate enough for the 1e-4 parity bar: every product runs as 3xTF32 (tc_common.cuh), error ~1e-6 relative.
 //
-// Shared-memory operand layout (both operands, SWIZZLE_NONE, K-major, "panel-major"): the tile is
-// cut into panels of 4 consecutive k (16 bytes); inside a panel row r sits at r*16 bytes:
-//     offset(r, k) = (k/4)*PANEL + r*16 + (k%4)*4
-// = the canonical UMMA layout of 8x16B core matrices with SBO = 128 B (next 8 rows) and
-// LBO = PANEL (next 4 k).  PANEL is padded by 16 B so the 8 threads that fill one row's 128 B hit
-// 8 distinct bank groups.  (Probed on B200 with tools/tc_probe.cu: this layout and SWIZZLE_128B
-// give identical results and MMA rate; MN-major tf32 operands without swizzle return zeros, so the
-// weight-gradient kernel transposes while staging and stays K-major.)
+//   forward        Y  = act(X W^T + b)                  A = X  [64 x k],      B = W   [n_out x k]
+//   backward-data  dX = (dY * act'(Y)) W  (* relu mask) A = dZ [64 x n_out],  B = W^T [k x n_out]
 //
-// One CTA = 128 rows = 128 TMEM lanes, 9 warps: 8 converter/epilogue warps (warps w and w+4 share TMEM
-// lane quadrant w: tcgen05.ld 32x32b) and one MMA-issuing warp.  Global -> shared goes through a ring of
-// cp.async (LDGSTS) stages of raw fp32 -- bytes in flight do not depend on occupancy (the first version
-// loaded through registers and sat on long-scoreboard stalls at 12 % active warps, see profiles/) --
-// then each converter thread splits exactly the 16-byte pieces it copied (no barrier between copy and
-// convert) into the hi/lo operand stage and arrives on its `full` mbarrier; the issuer waits, issues the
-// MMAs and releases the stage with tcgen05.commit -> `empty`.  A tcgen05.mma costs its issuing thread
-// ~100 cycles (measured), which is why it has a warp of its own.  The epilogue goes TMEM -> registers ->
-// (bias, activation) -> shared staging tile -> coalesced 16-byte stores (-> optional ReLU mask).
-//
-//   forward        Y  = act(X W^T + b)                  A = X[128 x k],      B = W   [n_out x k]
-//   backward-data  dX = dZ W   (* relu-mask epilogue)   A = dZ[128 x n_out], B = W^T [k x n_out]
-//   backward-wgt   dW^T = X^T dZ, accumulated in TMEM   A = X^T[k x rows],   B = dZ^T [n_out x rows]
-//
-// Roofline: HBM-bound per layer -- (k + n_out)*4 B per row forward.
+// The weight is resident in shared memory (hi / lo panels) per CTA of a persistent grid; each warpgroup reads its A
+// fragments of 64-row tiles straight from global memory and walks the output in 64-column blocks (DESIGN.md §5.2).
+// HBM-bound per layer -- (k + n_out)*4 B per row forward.  Backward-weight: wgrad_mn.cu.
 #include "common.cuh"
 #include "tc_common.cuh"
 
 namespace emer {
 namespace tc {
 
-constexpr int ROWS = 128;
-constexpr int CHUNK = 32;                    // k per pipeline stage
-constexpr int A_PANEL = ROWS * 16 + 16;      // 2064 B (padded LBO)
-constexpr int A_STAGE = (CHUNK / 4) * A_PANEL;   // one of hi / lo: 16512 B
-constexpr int RAW_STAGE = ROWS * CHUNK * 4;  // 16 KB of raw fp32 per chunk
-constexpr int NT = 256;                      // converter threads of a multi-CTA-per-SM launch (512 when one CTA owns the SM);
-                                             // warps w, w+4, ... share TMEM lane quadrant w
+constexpr int ROWS = 64;                     // rows per warpgroup tile
+constexpr int WGS = 2;                       // warpgroups per CTA
+constexpr int THREADS = WGS * 128;
+constexpr int KB = 4;                        // k steps per wgmma batch; the B panels are padded to a multiple of 8 KB
 
 __device__ __forceinline__ float act_fwd(float v, int act) {
     if (act == EMER_ACT_RELU) return v > 0.0f ? v : 0.0f;
@@ -72,693 +47,131 @@ struct Params {
     int k, n_out;         // layer widths
     int kred;             // reduction width: fwd k, bwd n_out
     int ncols;            // output width:    fwd n_out, bwd k
-    int kred_pad;         // multiple of 8
-    int n_pad;            // multiple of 16, <= 256
+    int kred_pad;         // multiple of 8 * KB
+    int n_pad;            // multiple of 16, <= 256 (rows of the B panels)
     int act;
     int accumulate;       // bwd: dX += result
-    int tmem_cols;        // power of two >= 2*n_pad
-    int use_async;        // cp.async ring (16-byte aligned rows, no act' in the loader)
-    int a_stages, raw_stages;   // ring depths chosen by the host
-    int ring_bytes;             // operand ring area (>= the 34 816 B epilogue staging tile)
 };
 
-// Warp-specialised: NTC / 32 (8 or 16) converter/epilogue warps + 1 MMA-issuing warp.
-//   converters : cp.async raw ring -> split hi/lo -> operand stage s -> arrive full[s]
-//                ... last chunk of a tile: wait accum -> epilogue -> arrive acc_free
-//   issuer     : wait full[s] -> 3 tcgen05.mma per k-step -> commit empty[s] (and accum on the last chunk)
-// so the ~100 cycles each tcgen05.mma costs its issuing thread (phase timers, profiles/) no longer sit
-// on the converters' critical path.  a_stages / raw_stages / ring_bytes are picked by the host so that
-// 2-3 CTAs share an SM whenever shared memory allows.
-
-template <int NTC>
-__device__ __forceinline__ void conv_sync() {        // barrier among the converter threads only
-    asm volatile("bar.sync 1, %0;" ::"n"(NTC) : "memory");
+template <bool BWD>
+__device__ __forceinline__ float a_val(const Params& p, int64_t row, int col, bool ok) {
+    if (!ok || col >= p.kred) return 0.0f;
+    const float v = __ldg(p.a + row * p.lda + col);
+    if (BWD && p.act != EMER_ACT_NONE) return act_bwd(v, __ldg(p.yact + row * p.ldy + col), p.act);
+    return v;
 }
 
-template <bool BWD, int ACT, int NTC>
-__global__ void __launch_bounds__(NTC + 32) tc_linear_kernel(const Params p) {
+// output columns [n0, n0 + NB) of one 64-row tile
+template <bool BWD, int NB>
+__device__ __forceinline__ void run_block(const Params& p, uint32_t b_hi, uint32_t b_lo, const float* bias_s, int n0,
+                                          int64_t row0, int64_t row1, bool ok0, bool ok1, int q) {
+    float acc[NB / 2];
+    for (int kb = 0; kb < p.kred_pad / 8; kb += KB) {
+        uint32_t ahi[KB][4], alo[KB][4];
+#pragma unroll
+        for (int i = 0; i < KB; ++i) {
+            const int c = (kb + i) * 8 + 2 * q;
+            frag_split(a_val<BWD>(p, row0, c, ok0), a_val<BWD>(p, row0, c + 1, ok0), a_val<BWD>(p, row1, c, ok1),
+                       a_val<BWD>(p, row1, c + 1, ok1), ahi[i], alo[i]);
+        }
+        wg_fence();
+#pragma unroll
+        for (int i = 0; i < KB; ++i)
+            mma3<NB>(acc, ahi[i], alo[i], b_desc(b_hi, p.n_pad, kb + i, n0), b_desc(b_lo, p.n_pad, kb + i, n0), kb + i > 0);
+        wg_commit();
+        wg_wait0();
+    }
+#pragma unroll
+    for (int j = 0; j < NB / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int64_t row = e < 2 ? row0 : row1;
+            const int col = n0 + 8 * j + 2 * q + (e & 1);
+            if (!(e < 2 ? ok0 : ok1) || col >= p.ncols) continue;
+            float v = acc[4 * j + e];
+            float* dst = p.c + row * p.ldc + col;
+            if (!BWD) {
+                *dst = act_fwd(v + bias_s[col], p.act);
+            } else {
+                if (col < p.relu_cols && !(__ldg(p.relu_src + row * p.ld_relu + col) > 0.0f)) v = 0.0f;
+                *dst = p.accumulate ? *dst + v : v;
+            }
+        }
+    }
+}
+
+template <bool BWD>
+__global__ void __launch_bounds__(THREADS) tc_linear_kernel(const Params p) {
     extern __shared__ __align__(128) uint8_t smem[];
-    // layout: [B_hi | B_lo | operand ring / epilogue staging | raw ring | bias | barriers]
-    const int b_panel = p.n_pad * 16;
-    const int b_bytes = (p.kred_pad / 4) * b_panel;
+    const int b_bytes = (p.kred_pad / 4) * p.n_pad * 16;
     uint8_t* b_hi = smem;
     uint8_t* b_lo = smem + b_bytes;
-    uint8_t* a_ring = smem + 2 * b_bytes;
-    uint8_t* raw = a_ring + p.ring_bytes;
-    float* bias_s = reinterpret_cast<float*>(raw + (p.use_async ? p.raw_stages * RAW_STAGE : 0));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(bias_s + 256);
-    uint64_t* full_bar = bars;                   // [2] converters -> issuer
-    uint64_t* empty_bar = bars + 2;              // [2] issuer (tcgen05.commit) -> converters
-    uint64_t* accum_bar = bars + 4;              // [1] issuer -> epilogue
-    uint64_t* accfree_bar = bars + 5;            // [1] epilogue -> issuer
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
-
+    float* bias_s = reinterpret_cast<float*>(smem + 2 * b_bytes);
     const int tid = threadIdx.x;
-    const int warp = tid >> 5;
-    const bool is_issuer = warp == NTC / 32;
+    for (int i = tid * 16; i < 2 * b_bytes; i += THREADS * 16) *reinterpret_cast<float4*>(smem + i) = make_float4(0.f, 0.f, 0.f, 0.f);
+    __syncthreads();
+    // B (n, kk): forward W[n, kk]; backward W^T, i.e. W[kk, n].  W is [n_out, k] row-major either way.
+    for (int e = tid; e < p.n_out * p.k; e += THREADS) {
+        const int o = e / p.k, i = e - o * p.k;
+        float h, l;
+        split(__ldg(p.w + e), h, l);
+        const int off = BWD ? b_off(i, o, p.n_pad) : b_off(o, i, p.n_pad);
+        *reinterpret_cast<float*>(b_hi + off) = h;
+        *reinterpret_cast<float*>(b_lo + off) = l;
+    }
+    for (int e = tid; e < p.n_pad; e += THREADS) bias_s[e] = (!BWD && p.bias && e < p.ncols) ? __ldg(p.bias + e) : 0.0f;
+    fence_async_proxy();
+    __syncthreads();
 
-    if (tid == 0) {
-        mbar_init(&full_bar[0], NTC);
-        mbar_init(&full_bar[1], NTC);
-        mbar_init(&empty_bar[0], 1);
-        mbar_init(&empty_bar[1], 1);
-        mbar_init(accum_bar, 1);
-        mbar_init(accfree_bar, NTC);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        __syncwarp();
-        tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    }
-    const int n_chunks = (p.kred_pad + CHUNK - 1) / CHUNK;
+    const uint32_t bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+    const int wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
     const int64_t n_tiles = (p.n + ROWS - 1) / ROWS;
-    const int my_tiles = (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
-    const int total = my_tiles * n_chunks;
-    const int a_stages = p.a_stages, raw_stages = p.raw_stages;
-
-    constexpr int PIECES = ROWS * (CHUNK / 4) / NTC;     // 4
-    const int my_r = (tid & (NTC - 1)) >> 3, my_q = tid & 7;
-    const int64_t piece_stride = (int64_t)(NTC / 8) * p.lda;
-    const float* thread_base = p.a + (int64_t)my_r * p.lda + my_q * 4;
-    int i_tl = 0, i_c = 0, i_stage = 0;
-    auto issue_next = [&]() {
-        const int64_t row0 = ((int64_t)blockIdx.x + (int64_t)i_tl * gridDim.x) * ROWS;
-        const bool kok = i_c * CHUNK + my_q * 4 < p.kred;
-        const float* src = thread_base + row0 * p.lda + i_c * CHUNK;
-        uint8_t* dst = raw + i_stage * RAW_STAGE + tid * 16;
-        const int64_t rows_left = p.n - row0 - my_r;
-#pragma unroll
-        for (int i = 0; i < PIECES; ++i) {
-            const bool ok = kok && (i * (NTC / 8) < rows_left);
-            cp_async16(dst + i * NTC * 16, ok ? src : p.a, ok ? 16u : 0u);
-            src += piece_stride;
-        }
-        if (++i_c == n_chunks) { i_c = 0; ++i_tl; }
-        if (++i_stage == raw_stages) i_stage = 0;
-    };
-    int issued = 0;
-    if (!is_issuer && p.use_async) {
-        for (int g = 0; g < raw_stages - 1; ++g) {
-            if (issued < total) { issue_next(); ++issued; }
-            cp_async_commit();
-        }
+    const int full_blocks = p.n_pad / 64, tail = p.n_pad - full_blocks * 64;
+    for (int64_t tile = (int64_t)blockIdx.x * WGS + wg; tile < n_tiles; tile += (int64_t)gridDim.x * WGS) {
+        const int64_t row0 = tile * ROWS + 16 * w + (lane >> 2), row1 = row0 + 8;
+        const bool ok0 = row0 < p.n, ok1 = row1 < p.n;
+        for (int b = 0; b < full_blocks; ++b) run_block<BWD, 64>(p, bh, bl, bias_s, b * 64, row0, row1, ok0, ok1, q);
+        const int n0 = full_blocks * 64;
+        if (tail == 16) run_block<BWD, 16>(p, bh, bl, bias_s, n0, row0, row1, ok0, ok1, q);
+        else if (tail == 32) run_block<BWD, 32>(p, bh, bl, bias_s, n0, row0, row1, ok0, ok1, q);
+        else if (tail == 48) run_block<BWD, 48>(p, bh, bl, bias_s, n0, row0, row1, ok0, ok1, q);
     }
-
-    // ---- resident B operand (converter threads): hi/lo panels of W
-    if (!is_issuer) {
-        if (!BWD) {
-            for (int e = tid; e < p.n_pad * p.kred_pad; e += NTC) {
-                const int nn = e / p.kred_pad, r = e - nn * p.kred_pad;
-                float v = 0.0f;
-                if (r < p.kred && nn < p.ncols) v = __ldg(p.w + (int64_t)nn * p.k + r);
-                float hi, lo;
-                split(v, hi, lo);
-                const int off = (r >> 2) * b_panel + nn * 16 + (r & 3) * 4;
-                *reinterpret_cast<float*>(b_hi + off) = hi;
-                *reinterpret_cast<float*>(b_lo + off) = lo;
-            }
-            for (int e = tid; e < 256; e += NTC) bias_s[e] = (p.bias && e < p.ncols) ? __ldg(p.bias + e) : 0.0f;
-        } else {
-            for (int e = tid; e < p.n_pad * p.kred_pad; e += NTC) {
-                const int r = e / p.n_pad, nn = e - r * p.n_pad;
-                float v = 0.0f;
-                if (r < p.kred && nn < p.ncols) v = __ldg(p.w + (int64_t)r * p.k + nn);
-                float hi, lo;
-                split(v, hi, lo);
-                const int off = (r >> 2) * b_panel + nn * 16 + (r & 3) * 4;
-                *reinterpret_cast<float*>(b_hi + off) = hi;
-                *reinterpret_cast<float*>(b_lo + off) = lo;
-            }
-        }
-        fence_async_proxy();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (is_issuer) {
-        // ================= MMA issuer warp (one lane issues; the warp stays converged) =================
-        const uint32_t idesc = make_idesc(128, p.n_pad);
-        const uint64_t desc_a = make_desc(0, A_PANEL, 128);
-        const uint64_t desc_b = make_desc(0, b_panel, 128);
-        const uint32_t a_ring_addr = smem_u32(a_ring) >> 4;
-        const uint32_t b_hi_addr = smem_u32(b_hi) >> 4, b_lo_addr = smem_u32(b_lo) >> 4;
-        const uint32_t d1 = tmem_base + (uint32_t)p.n_pad;
-        int tl = 0, c = 0;
-        uint32_t use0 = 0, use1 = 0;
-        for (int g = 0; g < total; ++g) {
-            const int s = (a_stages == 2) ? (g & 1) : 0;
-            const uint32_t uses = s ? use1 : use0;
-            mbar_wait(&full_bar[s], uses & 1);                       // operands of chunk g are in place
-            if (c == 0 && tl > 0) mbar_wait(accfree_bar, (tl - 1) & 1);   // previous tile's accumulators drained
-            tc_fence_after();
-            if (mma_issue_lane(tid)) {
-                const int k0 = c * CHUNK;
-                const int ksteps = min(CHUNK, p.kred_pad - k0) / 8;
-                const uint32_t a_hi_addr = a_ring_addr + (uint32_t)((s * 2) * A_STAGE >> 4);
-                const uint32_t a_lo_addr = a_hi_addr + (uint32_t)(A_STAGE >> 4);
-                const uint32_t b_off = (uint32_t)((k0 >> 2) * b_panel) >> 4;
-#pragma unroll 4
-                for (int ks = 0; ks < ksteps; ++ks) {
-                    const uint32_t ao = (uint32_t)(ks * 2 * A_PANEL) >> 4;
-                    const uint32_t bo = b_off + ((uint32_t)(ks * 2 * b_panel) >> 4);
-                    const uint64_t da_hi = desc_a | (uint64_t)(a_hi_addr + ao);
-                    const uint64_t da_lo = desc_a | (uint64_t)(a_lo_addr + ao);
-                    const uint64_t db_hi = desc_b | (uint64_t)(b_hi_addr + bo);
-                    const uint64_t db_lo = desc_b | (uint64_t)(b_lo_addr + bo);
-                    const uint32_t first = (c == 0 && ks == 0) ? 0u : 1u;
-                    mma_tf32(tmem_base, da_hi, db_hi, idesc, first);      // chain 0
-                    mma_tf32(d1, da_lo, db_hi, idesc, first);             // chain 1
-                    mma_tf32(d1, da_hi, db_lo, idesc, 1u);
-                }
-                tc_commit(&empty_bar[s]);
-                if (c == n_chunks - 1) tc_commit(accum_bar);
-            }
-            __syncwarp();
-            if (s) ++use1; else ++use0;
-            if (++c == n_chunks) { c = 0; ++tl; }
-        }
-    } else {
-        // ================= converter / epilogue warps =================
-        const bool vec_c = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.c) & 15) == 0);
-        const bool vec_m = p.relu_src && (p.ld_relu % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.relu_src) & 15) == 0);
-        int tl = 0, c = 0, rstage = 0;
-        uint32_t use0 = 0, use1 = 0;
-        for (int g = 0; g < total; ++g) {
-            const int64_t row0 = ((int64_t)blockIdx.x + (int64_t)tl * gridDim.x) * ROWS;
-            const int k0 = c * CHUNK;
-            const int s = (a_stages == 2) ? (g & 1) : 0;
-            uint8_t* a_hi = a_ring + (s * 2) * A_STAGE;
-            uint8_t* a_lo = a_hi + A_STAGE;
-            if (p.use_async) {
-                if (issued < total) { issue_next(); ++issued; }
-                cp_async_commit();
-                if (raw_stages == 4) cp_async_wait<3>();
-                else cp_async_wait<1>();
-            }
-            {
-                const uint32_t uses = s ? use1 : use0;
-                if (uses > 0) mbar_wait(&empty_bar[s], (uses - 1) & 1);     // MMAs that read stage s retired
-            }
-            const uint8_t* rs = raw + rstage * RAW_STAGE + tid * 16;
-            const int kk = k0 + my_q * 4;
-            const bool tail = k0 + CHUNK > p.kred;
-#pragma unroll
-            for (int i = 0; i < PIECES; ++i) {
-                const int r = i * (NTC / 8) + my_r;
-                float v[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-                if (p.use_async) {
-                    const float4 t = *reinterpret_cast<const float4*>(rs + i * NTC * 16);
-                    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
-                    if (tail) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j)
-                            if (kk + j >= p.kred) v[j] = 0.0f;
-                    }
-                } else {
-                    const int64_t row = row0 + r;
-                    if (row < p.n) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            if (kk + j < p.kred) {
-                                float t = __ldg(p.a + row * p.lda + kk + j);
-                                if (BWD && p.act != EMER_ACT_NONE) t = act_bwd(t, __ldg(p.yact + row * p.ldy + kk + j), p.act);
-                                v[j] = t;
-                            }
-                        }
-                    }
-                }
-                float4 h, l;
-                split(v[0], h.x, l.x); split(v[1], h.y, l.y); split(v[2], h.z, l.z); split(v[3], h.w, l.w);
-                *reinterpret_cast<float4*>(a_hi + my_q * A_PANEL + r * 16) = h;
-                *reinterpret_cast<float4*>(a_lo + my_q * A_PANEL + r * 16) = l;
-            }
-            fence_async_proxy();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
-            mbar_arrive(&full_bar[s]);
-            if (s) ++use1; else ++use0;
-            if (++rstage == raw_stages) rstage = 0;
-            const bool last_chunk = (c == n_chunks - 1);
-            const int tile_idx = tl;
-            if (++c == n_chunks) { c = 0; ++tl; }
-            if (!last_chunk) continue;
-
-            // ---- epilogue: TMEM -> registers -> (bias, activation) -> shared staging -> coalesced global.
-            // All MMAs of the tile have retired (accum barrier), so the operand ring doubles as staging.
-            mbar_wait(accum_bar, tile_idx & 1);
-            tc_fence_after();
-            float* stage = reinterpret_cast<float*>(a_ring);
-            constexpr int SLD = 64 + 4;
-            const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-            const int my_row = tid & 127;
-            for (int cb = 0; cb < p.n_pad; cb += 64) {
-                const int cw = min(64, p.n_pad - cb);
-                for (int c0 = (warp >> 2) * 16; c0 < cw; c0 += (NTC / 128) * 16) {
-                    uint32_t r0[16], r1[16];
-                    tmem_ld16(lane_addr + (uint32_t)(cb + c0), r0);
-                    tmem_ld16(lane_addr + (uint32_t)(p.n_pad + cb + c0), r1);
-                    tmem_ld_wait();
-                    float* dstp = stage + my_row * SLD + c0;
-#pragma unroll
-                    for (int j0 = 0; j0 < 16; j0 += 4) {
-                        float o[4];
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            float v = __uint_as_float(r0[j0 + j]) + __uint_as_float(r1[j0 + j]);
-                            if (!BWD) {
-                                v += bias_s[cb + c0 + j0 + j];
-                                if (ACT == EMER_ACT_RELU) v = v > 0.0f ? v : 0.0f;
-                                if (ACT == EMER_ACT_SIGMOID) v = 1.0f / (1.0f + expf(-v));
-                            }
-                            o[j] = v;
-                        }
-                        *reinterpret_cast<float4*>(dstp + j0) = make_float4(o[0], o[1], o[2], o[3]);
-                    }
-                }
-                if (cb + 64 >= p.n_pad) {
-                    // last TMEM read of this tile done: let the issuer start the next tile's MMAs
-                    tc_fence_before();
-                    mbar_arrive(accfree_bar);
-                }
-                conv_sync<NTC>();
-                // copy-out: consecutive threads write consecutive 16-byte pieces of a row
-                const int q_per_row = cw / 4;                  // 4, 8, 12 or 16
-                const int rows_per_pass = NTC / q_per_row;      // exact for 4, 8, 16; 12 -> 21 rows (+4 idle threads)
-                const int q = tid % q_per_row, r_first = tid / q_per_row;
-                if (r_first < rows_per_pass) {
-                    for (int r = r_first; r < ROWS; r += rows_per_pass) {
-                        const int64_t row = row0 + r;
-                        const int col = cb + q * 4;
-                        if (row >= p.n || col >= p.ncols) continue;
-                        const float4 sv = *reinterpret_cast<const float4*>(stage + r * SLD + q * 4);
-                        float o[4] = {sv.x, sv.y, sv.z, sv.w};
-                        const bool full = col + 3 < p.ncols;
-                        if (BWD && p.relu_src && col < p.relu_cols) {
-                            const float* m = p.relu_src + row * p.ld_relu + col;
-                            if (vec_m && full && col + 3 < p.relu_cols) {
-                                const float4 mm = __ldg(reinterpret_cast<const float4*>(m));
-                                if (!(mm.x > 0.0f)) o[0] = 0.0f;
-                                if (!(mm.y > 0.0f)) o[1] = 0.0f;
-                                if (!(mm.z > 0.0f)) o[2] = 0.0f;
-                                if (!(mm.w > 0.0f)) o[3] = 0.0f;
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 4; ++j)
-                                    if (col + j < p.ncols && col + j < p.relu_cols && !(__ldg(m + j) > 0.0f)) o[j] = 0.0f;
-                            }
-                        }
-                        float* out = p.c + row * p.ldc + col;
-                        if (vec_c && full) {
-                            if (BWD && p.accumulate) {
-                                const float4 old = *reinterpret_cast<const float4*>(out);
-                                o[0] += old.x; o[1] += old.y; o[2] += old.z; o[3] += old.w;
-                            }
-                            *reinterpret_cast<float4*>(out) = make_float4(o[0], o[1], o[2], o[3]);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                if (col + j < p.ncols) {
-                                    if (BWD && p.accumulate) o[j] += out[j];
-                                    out[j] = o[j];
-                                }
-                            }
-                        }
-                    }
-                }
-                conv_sync<NTC>();         // staging buffer free (next column block / next tile's operands)
-            }
-        }
-        if (p.use_async) cp_async_wait<0>();
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
 }
 
-static int round_up(int v, int m) { return (v + m - 1) / m * m; }
+inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
-template <bool BWD, int ACT, int NTC>
-static int launch_t(Params& p, size_t smem, int64_t grid, cudaStream_t st, const char* what) {
-    static size_t configured_dev[64] = {0};          // the attribute is per device
-    size_t& configured = configured_dev[current_device()];
+template <bool BWD>
+static int launch(Params& p, cudaStream_t st, const char* what) {
+    p.kred = BWD ? p.n_out : p.k;
+    p.ncols = BWD ? p.k : p.n_out;
+    p.kred_pad = round_up(p.kred, 8 * KB);
+    p.n_pad = round_up(p.ncols, 16);
+    EMER_REQUIRE(p.n_pad <= 256, "%s: output width %d exceeds one MMA (256)", what, p.ncols);
+    const size_t smem = (size_t)2 * (p.kred_pad / 4) * p.n_pad * 16 + (size_t)p.n_pad * 4;
+    EMER_REQUIRE(smem <= 227 * 1024, "%s: layer %dx%d needs %zu B of shared memory", what, p.k, p.n_out, smem);
+    static size_t configured_dev[2][64] = {{0}};          // the attribute is per kernel and per device
+    size_t& configured = configured_dev[BWD ? 1 : 0][current_device()];
     if (smem > configured) {
-        cudaError_t e = cudaFuncSetAttribute(tc_linear_kernel<BWD, ACT, NTC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(tc_linear_kernel<BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) {
             set_error("%s: cudaFuncSetAttribute(%zu): %s", what, smem, cudaGetErrorString(e));
             return -2;
         }
         configured = smem;
     }
-    tc_linear_kernel<BWD, ACT, NTC><<<(unsigned)grid, NTC + 32, smem, st>>>(p);
+    // persistent grid of the CTAs resident at once (registers queried once, shared memory from this layer's panels)
+    static int cache[64] = {0};
+    int ctas_per_sm = resident_ctas(tc_linear_kernel<BWD>, THREADS, 0, st, cache);
+    const int by_smem = (int)((228 * 1024) / (smem + 1024));
+    if (ctas_per_sm > by_smem) ctas_per_sm = by_smem > 0 ? by_smem : 1;
+    const int64_t ctas = ceil_div(ceil_div(p.n, ROWS), WGS);
+    int64_t grid = (int64_t)sm_count() * ctas_per_sm;
+    if (grid > ctas) grid = ctas;
+    tc_linear_kernel<BWD><<<(unsigned)grid, THREADS, smem, st>>>(p);
     return check_launch(what);
 }
 
-// One CTA per SM (wide layers: the resident weight panels fill shared memory) runs 16 converter warps, the
-// 2-3 CTA configurations 8 each: either way ~16+ warps per SM hide the converters' fixed-latency chains.
-template <bool BWD, int ACT>
-static int launch_w(Params& p, size_t smem, int64_t grid, int ctas_per_sm, cudaStream_t st, const char* what) {
-    if (ctas_per_sm == 1) return launch_t<BWD, ACT, 512>(p, smem, grid, st, what);
-    return launch_t<BWD, ACT, NT>(p, smem, grid, st, what);
-}
-
-template <bool BWD>
-static int launch(Params& p, cudaStream_t st, const char* what) {
-    p.kred = BWD ? p.n_out : p.k;
-    p.ncols = BWD ? p.k : p.n_out;
-    p.kred_pad = round_up(p.kred, 8);
-    p.n_pad = round_up(p.ncols, 16);
-    EMER_REQUIRE(p.n_pad <= 256, "%s: output width %d exceeds one MMA (256)", what, p.ncols);
-    p.tmem_cols = 32;
-    while (p.tmem_cols < 2 * p.n_pad) p.tmem_cols *= 2;
-    const size_t w_bytes = (size_t)2 * (p.kred_pad / 4) * p.n_pad * 16;
-    const size_t misc = 256 * 4 + 6 * 8 + 16;
-    const size_t staging = (size_t)ROWS * 68 * 4;                        // epilogue tile: 128 x (64+4) floats
-    const size_t ring1 = staging > (size_t)2 * A_STAGE ? staging : (size_t)2 * A_STAGE;
-    const size_t ring2 = (size_t)2 * 2 * A_STAGE;
-    const bool can_async = (p.lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.a) & 15) == 0) &&
-                           !(BWD && p.act != EMER_ACT_NONE);
-    // The kernel is instruction-latency bound inside one CTA (measured with the phase timers), so
-    // prefer the ring depths that let 2-3 CTAs share an SM; deeper rings only when one CTA fits anyway.
-    struct Cfg { int a, raw; size_t bytes; };
-    Cfg cands[4] = {{1, 2, w_bytes + ring1 + 2 * RAW_STAGE + misc}, {2, 4, w_bytes + ring2 + 4 * RAW_STAGE + misc},
-                    {2, 2, w_bytes + ring2 + 2 * RAW_STAGE + misc}, {1, 2, w_bytes + ring1 + 2 * RAW_STAGE + misc}};
-    size_t smem = 0;
-    int ctas_per_sm = 1;
-    p.use_async = 0;
-    if (can_async) {
-        if (cands[0].bytes <= 113 * 1024) {
-            p.use_async = 1; p.a_stages = 1; p.raw_stages = 2; p.ring_bytes = (int)ring1; smem = cands[0].bytes;
-            ctas_per_sm = smem <= 75 * 1024 ? 3 : 2;
-        } else {
-            for (int i = 1; i < 4 && !p.use_async; ++i) {
-                if (cands[i].bytes <= 227 * 1024) {
-                    p.use_async = 1; p.a_stages = cands[i].a; p.raw_stages = cands[i].raw;
-                    p.ring_bytes = (int)(cands[i].a == 2 ? ring2 : ring1); smem = cands[i].bytes;
-                }
-            }
-        }
-    }
-    if (!p.use_async) {
-        p.a_stages = 2; p.raw_stages = 2; p.ring_bytes = (int)ring2;
-        smem = w_bytes + ring2 + misc;
-        if (smem > 227 * 1024) { p.a_stages = 1; p.ring_bytes = (int)ring1; smem = w_bytes + ring1 + misc; }
-        ctas_per_sm = smem <= 75 * 1024 ? 3 : (smem <= 113 * 1024 ? 2 : 1);
-    }
-    EMER_REQUIRE(smem <= 227 * 1024, "%s: layer %dx%d needs %zu B of shared memory", what, p.k, p.n_out, smem);
-    // TMEM: co-resident CTAs share 512 columns
-    while (ctas_per_sm > 1 && ctas_per_sm * p.tmem_cols > 512) --ctas_per_sm;
-    const int64_t n_tiles = ceil_div(p.n, ROWS);
-    int64_t grid = (int64_t)sm_count() * ctas_per_sm;
-    if (grid > n_tiles) grid = n_tiles;
-    if (BWD) return launch_w<true, 0>(p, smem, grid, ctas_per_sm, st, what);
-    if (p.act == EMER_ACT_RELU) return launch_w<false, EMER_ACT_RELU>(p, smem, grid, ctas_per_sm, st, what);
-    if (p.act == EMER_ACT_SIGMOID) return launch_w<false, EMER_ACT_SIGMOID>(p, smem, grid, ctas_per_sm, st, what);
-    return launch_w<false, EMER_ACT_NONE>(p, smem, grid, ctas_per_sm, st, what);
-}
-
 }  // namespace tc
-
-// ------------------------------------------------------------------------------------------------
-// Weight gradient:  dW^T[k, n_out] += X^T dZ,  db += sum_rows dZ.
-//
-// The reduction runs over the ROWS.  tf32 operands must stay K-major (see the probe note above), so
-// the staging step transposes: a tile is 64 rows; panel rq holds rows 4rq..4rq+3 as the 16-byte
-// "k" group and the FEATURE is the operand row:   offset(f, r) = (r/4)*PANEL + f*16 + (r%4)*4.
-// A = X^T (M = one 128-feature block of k), B = dZ^T (N = n_out), 8 tf32 k-steps per tile.
-// Raw fp32 rows arrive through cp.async; each thread then gathers 4 rows x 1 feature from the raw
-// tile (conflict-free: consecutive threads, consecutive features) and writes one 16-byte group.
-// Every persistent CTA keeps dW^T in TMEM across all of its tiles (hi*hi chain and cross-term
-// chain per 128-feature block) and flushes once with atomics.
-namespace tcw {
-
-using namespace emer::tc;
-
-struct WParams {
-    const float* x;
-    int64_t ldx;
-    const float* dz;     // dZ (activation derivative already applied)
-    int64_t lddz;
-    float* dw;           // [n_out, k]
-    float* db;           // [n_out] or null
-    int64_t n;
-    int k, n_out;
-    int k_pad4;          // k rounded to 4  (raw row width)
-    int n_pad;           // n_out rounded to 16
-    int m_blocks;        // ceil(k / 128)
-    int w_rows;          // rows per tile: 64 or 32 (4 rows = one 16-byte k group, 8 rows = one k-step)
-    int a_rows;          // feature rows per A panel: 64 when k <= 64 (the MMA's rows 64..127 then read the next
-                         // panel's finite data and land in accumulator lanes nobody reads), else 128
-    int nbuf;            // operand buffers (2: conversion of tile t+1 overlaps the MMAs of tile t)
-    int raw_stages;      // cp.async stages of raw rows
-    int tmem_cols;
-};
-
-// 16 converter warps + 1 MMA-issuing warp, mbarrier ring between them (see tc_linear_kernel).  One CTA per SM
-// (the operand buffers fill shared memory), so the converter warps are the only latency hiding there is:
-// the ncu capture of the 8-warp version (profiles/r1_prof_wgrad_summary.md) sat at 2.2 warps per scheduler,
-// 42 % issue-active, stalled on fixed-latency dependencies (`wait`) -- hence 16 warps, and item indices
-// advanced incrementally instead of by integer division.
-constexpr int WNT = 512;
-constexpr int WNT_ALL = WNT + 32;
-
-__device__ __forceinline__ void wconv_sync() {       // barrier among the converter threads only
-    asm volatile("bar.sync 1, 512;" ::: "memory");
-}
-
-__global__ void __launch_bounds__(WNT_ALL) tc_wgrad_kernel(const WParams p) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int RQn = p.w_rows / 4;
-    const int a_panel = p.a_rows * 16 + 16;
-    const int b_panel = p.n_pad * 16 + 16;
-    const int a_bytes = p.m_blocks * RQn * a_panel;         // one of hi / lo, one buffer
-    const int b_bytes = RQn * b_panel;
-    const int buf_bytes = 2 * a_bytes + 2 * b_bytes;        // [A_hi | A_lo | B_hi | B_lo]
-    const int rawx_bytes = p.w_rows * p.k_pad4 * 4;
-    const int rawz_bytes = p.w_rows * p.n_pad * 4;
-    const int raw_stage = rawx_bytes + rawz_bytes;
-    uint8_t* ops = smem;
-    uint8_t* raw = ops + p.nbuf * buf_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(raw + p.raw_stages * raw_stage);
-    uint64_t* full_bar = bars;            // [2]
-    uint64_t* empty_bar = bars + 2;       // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-
-    const int tid = threadIdx.x;
-    const int warp = tid >> 5;
-    const bool is_issuer = warp == WNT / 32;
-    if (tid == 0) {
-        mbar_init(&full_bar[0], WNT);
-        mbar_init(&full_bar[1], WNT);
-        mbar_init(&empty_bar[0], 1);
-        mbar_init(&empty_bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        __syncwarp();
-        tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    }
-    // operand buffers start as zeros: padding features / columns never hold NaN bit patterns
-    for (int i = tid * 16; i < p.nbuf * buf_bytes; i += WNT_ALL * 16)
-        *reinterpret_cast<float4*>(smem + i) = make_float4(0.f, 0.f, 0.f, 0.f);
-
-    const int64_t n_tiles = (p.n + p.w_rows - 1) / p.w_rows;
-    const int my_tiles = (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
-    const int xq = p.k_pad4 / 4, zq = p.n_pad / 4;
-
-    // Work items e = tid, tid + WNT, ... of a [major, minor] index space: (e / width, e % width) advanced by
-    // (WNT / width, WNT % width) with one carry -- the divisions happen once per kernel, not once per item.
-    struct Walk { int maj0, min0, dmaj, dmin; };
-    auto walk = [&](int width) { return Walk{tid / width, tid % width, WNT / width, WNT % width}; };
-    const Walk w_xq = walk(xq), w_zq = walk(zq), w_a = walk(p.k_pad4), w_b = walk(p.n_pad);
-
-    auto issue = [&](int t) {             // converter threads only
-        const int64_t row0 = ((int64_t)blockIdx.x + (int64_t)t * gridDim.x) * p.w_rows;
-        uint8_t* dx = raw + (t % p.raw_stages) * raw_stage;
-        uint8_t* dzs = dx + rawx_bytes;
-        {
-            int r = w_xq.maj0, q = w_xq.min0;
-            for (int e = tid; e < p.w_rows * xq; e += WNT) {
-                const int64_t row = row0 + r;
-                const bool ok = (row < p.n) && (q * 4 < p.k);
-                cp_async16(dx + e * 16, ok ? (p.x + row * p.ldx + q * 4) : p.x, ok ? 16u : 0u);
-                r += w_xq.dmaj; q += w_xq.dmin;
-                if (q >= xq) { q -= xq; ++r; }
-            }
-        }
-        {
-            int r = w_zq.maj0, q = w_zq.min0;
-            for (int e = tid; e < p.w_rows * zq; e += WNT) {
-                const int64_t row = row0 + r;
-                const bool ok = (row < p.n) && (q * 4 < p.n_out);
-                cp_async16(dzs + e * 16, ok ? (p.dz + row * p.lddz + q * 4) : p.dz, ok ? 16u : 0u);
-                r += w_zq.dmaj; q += w_zq.dmin;
-                if (q >= zq) { q -= zq; ++r; }
-            }
-        }
-    };
-    if (!is_issuer) {
-        for (int t = 0; t < p.raw_stages; ++t) {
-            if (t < my_tiles) issue(t);
-            cp_async_commit();
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (is_issuer) {
-        const uint32_t idesc = make_idesc(128, p.n_pad);
-        const uint64_t desc_a = make_desc(0, a_panel, 128), desc_b = make_desc(0, b_panel, 128);
-        const int ksteps = p.w_rows / 8;
-        uint32_t use[2] = {0, 0};
-        for (int t = 0; t < my_tiles; ++t) {
-            const int b = (p.nbuf == 2) ? (t & 1) : 0;
-            mbar_wait(&full_bar[b], use[b] & 1);
-            tc_fence_after();
-            if (mma_issue_lane(tid)) {
-                const uint32_t base = smem_u32(ops + b * buf_bytes);
-                const uint32_t a_hi_addr = base >> 4, a_lo_addr = (base + a_bytes) >> 4;
-                const uint32_t b_hi_addr = (base + 2 * a_bytes) >> 4, b_lo_addr = (base + 2 * a_bytes + b_bytes) >> 4;
-                for (int ks = 0; ks < ksteps; ++ks) {
-                    const uint32_t bo = (uint32_t)(ks * 2 * b_panel) >> 4;
-                    const uint64_t db_hi = desc_b | (uint64_t)(b_hi_addr + bo);
-                    const uint64_t db_lo = desc_b | (uint64_t)(b_lo_addr + bo);
-                    const uint32_t acc = (t == 0 && ks == 0) ? 0u : 1u;
-                    for (int mb = 0; mb < p.m_blocks; ++mb) {
-                        const uint32_t ao = (uint32_t)((mb * RQn + ks * 2) * a_panel) >> 4;
-                        const uint64_t da_hi = desc_a | (uint64_t)(a_hi_addr + ao);
-                        const uint64_t da_lo = desc_a | (uint64_t)(a_lo_addr + ao);
-                        const uint32_t d0 = tmem_base + (uint32_t)(mb * 2 * p.n_pad);
-                        mma_tf32(d0, da_hi, db_hi, idesc, acc);                           // chain 0
-                        mma_tf32(d0 + (uint32_t)p.n_pad, da_lo, db_hi, idesc, acc);       // chain 1
-                        mma_tf32(d0 + (uint32_t)p.n_pad, da_hi, db_lo, idesc, 1u);
-                    }
-                }
-                tc_commit(&empty_bar[b]);
-            }
-            __syncwarp();
-            ++use[b];
-        }
-    } else {
-        // db: with n_pad | WNT every thread meets one dZ column only (o = tid % n_pad) and keeps its partial column
-        // sum in a register; otherwise threads 0..n_out-1 walk the raw tile (the old, slower way)
-        const bool bias_in_loop = p.db && (WNT % p.n_pad == 0);
-        float bsum = 0.0f;
-        uint32_t use[2] = {0, 0};
-        for (int t = 0; t < my_tiles; ++t) {
-            const int b = (p.nbuf == 2) ? (t & 1) : 0;
-            // raw tile t landed (each thread waits for its own pieces; the barrier publishes all of them)
-            if (p.raw_stages == 2) cp_async_wait<1>();
-            else cp_async_wait<0>();
-            wconv_sync();
-            if (use[b] > 0) mbar_wait(&empty_bar[b], (use[b] - 1) & 1);     // MMAs that read buffer b retired
-            uint8_t* a_hi = ops + b * buf_bytes;
-            uint8_t* a_lo = a_hi + a_bytes;
-            uint8_t* b_hi = a_lo + a_bytes;
-            uint8_t* b_lo = b_hi + b_bytes;
-            const float* rx = reinterpret_cast<const float*>(raw + (t % p.raw_stages) * raw_stage);
-            const float* rz = reinterpret_cast<const float*>(raw + (t % p.raw_stages) * raw_stage + rawx_bytes);
-            // ---- A = X^T: item (rq, f): rows 4rq..4rq+3 of feature f -> one 16-byte k group
-            {
-                int rq = w_a.maj0, f = w_a.min0;
-                for (int e = tid; e < RQn * p.k_pad4; e += WNT) {
-                    float4 h, l;
-                    if (f < p.k) {
-                        const float* src = rx + (rq * 4) * p.k_pad4 + f;
-                        split(src[0], h.x, l.x);
-                        split(src[p.k_pad4], h.y, l.y);
-                        split(src[2 * p.k_pad4], h.z, l.z);
-                        split(src[3 * p.k_pad4], h.w, l.w);
-                    } else {
-                        h = l = make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
-                    const int off = (p.a_rows == 128) ? ((f >> 7) * RQn + rq) * a_panel + (f & 127) * 16
-                                                      : rq * a_panel + f * 16;
-                    *reinterpret_cast<float4*>(a_hi + off) = h;
-                    *reinterpret_cast<float4*>(a_lo + off) = l;
-                    rq += w_a.dmaj; f += w_a.dmin;
-                    if (f >= p.k_pad4) { f -= p.k_pad4; ++rq; }
-                }
-            }
-            // ---- B = dZ^T
-            {
-                int rq = w_b.maj0, o = w_b.min0;
-                for (int e = tid; e < RQn * p.n_pad; e += WNT) {
-                    float4 h, l;
-                    if (o < p.n_out) {
-                        const float* src = rz + (rq * 4) * p.n_pad + o;
-                        const float v0 = src[0], v1 = src[p.n_pad], v2 = src[2 * p.n_pad], v3 = src[3 * p.n_pad];
-                        if (bias_in_loop) bsum += (v0 + v1) + (v2 + v3);
-                        split(v0, h.x, l.x);
-                        split(v1, h.y, l.y);
-                        split(v2, h.z, l.z);
-                        split(v3, h.w, l.w);
-                    } else {
-                        h = l = make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
-                    *reinterpret_cast<float4*>(b_hi + rq * b_panel + o * 16) = h;
-                    *reinterpret_cast<float4*>(b_lo + rq * b_panel + o * 16) = l;
-                    rq += w_b.dmaj; o += w_b.dmin;
-                    if (o >= p.n_pad) { o -= p.n_pad; ++rq; }
-                }
-            }
-            if (p.db && !bias_in_loop && tid < p.n_out) {
-                for (int r = 0; r < p.w_rows; ++r) bsum += rz[r * p.n_pad + tid];
-            }
-            fence_async_proxy();
-            mbar_arrive(&full_bar[b]);
-            ++use[b];
-            wconv_sync();                       // everyone is done reading raw stage t
-            if (t + p.raw_stages < my_tiles) issue(t + p.raw_stages);
-            cp_async_commit();
-        }
-        cp_async_wait<0>();
-        if (my_tiles > 0) {
-            const int lb = (p.nbuf == 2) ? ((my_tiles - 1) & 1) : 0;
-            mbar_wait(&empty_bar[lb], (use[lb] - 1) & 1);          // the last tile's MMAs retired
-            if (p.nbuf == 2 && my_tiles > 1) mbar_wait(&empty_bar[lb ^ 1], (use[lb ^ 1] - 1) & 1);
-            tc_fence_after();
-            // flush: lane f of block mb holds dW^T[mb*128 + f, :]; warps w, w+4, w+8, w+12 share lane quadrant w
-            for (int mb = 0; mb < p.m_blocks; ++mb) {
-                const int f = mb * 128 + (tid & 127);
-                const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(mb * 2 * p.n_pad);
-                for (int c0 = (warp >> 2) * 16; c0 < p.n_pad; c0 += (WNT / 128) * 16) {
-                    uint32_t r0[16], r1[16];
-                    tmem_ld16(lane_addr + (uint32_t)c0, r0);
-                    tmem_ld16(lane_addr + (uint32_t)(p.n_pad + c0), r1);
-                    tmem_ld_wait();
-                    if (f < p.k) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const int o = c0 + j;
-                            if (o < p.n_out)
-                                atomicAdd(p.dw + (int64_t)o * p.k + f, __uint_as_float(r0[j]) + __uint_as_float(r1[j]));
-                        }
-                    }
-                }
-            }
-            if (bias_in_loop) {
-                // fold the WNT / n_pad partial sums of every column in shared memory (the raw ring is idle now)
-                float* red = reinterpret_cast<float*>(raw);
-                red[tid] = bsum;
-                wconv_sync();
-                if (tid < p.n_out) {
-                    float acc = 0.0f;
-                    for (int j = tid; j < WNT; j += p.n_pad) acc += red[j];
-                    atomicAdd(p.db + tid, acc);
-                }
-            } else if (p.db && tid < p.n_out) {
-                atomicAdd(p.db + tid, bsum);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-}
-
-}  // namespace tcw
 }  // namespace emer
 
 using namespace emer;
@@ -786,60 +199,4 @@ extern "C" int emer_linear_tc_bwd_data(const float* dy, int64_t lddy, const floa
     p.relu_src = relu_src; p.ld_relu = ld_relu; p.relu_cols = relu_src ? relu_cols : 0;
     p.n = n; p.k = k; p.n_out = n_out; p.act = act; p.accumulate = accumulate;
     return tc::launch<true>(p, (cudaStream_t)stream, "emer_linear_tc_bwd_data");
-}
-
-extern "C" int emer_linear_tc_bwd_weight(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw,
-                                         float* db, int64_t n, int k, int n_out, void* stream) {
-    using namespace emer::tcw;
-    if (n == 0) return 0;
-    EMER_REQUIRE(x && dz && dw, "emer_linear_tc_bwd_weight: NULL pointer");
-    EMER_REQUIRE(n_out <= 128 && k <= 256, "emer_linear_tc_bwd_weight: widths k=%d n_out=%d out of range", k, n_out);
-    EMER_REQUIRE(ldx % 4 == 0 && lddz % 4 == 0 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)dz & 15) == 0,
-                 "emer_linear_tc_bwd_weight: rows must be 16-byte aligned (ldx=%lld lddz=%lld)", (long long)ldx,
-                 (long long)lddz);
-    WParams p{};
-    p.x = x; p.ldx = ldx; p.dz = dz; p.lddz = lddz; p.dw = dw; p.db = db;
-    p.n = n; p.k = k; p.n_out = n_out;
-    p.k_pad4 = (k + 3) / 4 * 4;
-    EMER_REQUIRE(p.k_pad4 <= ldx, "emer_linear_tc_bwd_weight: row stride %lld shorter than padded width %d", (long long)ldx,
-                 p.k_pad4);
-    p.n_pad = (n_out + 15) / 16 * 16;
-    EMER_REQUIRE((n_out + 3) / 4 * 4 <= lddz, "emer_linear_tc_bwd_weight: dZ rows too short");
-    p.m_blocks = (k + 127) / 128;
-    p.tmem_cols = 32;
-    while (p.tmem_cols < p.m_blocks * 2 * p.n_pad) p.tmem_cols *= 2;
-    EMER_REQUIRE(p.tmem_cols <= 512, "emer_linear_tc_bwd_weight: accumulator does not fit TMEM");
-    p.a_rows = p.k_pad4 <= 64 ? 64 : 128;
-    // tile rows / operand buffers / raw stages: the deepest overlap that fits 227 KB
-    const int cand[6][3] = {{64, 2, 2}, {64, 2, 1}, {32, 2, 2}, {32, 2, 1}, {64, 1, 2}, {64, 1, 1}};
-    size_t smem = 0;
-    bool found = false;
-    for (int i = 0; i < 6 && !found; ++i) {
-        const int wr = cand[i][0], nb = cand[i][1], rs = cand[i][2];
-        const size_t rq = wr / 4;
-        const size_t ops1 = 2 * ((size_t)p.m_blocks * rq * (p.a_rows * 16 + 16)) + 2 * (rq * (p.n_pad * 16 + 16));
-        const size_t raw1 = (size_t)wr * (p.k_pad4 + p.n_pad) * 4;
-        const size_t total = nb * ops1 + rs * raw1 + 4 * 8 + 16 + 2048;     // +2 KB: the a_rows=64 overrun stays inside
-        if (total <= 227 * 1024) {
-            p.w_rows = wr; p.nbuf = nb; p.raw_stages = rs; smem = total; found = true;
-        }
-    }
-    EMER_REQUIRE(found, "emer_linear_tc_bwd_weight: layer %dx%d does not fit shared memory", k, n_out);
-    static size_t configured_dev[64] = {0};          // the attribute is per device
-    size_t& configured = configured_dev[emer::current_device()];
-    if (smem > configured) {
-        cudaError_t e = cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) {
-            emer::set_error("emer_linear_tc_bwd_weight: cudaFuncSetAttribute(%zu): %s", smem, cudaGetErrorString(e));
-            return -2;
-        }
-        configured = smem;
-    }
-    const int64_t n_tiles = emer::ceil_div(n, p.w_rows);
-    int64_t grid = emer::sm_count();
-    // every CTA ends with n_out x k atomics onto the same addresses: with few tiles (the per-ray products, 8192 rows)
-    // one tile per CTA makes the flush the whole cost (79 us for 49 -> 128 over 8192 rows), so give a CTA >= 4 tiles
-    if (grid > emer::ceil_div(n_tiles, (int64_t)4)) grid = emer::ceil_div(n_tiles, (int64_t)4);
-    tc_wgrad_kernel<<<(unsigned)grid, WNT_ALL, smem, (cudaStream_t)stream>>>(p);
-    return emer::check_launch("emer_linear_tc_bwd_weight");
 }

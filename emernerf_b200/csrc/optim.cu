@@ -5,7 +5,7 @@
 // weight_decay 1e-5, betas (0.9, 0.99)), stepped twice per training iteration, train_emernerf.py:742-745,823-826):
 // optimizer.zero_grad() + tiny-cuda-nn's full-table gradient memset + the foreach / fused Adam launches.
 // The 122 MB hash table dominates: 4 streams read (param, grad, exp_avg, exp_avg_sq), 4 written (the same, grad := 0)
-// = 32 B per parameter -- HBM-bound, 0.15 ms for the static grid at the measured 6.58 TB/s.
+// = 32 B per parameter -- HBM-bound.
 //
 // Arithmetic of torch.optim.Adam (amsgrad = False, maximize = False), fp32 state:
 //     g  = grad + weight_decay * p

@@ -1,5 +1,10 @@
-// tcgen05 / TMEM / mbarrier / cp.async PTX wrappers shared by the tensor-core kernels of libemer_b200
-// (linear_tc.cu: one layer per launch; field_fused.cu: the fused field chain).  sm_100a only.
+// Warpgroup MMA (wgmma, sm_90a) helpers of the tensor-core kernels (linear_tc.cu, wgrad_mn.cu, field_fused.cu): 3xTF32
+// products (A_hi B_hi + A_lo B_hi + A_hi B_lo, fp32 accumulate), A from registers, B from shared memory, K-major without
+// swizzle: element (n, k) at (k/4)*PANEL + n*16 + (k%4)*4, PANEL = rows*16 (LBO = PANEL, SBO = 128 B).  DESIGN.md §5.
+//
+// Fragments (thread t: warp w = t/32, g = (t%32)/4, q = t%4; rows r0 = 16w + g, r1 = r0 + 8): accumulator d[4j + e] is
+// (r0 | r1 for e < 2 | >= 2, column 8j + 2q + (e & 1)); tf32 A is (r0, q), (r1, q), (r0, q + 4), (r1, q + 4).  Feeding
+// A position q with column 2q and q + 4 with 2q + 1 (kpos, B alike) makes one layer's accumulator the next one's A.
 #pragma once
 #include "common.cuh"
 
@@ -9,180 +14,111 @@ namespace tc {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
 }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    while (!mbar_try_wait(bar, parity)) {
-    }
-}
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_proxy() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, tf32 inputs, fp32 accumulate
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major, SWIZZLE_NONE shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4   [16,30) LBO>>4   [32,46) SBO>>4   [46,48) version=1   [61,64) layout=0
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): c=f32 (bit4), a=b=tf32 (2<<7, 2<<10),
-// K-major both, N>>3 at bit 17, M>>4 at bit 24
-__device__ __forceinline__ uint32_t make_idesc(int m, int n) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ float to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
-// x = hi + lo with hi, lo representable in tf32 (low 13 mantissa bits clear).  Truncation instead of
-// cvt.rna keeps the split on the full-rate integer/FP pipes (cvt is a quarter-rate conversion);
-// |x - hi - lo| <= 2^-20 |x|.
+// x = hi + lo with hi, lo representable in tf32 (low 13 mantissa bits clear).  Truncation instead of cvt.rna keeps the
+// split on the full-rate integer/FP pipes; |x - hi - lo| <= 2^-20 |x|.
 __device__ __forceinline__ void split(float x, float& hi, float& lo) {
     hi = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
     lo = __uint_as_float(__float_as_uint(x - hi) & 0xFFFFE000u);
 }
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, uint32_t src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src),
-                 "r"(src_bytes)
-                 : "memory");
+
+// position inside its 8-wide k step at which A and B hold reduction index k (see the fragment note above)
+__host__ __device__ constexpr int kpos(int k) { return (k & ~7) | (((k & 7) >> 1) + ((k & 1) << 2)); }
+// byte offset of B element (n, k) in panels of `rows` rows
+__host__ __device__ inline int b_off(int n, int k, int rows) {
+    const int p = kpos(k);
+    return (p >> 2) * rows * 16 + n * 16 + (p & 3) * 4;
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// shared-memory matrix descriptor, K-major, no swizzle: [0,14) start >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
+           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
+}
+// descriptor of k step ks, rows [n0, n0 + N) of a B operand at shared address `base` with `rows` rows per panel
+__device__ __forceinline__ uint64_t b_desc(uint32_t base, int rows, int ks, int n0) {
+    return make_desc(base + (uint32_t)(ks * 2 * rows * 16 + n0 * 16), (uint32_t)(rows * 16), 128u);
+}
+
+// A fragment of one k step from four values in accumulator order (r0, c), (r0, c + 1), (r1, c), (r1, c + 1)
+__device__ __forceinline__ void frag_split(float v0, float v1, float v2, float v3, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+    float h, l;
+    split(v0, h, l); hi[0] = __float_as_uint(h); lo[0] = __float_as_uint(l);
+    split(v2, h, l); hi[1] = __float_as_uint(h); lo[1] = __float_as_uint(l);
+    split(v1, h, l); hi[2] = __float_as_uint(h); lo[2] = __float_as_uint(l);
+    split(v3, h, l); hi[3] = __float_as_uint(h); lo[3] = __float_as_uint(l);
+}
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x N] (+)= A[64 x 8] (registers) * B[N x 8]^T (shared memory); acc = 0 overwrites D; d: N/2 accumulators
 template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-// 16 accumulator columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld16(uint32_t addr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(addr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(cols) : "memory");
-}
-
-// The lane of the issuer warp that issues the tcgen05.mma / tcgen05.commit instructions.
-//   1 (default): elect.sync, what CUTLASS's elect_one_sync does -- the descriptors live in uniform registers and the
-//     UTCHMMA are issued back to back.
-//   0: lane 0 by thread index.  The compiler cannot prove that a single lane is active, so every descriptor is treated
-//     as possibly divergent and each tcgen05.mma is wrapped in an ELECT / 4x R2UR.BROADCAST / BRA.U.ANY waterfall loop
-//     (cuobjdump -sass; profiles/r1_sass_mma_issue.md).  Measured A/B on B200 (round 2, same box, 120 steps): 4.07 ms
-//     per step with the waterfall, 3.95 ms with elect.sync, GPU parity tests green on both.
-#ifndef EMER_TC_ELECT_ONE
-#define EMER_TC_ELECT_ONE 1
-#endif
-__device__ __forceinline__ bool mma_issue_lane(int tid) {
-#if EMER_TC_ELECT_ONE
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-#else
-    return (tid & 31) == 0;
-#endif
-}
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// Arrival of a whole (converged) warp.  EMER_WARP_ARRIVE=1: the lanes synchronise and ONE lane arrives, so a barrier
-// fed by 256 threads sees 8 shared-memory atomics per phase instead of 256 on one word; the barrier is then initialised
-// with arrivals(threads).  Every lane must have executed its own fences (fence.proxy.async /
-// tcgen05.fence::before_thread_sync) before the call; __syncwarp orders them before the elected lane's release.
-// Measured A/B on one box (GPU suite green on both): step 2.603 ms with, 2.593 ms without, field_fwd 0.243 / 0.237 ms --
-// the 256 arrivals are not what the stage hand-off waits for.  Default: every thread arrives.
-#ifndef EMER_WARP_ARRIVE
-#define EMER_WARP_ARRIVE 0
-#endif
-__host__ __device__ constexpr int arrivals(int threads) { return EMER_WARP_ARRIVE ? threads / 32 : threads; }
-__device__ __forceinline__ void mbar_arrive_warp(uint64_t* bar) {
-#if EMER_WARP_ARRIVE
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
-#else
-    mbar_arrive(bar);
-#endif
+struct Wgmma;
+// the N of every product in this library (fused chain: 8, 32, 40, 64; per-layer blocks: 16 .. 64; weight gradients:
+// 16, 32, 64, 128)
+template <> struct Wgmma<8> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t (&a)[4], uint64_t b, int acc) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %9, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0, %1, %2, %3}, "
+            "{%4, %5, %6, %7}, %8, p, 1, 1;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+    }
+};
+template <> struct Wgmma<16> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t (&a)[4], uint64_t b, int acc) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, "
+            "{%8, %9, %10, %11}, %12, p, 1, 1;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+    }
+};
+template <> struct Wgmma<32> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t (&a)[4], uint64_t b, int acc) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+            "{%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+    }
+};
+template <> struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t (&a)[4], uint64_t b, int acc) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+            "{%32, %33, %34, %35}, %36, p, 1, 1;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+    }
+};
+// other N (40, 48, 128): the shapes above on consecutive 8-row groups of B (the descriptor's start moves n0 rows)
+template <int N>
+__device__ __forceinline__ void mma_n(float* d, const uint32_t (&a)[4], uint64_t b, int acc) {
+    if constexpr (N == 8 || N == 16 || N == 32 || N == 64) {
+        Wgmma<N>::mma(d, a, b, acc);
+    } else {
+        constexpr int N0 = N > 64 ? 64 : (N > 32 ? 32 : 16);
+        mma_n<N0>(d, a, b, acc);
+        mma_n<N - N0>(d + N0 / 2, a, b + (uint64_t)N0, acc);     // + N0 rows of 16 B in the start field (>> 4)
+    }
 }
 
-// ---- operand A from TENSOR MEMORY (the ".ts" form): D[tmem] (+)= A[tmem] * B[smem]^T.  A is [128 lanes x K columns]
-// of 32-bit tf32 containers: lane = row, column = k; 8 columns per instruction.
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 16 / 8 columns of this thread's TMEM lane <- registers
-__device__ __forceinline__ void tmem_st16(uint32_t addr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-          "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t addr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld4(uint32_t addr, uint32_t (&r)[4]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-                 : "r"(addr)
-                 : "memory");
+// one 3xTF32 k step: D += A_hi B_hi + A_lo B_hi + A_hi B_lo (acc = 0: D = ... on the first product)
+template <int N>
+__device__ __forceinline__ void mma3(float (&d)[N / 2], const uint32_t (&ahi)[4], const uint32_t (&alo)[4], uint64_t bhi,
+                                     uint64_t blo, int acc) {
+    mma_n<N>(d, ahi, bhi, acc);
+    mma_n<N>(d, alo, bhi, 1);
+    mma_n<N>(d, ahi, blo, 1);
 }
 
 }  // namespace tc

@@ -1,274 +1,161 @@
-// Weight gradient dW^T[k, 64] += X^T dZ, db += column sums of dZ, with the operands used AS THEY LIE IN MEMORY.
-//
-// The reduction of a weight gradient runs over the ROWS, so in their natural row-major layout both operands are
-// "MN-major" for the tensor core (consecutive memory runs along the feature index).  tc_wgrad_kernel (linear_tc.cu) only
-// had K-major operands and transposed while staging -- 4 rows x 1 feature gathers, ~40 instructions per staged element,
-// instruction-bound at a third of the HBM roofline (profiles/r1_prof_wgrad_summary.md).  tools/mn_probe.cu established on
-// the B200 that tcgen05.mma.kind::tf32 takes MN-major shared-memory operands in the SWIZZLE_128B_BASE32B canonical layout
-// (cute's Layout_MN_SW128_32B_Atom: 4-row atoms of 128-byte rows = 32 features, 32-byte chunks XOR-ed with row % 4;
-// LBO = stride between 32-feature blocks, SBO = stride between 4-row atoms) -- and NOT in plain SWIZZLE_128B or without
-// swizzle (both return zeros).  So here
-//   * cp.async drops every 16-byte piece of a raw fp32 row straight at its swizzled place,
-//   * the thread that copied a piece splits it into tf32 hi (in place) and lo (twin buffer): elementwise, 16 bytes at a
-//     time, no transposition, ~4 instructions per element,
-//   * one warp issues 3 tcgen05.mma per 8 rows (A = X^T, B = dZ^T, both MN-major) into ONE persistent TMEM accumulator
-//     per CTA, flushed once with coalesced atomics.
-// HBM-bound: (k + 64) * 4 B per row.
+// Weight gradients  dW[n_out, k] += dZ^T X,  db += column sums of dZ,  on Hopper warpgroup MMA (3xTF32, tc_common.cuh).
+// Entry points: emer_linear_tc_bwd_weight (any n_out <= 128, k <= 256) and emer_linear_tc_bwd_weight_mn (the 64-wide
+// layers of the field chain, read as they lie in memory: row-major X and dZ); both run wgrad_kernel.
+// D[k x n_out] = X^T dZ: A = X^T straight from the row-major X (the 8 lanes with the same q read one 32-byte sector of
+// a row), B = dZ^T staged per tile into K-major panels; D stays in registers across the persistent CTA's tiles and is
+// flushed once with atomics (DESIGN.md §5.3).  HBM-bound: (k + n_out) * 4 B per row.
 #include "common.cuh"
 #include "tc_common.cuh"
 
-#ifndef EMER_MN_LAYOUT
-#define EMER_MN_LAYOUT 1          // 1: SWIZZLE_128B_BASE32B -- the one that works for tf32 (tools/mn_probe.cu); 2: SWIZZLE_128B
-#endif
-
 namespace emer {
-namespace wmn {
+namespace wg {
 
 using namespace emer::tc;
 
-constexpr int NCONV = 256;               // converter threads
-constexpr int NTHREADS = NCONV + 32;     // + the MMA-issuing warp
-constexpr int NOUT = 64;
-
-// byte offset of element (mn, row) of a tile with MB 32-wide feature blocks.
-//   LAYOUT 2 = SWIZZLE_128B:         8-row atoms of 1024 B, 16-byte chunks ^ (row % 8)
-//   LAYOUT 1 = SWIZZLE_128B_BASE32B: 4-row atoms of  512 B, 32-byte chunks ^ (row % 4)
-template <int LAYOUT>
-__device__ __forceinline__ int piece_off(int chunk16, int row, int MB) {     // chunk16: 16-byte piece index along the row
-    const int blk = chunk16 >> 3, c = chunk16 & 7;
-    if (LAYOUT == 2) return (row >> 3) * (MB * 1024) + blk * 1024 + (row & 7) * 128 + ((c ^ (row & 7)) << 4);
-    return (row >> 2) * (MB * 512) + blk * 512 + (row & 3) * 128 + ((((c >> 1) ^ (row & 3)) << 5) | ((c & 1) << 4));
-}
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t addr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
-    uint64_t d = 0;
-    d |= (uint64_t)((addr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)layout << 61;
-    return d;
-}
+constexpr int TR = 32;                       // rows per tile = 4 k steps
+constexpr int MIN_TILES = 4;
 
 struct Params {
-    const float* x; int64_t ldx; int k;       // [n, k]
-    const float* dz; int64_t lddz;            // [n, 64]
-    float* dw;                                // [64, k] row-major, accumulated
-    float* db;                                // [64] or null, accumulated
+    const float* x; int64_t ldx; int k;       // [n, ldx]
+    const float* dz; int64_t lddz; int n_out; // [n, lddz]
+    float* dw;                                // [n_out, k] row-major, accumulated
+    float* db;                                // [n_out] accumulated, or null
     int64_t n;
 };
 
-// TILE rows per pipeline stage (TILE / 8 k-steps of 8 rows).  Per tile a converter thread: waits for its own cp.async
-// pieces, splits them, arrives on full[stage] -- and only THEN waits for the MMAs of the previous tile to retire and
-// refills that tile's stage, so the split of tile t runs while the tensor pipe works on tile t - 1 (the first version
-// waited for the MMAs before splitting: split and MMA alternated, 110 us for 268 MB, profiles/r2_chain_ncu_summary.md).
-// Loads run STAGES - 1 tiles ahead of the split.
-template <int KXP, int LAYOUT, int STAGES, int TILE>
-__global__ void __launch_bounds__(NTHREADS, 1) wgrad_mn_kernel(const Params p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    constexpr int MBA = KXP / 32, MBB = NOUT / 32;
-    constexpr int A_BYTES = TILE * KXP * 4, B_BYTES = TILE * NOUT * 4;
-    constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;          // [A_hi | A_lo | B_hi | B_lo]
-    constexpr int ATOM_ROWS = LAYOUT == 2 ? 8 : 4;
-    constexpr int A_SBO = MBA * (ATOM_ROWS * 128), B_SBO = MBB * (ATOM_ROWS * 128), LBO = ATOM_ROWS * 128;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-    uint64_t* full_bar = bars;                 // [STAGES]
-    uint64_t* empty_bar = bars + STAGES;       // [STAGES]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES);
-    float* red = reinterpret_cast<float*>(bars + 2 * STAGES + 2);   // [NCONV * 4] bias partial sums (16-byte aligned:
-                                                                    // (2 STAGES + 2) * 8 is a multiple of 16)
+// NP: n_out padded to a power of two in [16, 128], so that every thread stages one fixed column (blockDim % NP == 0);
+// MB: warpgroups = 64-feature blocks of X in the CTA
+template <int NP, int MB>
+__global__ void __launch_bounds__(128 * MB) wgrad_kernel(const Params p) {
+    constexpr int NT = 128 * MB, PER = (TR * NP + NT - 1) / NT;      // dZ values a thread stages per tile (at most)
+    __shared__ __align__(128) uint8_t smem[2 * TR * NP * 4];
+    uint8_t* b_hi = smem;
+    uint8_t* b_lo = smem + TR * NP * 4;
+    const int tid = threadIdx.x;
+    const int wgi = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+    const int f0 = wgi * 64 + 16 * w + (lane >> 2), f1 = f0 + 8;    // this thread's two features (A rows)
+    const bool fok0 = f0 < p.k, fok1 = f1 < p.k;
+    const int o_st = tid % NP;                                       // the column this thread stages
+    const uint32_t bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+    const int64_t n_tiles = (p.n + TR - 1) / TR;
 
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const bool is_issuer = warp == NCONV / 32;
-    if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], arrivals(NCONV)); mbar_init(&empty_bar[s], 1); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    float xr[TR / 8][4], zr[PER];
+    auto load = [&](int64_t tile) {
+        const int64_t r_base = tile * TR;
+#pragma unroll
+        for (int ks = 0; ks < TR / 8; ++ks) {
+            const int64_t ra = r_base + 8 * ks + 2 * q, rb = ra + 1;
+            const bool oka = ra < p.n, okb = rb < p.n;
+            xr[ks][0] = (oka && fok0) ? __ldg(p.x + ra * p.ldx + f0) : 0.0f;
+            xr[ks][1] = (okb && fok0) ? __ldg(p.x + rb * p.ldx + f0) : 0.0f;
+            xr[ks][2] = (oka && fok1) ? __ldg(p.x + ra * p.ldx + f1) : 0.0f;
+            xr[ks][3] = (okb && fok1) ? __ldg(p.x + rb * p.ldx + f1) : 0.0f;
+        }
+#pragma unroll
+        for (int i = 0; i < PER; ++i) {
+            const int e = tid + i * NT;                                  // (o_st, e / NP) of the tile
+            const int64_t row = r_base + e / NP;
+            zr[i] = (e < TR * NP && row < p.n && o_st < p.n_out) ? __ldg(p.dz + row * p.lddz + o_st) : 0.0f;
+        }
+    };
+
+    float acc[NP / 2];
+#pragma unroll
+    for (int i = 0; i < NP / 2; ++i) acc[i] = 0.0f;
+    float dbp = 0.0f;
+    load(blockIdx.x);
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        __syncthreads();                      // the previous tile's MMAs have finished reading B
+#pragma unroll
+        for (int i = 0; i < PER; ++i) {
+            const int e = tid + i * NT;
+            if (e < TR * NP) {
+                dbp += zr[i];
+                float h, l;
+                split(zr[i], h, l);
+                const int off = b_off(o_st, e / NP, NP);
+                *reinterpret_cast<float*>(b_hi + off) = h;
+                *reinterpret_cast<float*>(b_lo + off) = l;
+            }
+        }
+        fence_async_proxy();
+        __syncthreads();
+        uint32_t ahi[TR / 8][4], alo[TR / 8][4];
+#pragma unroll
+        for (int ks = 0; ks < TR / 8; ++ks) frag_split(xr[ks][0], xr[ks][1], xr[ks][2], xr[ks][3], ahi[ks], alo[ks]);
+        load(tile + gridDim.x);               // the next tile's values arrive under this tile's MMAs
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < TR / 8; ++ks) mma3<NP>(acc, ahi[ks], alo[ks], b_desc(bh, NP, ks, 0), b_desc(bl, NP, ks, 0), 1);
+        wg_commit();
+        wg_wait0();
     }
-    if (warp == 0) {
-        __syncwarp();
-        tmem_alloc(tmem_slot, 64u);
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    const int64_t n_tiles = (p.n + TILE - 1) / TILE;
-    const int my_tiles = (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
-
-    if (is_issuer) {
-        const uint32_t idesc = make_idesc(128, NOUT) | (1u << 15) | (1u << 16);       // A and B MN-major
-        const uint32_t sbase = smem_u32(smem);
-        int s = 0;
-        uint32_t par = 0;                          // stage and parity of tile t: t % STAGES, (t / STAGES) & 1
-        for (int t = 0; t < my_tiles; ++t) {
-            mbar_wait(&full_bar[s], par);
-            tc_fence_after();
-            if (mma_issue_lane(tid)) {
-                const uint32_t a_hi = sbase + s * STAGE_BYTES, a_lo = a_hi + A_BYTES, b_hi = a_lo + A_BYTES, b_lo = b_hi + B_BYTES;
+    // flush: D[f][o] -> dW[o, f]
 #pragma unroll
-                for (int ks = 0; ks < TILE / 8; ++ks) {
-                    const uint32_t ao = ks * (8 / ATOM_ROWS) * A_SBO, bo = ks * (8 / ATOM_ROWS) * B_SBO;
-                    const uint64_t da_hi = make_desc_mn(a_hi + ao, LBO, A_SBO, LAYOUT), da_lo = make_desc_mn(a_lo + ao, LBO, A_SBO, LAYOUT);
-                    const uint64_t db_hi = make_desc_mn(b_hi + bo, LBO, B_SBO, LAYOUT), db_lo = make_desc_mn(b_lo + bo, LBO, B_SBO, LAYOUT);
-                    mma_tf32(tmem_base, da_hi, db_hi, idesc, (t > 0 || ks > 0) ? 1u : 0u);
-                    mma_tf32(tmem_base, da_lo, db_hi, idesc, 1u);
-                    mma_tf32(tmem_base, da_hi, db_lo, idesc, 1u);
-                }
-                tc_commit(&empty_bar[s]);
-            }
-            __syncwarp();
-            if (++s == STAGES) { s = 0; par ^= 1u; }
-        }
-    } else {
-        constexpr int XQ = KXP / 4, ZQ = NOUT / 4;                   // 16-byte pieces per row
-        constexpr int XP = TILE * XQ / NCONV, ZP = TILE * ZQ / NCONV; // pieces per thread per tile
-        constexpr int XR = NCONV / XQ, ZR = NCONV / ZQ;               // rows between two pieces of one thread
-        static_assert(XP >= 1 && ZP >= 1 && XR % ATOM_ROWS == 0 && ZR % ATOM_ROWS == 0, "tile too small for 256 converters");
-        // a thread's pieces sit in one column of 16 bytes, XR (ZR) rows apart: whole swizzle atoms apart, so their
-        // shared-memory offsets differ by a constant
-        constexpr int XSTEP = (XR / ATOM_ROWS) * A_SBO, ZSTEP = (ZR / ATOM_ROWS) * B_SBO;
-        const int xr0 = tid / XQ, xc = tid % XQ, zr0 = tid / ZQ, zc = tid % ZQ;
-        const int xoff0 = piece_off<LAYOUT>(xc, xr0, MBA), zoff0 = piece_off<LAYOUT>(zc, zr0, MBB);
-        const bool x_col_ok = xc < (p.k + 3) / 4;
-        const float* xsrc = p.x + xc * 4;
-        const float* zsrc = p.dz + zc * 4;
-        auto issue = [&](int t, int s) {
-            const int64_t row0 = ((int64_t)blockIdx.x + (int64_t)t * gridDim.x) * TILE;
-            uint8_t* a_hi = smem + s * STAGE_BYTES + xoff0;
-            uint8_t* b_hi = smem + s * STAGE_BYTES + 2 * A_BYTES + zoff0;
+    for (int j = 0; j < NP / 8; ++j) {
 #pragma unroll
-            for (int i = 0; i < XP; ++i) {
-                const int64_t row = row0 + xr0 + i * XR;
-                const bool ok = x_col_ok && row < p.n;
-                cp_async16(a_hi + i * XSTEP, ok ? xsrc + row * p.ldx : p.x, ok ? 16u : 0u);
-            }
-#pragma unroll
-            for (int i = 0; i < ZP; ++i) {
-                const int64_t row = row0 + zr0 + i * ZR;
-                const bool ok = row < p.n;
-                cp_async16(b_hi + i * ZSTEP, ok ? zsrc + row * p.lddz : p.dz, ok ? 16u : 0u);
-            }
-        };
-#pragma unroll
-        for (int t = 0; t < STAGES - 1; ++t) {
-            if (t < my_tiles) issue(t, t);
-            cp_async_commit();
-        }
-        float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
-        int s = 0, sn = STAGES - 1;                  // stages of tile t and of tile t + STAGES - 1
-        uint32_t epar = 1;                           // parity of the empty-barrier phase tile t + STAGES - 1 waits for:
-                                                     // use (tn / STAGES) - 1 of its stage, first needed at tn = STAGES
-        for (int t = 0; t < my_tiles; ++t) {
-            cp_async_wait<STAGES - 2>();                     // this thread's pieces of tile t have landed
-            uint8_t* a_hi = smem + s * STAGE_BYTES + xoff0;
-            uint8_t* b_hi = smem + s * STAGE_BYTES + 2 * A_BYTES + zoff0;
-#pragma unroll
-            for (int i = 0; i < XP; ++i) {
-                float4* ph = reinterpret_cast<float4*>(a_hi + i * XSTEP);
-                const float4 v = *ph;
-                float4 h, l;
-                split(v.x, h.x, l.x); split(v.y, h.y, l.y); split(v.z, h.z, l.z); split(v.w, h.w, l.w);
-                *ph = h;
-                *reinterpret_cast<float4*>(a_hi + i * XSTEP + A_BYTES) = l;
-            }
-#pragma unroll
-            for (int i = 0; i < ZP; ++i) {
-                float4* ph = reinterpret_cast<float4*>(b_hi + i * ZSTEP);
-                const float4 v = *ph;
-                bsum.x += v.x; bsum.y += v.y; bsum.z += v.z; bsum.w += v.w;     // (column zc for every i)
-                float4 h, l;
-                split(v.x, h.x, l.x); split(v.y, h.y, l.y); split(v.z, h.z, l.z); split(v.w, h.w, l.w);
-                *ph = h;
-                *reinterpret_cast<float4*>(b_hi + i * ZSTEP + B_BYTES) = l;
-            }
-            fence_async_proxy();
-            mbar_arrive_warp(&full_bar[s]);
-            // refill the stage tile t - 1 used with tile t + STAGES - 1: the MMAs of t - 1 had this tile's split to retire
-            const int tn = t + STAGES - 1;
-            if (tn < my_tiles) {
-                if (tn >= STAGES) mbar_wait(&empty_bar[sn], epar);
-                issue(tn, sn);
-            }
-            cp_async_commit();
-            if (++s == STAGES) s = 0;
-            if (++sn == STAGES) { sn = 0; epar ^= 1u; }
-        }
-        cp_async_wait<0>();
-        // ---- flush: wait for the last tile's MMAs, then lane f of the accumulator holds dW^T[f, 0..63]
-        if (my_tiles > 0) {
-            const int sl = (my_tiles - 1) % STAGES;
-            // the last use of stage sl: its commit is the (number of uses)-th completion of empty_bar[sl]
-            const int uses = (my_tiles - 1) / STAGES + 1;
-            mbar_wait(&empty_bar[sl], (uint32_t)((uses - 1) & 1));
-            tc_fence_after();
-            if (warp < 4) {
-                const int f = warp * 32 + (tid & 31);
-                const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-#pragma unroll
-                for (int c0 = 0; c0 < NOUT; c0 += 16) {
-                    uint32_t r[16];
-                    tmem_ld16(lane_addr + (uint32_t)c0, r);
-                    tmem_ld_wait();
-                    if (f < p.k) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) atomicAdd(p.dw + (int64_t)(c0 + j) * p.k + f, __uint_as_float(r[j]));
-                    }
-                }
-            }
-            if (p.db) {
-                reinterpret_cast<float4*>(red)[tid] = bsum;
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (tid < NOUT) {
-                    // column o = 4 (t % 16) + j: threads t = o / 4 + 16 m
-                    float acc = 0.0f;
-                    for (int m = 0; m < NCONV / 16; ++m) acc += red[((tid >> 2) + 16 * m) * 4 + (tid & 3)];
-                    atomicAdd(p.db + tid, acc);
-                }
-            }
+        for (int e = 0; e < 4; ++e) {
+            const int f = e < 2 ? f0 : f1, o = 8 * j + 2 * q + (e & 1);
+            if ((e < 2 ? fok0 : fok1) && o < p.n_out) atomicAdd(p.dw + (int64_t)o * p.k + f, acc[4 * j + e]);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, 64u);
+    if (p.db && o_st < p.n_out) atomicAdd(p.db + o_st, dbp);
 }
 
-}  // namespace wmn
+template <int NP, int MB>
+static int launch_t(const Params& p, cudaStream_t st, const char* what) {
+    // persistent grid of the CTAs resident at once, with at least MIN_TILES tiles each (every CTA ends with k x n_out
+    // atomics onto the same dW addresses, which would dominate small products such as the 8192-row per-ray ones)
+    static int cache[64] = {0};
+    int64_t grid = (int64_t)sm_count() * resident_ctas(wgrad_kernel<NP, MB>, 128 * MB, 0, st, cache);
+    const int64_t ctas = ceil_div(ceil_div(p.n, TR), MIN_TILES);
+    if (grid > ctas) grid = ctas;
+    wgrad_kernel<NP, MB><<<(unsigned)grid, 128 * MB, 0, st>>>(p);
+    return check_launch(what);
+}
+
+template <int NP>
+static int launch_np(const Params& p, cudaStream_t st, const char* what) {
+    switch ((p.k + 63) / 64) {
+        case 1: return launch_t<NP, 1>(p, st, what);
+        case 2: return launch_t<NP, 2>(p, st, what);
+        case 3: return launch_t<NP, 3>(p, st, what);
+        default: return launch_t<NP, 4>(p, st, what);
+    }
+}
+
+static int launch(const Params& p, cudaStream_t st, const char* what) {
+    if (p.n_out <= 16) return launch_np<16>(p, st, what);
+    if (p.n_out <= 32) return launch_np<32>(p, st, what);
+    if (p.n_out <= 64) return launch_np<64>(p, st, what);
+    return launch_np<128>(p, st, what);
+}
+
+}  // namespace wg
 }  // namespace emer
 
-using namespace emer;
+extern "C" int emer_linear_tc_bwd_weight(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw,
+                                         float* db, int64_t n, int k, int n_out, void* stream) {
+    if (n == 0) return 0;
+    EMER_REQUIRE(x && dz && dw, "emer_linear_tc_bwd_weight: NULL pointer");
+    EMER_REQUIRE(n_out <= 128 && k <= 256, "emer_linear_tc_bwd_weight: widths k=%d n_out=%d out of range", k, n_out);
+    EMER_REQUIRE(ldx % 4 == 0 && lddz % 4 == 0 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)dz & 15) == 0,
+                 "emer_linear_tc_bwd_weight: rows must be 16-byte aligned (ldx=%lld lddz=%lld)", (long long)ldx,
+                 (long long)lddz);
+    EMER_REQUIRE((k + 3) / 4 * 4 <= ldx, "emer_linear_tc_bwd_weight: row stride %lld shorter than padded width %d",
+                 (long long)ldx, (k + 3) / 4 * 4);
+    EMER_REQUIRE((n_out + 3) / 4 * 4 <= lddz, "emer_linear_tc_bwd_weight: dZ rows too short");
+    emer::wg::Params p{x, ldx, k, dz, lddz, n_out, dw, db, n};
+    return emer::wg::launch(p, (cudaStream_t)stream, "emer_linear_tc_bwd_weight");
+}
 
 extern "C" int emer_linear_tc_bwd_weight_mn(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw, float* db,
                                             int64_t n, int k, int n_out, void* stream) {
-    using namespace emer::wmn;
     if (n == 0) return 0;
     EMER_REQUIRE(x && dz && dw, "emer_linear_tc_bwd_weight_mn: NULL pointer");
-    EMER_REQUIRE(n_out == NOUT && k >= 4 && k <= 128, "emer_linear_tc_bwd_weight_mn: shape k=%d n_out=%d (need n_out = 64, k <= 128)", k, n_out);
+    EMER_REQUIRE(n_out == 64 && k >= 4 && k <= 128, "emer_linear_tc_bwd_weight_mn: shape k=%d n_out=%d (need n_out = 64, k <= 128)", k, n_out);
     EMER_REQUIRE(ldx % 4 == 0 && lddz % 4 == 0 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)dz & 15) == 0 && (k + 3) / 4 * 4 <= ldx,
                  "emer_linear_tc_bwd_weight_mn: rows must be 16-byte aligned");
-    Params p{x, ldx, k, dz, lddz, dw, db, n};
-    constexpr int TILE = 32;
-    const int64_t n_tiles = ceil_div(n, TILE);
-    int64_t grid = sm_count();
-    if (grid > n_tiles) grid = n_tiles;
-    auto launch = [&](auto kernel, size_t smem, size_t& configured) -> int {
-        if (smem > configured) {
-            cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) {
-                set_error("emer_linear_tc_bwd_weight_mn: cudaFuncSetAttribute(%zu): %s", smem, cudaGetErrorString(e));
-                return -2;
-            }
-            configured = smem;
-        }
-        kernel<<<(unsigned)grid, NTHREADS, smem, (cudaStream_t)stream>>>(p);
-        return 0;
-    };
-    static size_t configured_dev[2][64] = {{0}};
-    const int dev = current_device();
-    constexpr int LAYOUT = EMER_MN_LAYOUT;
-    int rc;
-    // 192 KB of stages either way: 6 x 32 KB (k <= 64) or 4 x 48 KB, + barriers and the bias scratch
-    if (k <= 64) rc = launch(wgrad_mn_kernel<64, LAYOUT, 6, TILE>, 6 * (4 * TILE * 64 * 4) + 4096 + 1024, configured_dev[0][dev]);
-    else rc = launch(wgrad_mn_kernel<128, LAYOUT, 4, TILE>, 4 * (2 * TILE * 128 * 4 + 2 * TILE * 64 * 4) + 4096 + 1024, configured_dev[1][dev]);
-    if (rc) return rc;
-    return check_launch("emer_linear_tc_bwd_weight_mn");
+    emer::wg::Params p{x, ldx, k, dz, lddz, n_out, dw, db, n};
+    return emer::wg::launch(p, (cudaStream_t)stream, "emer_linear_tc_bwd_weight_mn");
 }

@@ -1,5 +1,5 @@
 """Position / direction encoders with the reference's class names and constructor arguments
-(radiance_fields/encodings.py of NVlabs/EmerNeRF), backed by the sm_100a hash-grid kernels."""
+(radiance_fields/encodings.py of NVlabs/EmerNeRF), backed by the sm_90a hash-grid kernels."""
 from __future__ import annotations
 
 import json

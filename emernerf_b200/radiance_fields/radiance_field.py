@@ -1,6 +1,6 @@
 """``RadianceField`` / ``DensityField`` with the reference's constructor arguments, attribute names,
 state-dict keys and ``forward`` contracts (radiance_fields/radiance_field.py of NVlabs/EmerNeRF),
-evaluated on the sm_100a kernels of libemer_b200.so:
+evaluated on the sm_90a kernels of libemer_b200.so:
 
   contract + selector  -> emer_contract_*      (radiance_field.py:278-300,828-835)
   hash grids           -> emer_grid_*          (:314,341,376,836)
@@ -333,7 +333,7 @@ class RadianceField(nn.Module):
         _ops.join_before_field()               # (multi-GPU: a parameter all-gather may still be running beside the sampling)
         G, S = self.geometry_feature_dim, self.semantic_feature_dim
         tail = None if (return_density_only or positions.dim() != 3) else self._tail_inputs(directions, data_dict)
-        # the fused chain (base MLP + density + colour head in one tcgen05 kernel) when the model has its shape
+        # the fused chain (base MLP + density + colour head in one wgmma kernel) when the model has its shape
         chain = tail is not None and self._chain_usable(self.xyz_encoder, self.base_mlp)
         rgb_in_static = static_rgb = None
         if chain:

@@ -1,5 +1,5 @@
 """``render_rays`` / ``rendering`` with the reference's signatures and output dictionaries
-(radiance_fields/render_utils.py of NVlabs/EmerNeRF), on the sm_100a kernels:
+(radiance_fields/render_utils.py of NVlabs/EmerNeRF), on the sm_90a kernels:
 
   transmittance / alpha / weights / opacity / depth / median depth -> emer_composite_fwd/bwd
   every accumulate_along_rays                                      -> emer_accumulate_fwd/bwd

@@ -1,5 +1,5 @@
 /*
- * emer_b200 -- C ABI of the B200-native EmerNeRF hot path (libemer_b200.so, sm_100a only).
+ * emer_b200 -- C ABI of the H100-native EmerNeRF hot path (libemer_b200.so, sm_90a only).
  *
  * This is the drop-in boundary.  The reference reaches its native code through two Python
  * FFIs: the tiny-cuda-nn pybind object (third_party/tcnn_modules.py:102,122,161,216-219) and
@@ -104,8 +104,8 @@ int emer_linear_narrow_bwd_data(const float* dz, int64_t lddz, const float* w, f
 int emer_linear_narrow_bwd_weight(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw,
                                   float* db, int64_t n, int k, int n_out, void* stream);
 
-/* Same contracts on the tcgen05 tensor cores: fp32 operands split into tf32 hi+lo, three
- * tcgen05.mma.kind::tf32 per k-step accumulate A_lo*B_hi + A_hi*B_lo + A_hi*B_hi in TMEM
+/* Same contracts on the tensor cores: fp32 operands split into tf32 hi+lo, three
+ * wgmma.mma_async ...tf32 per k-step accumulate A_hi*B_hi + A_lo*B_hi + A_hi*B_lo in registers
  * (fp32-accurate "3xTF32"; see emernerf_b200/csrc/linear_tc.cu).  Widths: k, n_out <= 256. */
 int emer_linear_tc_fwd(const float* x, int64_t ldx, const float* w, const float* b, float* y,
                        int64_t ldy, int64_t n, int k, int n_out, int act, void* stream);
@@ -116,7 +116,7 @@ int emer_linear_tc_bwd_data(const float* dy, int64_t lddy, const float* y, int64
 /* relu_src (may be NULL): the layer's input when that input is itself a ReLU output; the epilogue
  * then writes dX[:, :relu_cols] * (relu_src > 0), i.e. the dZ of the layer below (fused mask). */
 /* dW[n_out, k] += dZ^T X, db += column sums of dZ (dZ = dY * act'(Y) supplied by the caller).
- * dW^T accumulates in TMEM across each CTA's row tiles, flushed once with atomics.
+ * dW^T accumulates in registers across each CTA's row tiles, flushed once with atomics (csrc/wgrad_mn.cu).
  * Needs 16-byte aligned rows (ldx, lddz multiples of 4); k <= 256, n_out <= 128. */
 int emer_linear_tc_bwd_weight(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw,
                               float* db, int64_t n, int k, int n_out, void* stream);
@@ -181,17 +181,17 @@ int emer_field_tail_bwd(const float* feats, int64_t ld_feats, float* d_out, int6
                         const float* d_sigma, const int64_t* idx, float* d_emb, int e_dim, int64_t n_rays,
                         int n_samples, void* stream);
 
-/* Same contract as emer_linear_tc_bwd_weight for n_out == 64, k <= 128 (csrc/wgrad_mn.cu): the operands are used as they
- * lie in memory (MN-major, 128-byte swizzle with 32-byte base) instead of being transposed while staging. */
+/* Same contract and kernel as emer_linear_tc_bwd_weight, for the field chain's layers: n_out == 64, k <= 128
+ * (csrc/wgrad_mn.cu). */
 int emer_linear_tc_bwd_weight_mn(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw, float* db,
                                  int64_t n, int k, int n_out, void* stream);
 
-/* ---- the fused field chain (csrc/field_fused.cu): base MLP -> density + colour head in ONE tcgen05 kernel with the
- *      activations in tensor memory.  Replaces the chain of nn.Linear / torch.cat / trunc_exp / sigmoid calls of
+/* ---- the fused field chain (csrc/field_fused.cu): base MLP -> density + colour head in ONE wgmma kernel with the
+ *      activations in registers.  Replaces the chain of nn.Linear / torch.cat / trunc_exp / sigmoid calls of
  *      radiance_fields/radiance_field.py:74-80,314-318 (base_mlp), :422 (density), :131-143,622-658 (query_rgb) and
  *      radiance_fields/mlp.py:38-46 for one block of hash-grid features.
- *   enc[N, k_enc] (k_enc = 32, 40 or 64; rows 32-byte aligned: ld_enc % 8 == 0 -- the kernel moves rows 256 bits at a time,
- *   and so must be the save buffers)
+ *   enc[N, k_enc] (k_enc = 32, 40 or 64; rows 32-byte aligned: ld_enc % 8 == 0, and so must be the save
+ *   buffers)
  *   feats = relu(enc wb0^T + bb0) wb1^T + bb1        wb0 [64, k_enc], wb1 [n_feat, 64], n_feat = 64 | 128
  *   sigma[n] = exp(feats[n, 0] - 1)
  *   h0 = relu(geo w0g^T + ray_bias[ray, 0:64]),  h1 = relu(h0 w1h^T + geo w1g^T + ray_bias[ray, 64:128]),
@@ -209,7 +209,7 @@ int emer_field_fwd(const float* enc, int64_t ld_enc, int k_enc, const float* wb0
                    float* save_h1, float* save_sem, int64_t n, void* stream);
 
 /* Backward of emer_field_fwd, data path (the autograd graph of the same reference lines), one kernel, every
- * intermediate gradient in tensor memory:
+ * intermediate gradient in registers:
  *   dz2[N,3] = d_rgb * rgb (1 - rgb);  dz1[N,64] = (dz2 w2) * (h1 > 0);
  *   d1[N,128] = [dz0 | dF]: dz0 = (dz1 w1h) * (h0 > 0), dF = dz1 w1g + dz0 w0g + d_geo, dF[:,0] += d_sigma * min(sigma, e^15)
  *   dzb[N,64] = (dF wb1[:64] + d_sem wb1[64:]) * (hb > 0);  d_enc[N, k_enc] = dzb wb0   (row stride ld_denc)

@@ -11,7 +11,7 @@ What is restated here and how it is pinned
   (``radiance_fields/{radiance_field,render_utils,encodings,mlp,nerf_utils}.py``
   and ``third_party/nerfacc_prop_net.py`` at NVlabs/EmerNeRF@8c051d7) as plain
   functions over a state-dict.  It is PINNED: ``tests/golden/make_golden.py``
-  imports the reference's own modules from ``/root/reference`` (with the three
+  imports the reference's own modules from a checkout (``EMER_REFERENCE_ROOT``; with the three
   stand-in modules of ``oracle.ref_shims`` injected), runs them, and commits the
   results under ``tests/golden/``; ``tests/test_oracle_golden.py`` checks this
   restatement against those vectors.
@@ -21,8 +21,8 @@ What is restated here and how it is pinned
   *unpinned from master* by the reference, README.md:51) and
   ``oracle.nerfacc_ref`` restates the seven nerfacc symbols the path uses
   (nerfacc pinned at 8340e19daad4bafe24125150a8c56161838086fa, README.md:50).
-  Neither library's source is under ``/root/reference`` and neither can be
-  installed here.  **Parity unpinned** for these two: the only published
+  Neither library's source is in the reference tree, and neither is
+  installed in the build environment.  **Parity unpinned** for these two: the only published
   known-answer vector available offline is the ``importance_sampling``
   docstring example of nerfacc (checked in ``tests/test_oracle_nerfacc.py``);
   everything else is anchored on the reference's call sites.

@@ -1,11 +1,11 @@
 """CPU restatement of EmerNeRF's per-ray-batch hot path as plain functions over a state-dict.
 
-TEST INFRASTRUCTURE -- see ``oracle/__init__.py``.  This file travels to the GPU
-box (``/root/reference`` does not) and is what the ``-m gpu`` parity tests, the
-``smoke()`` check and the ``cpu_baseline`` leg of ``bench.py`` run.
+TEST INFRASTRUCTURE -- see ``oracle/__init__.py``.  Self-contained (the reference
+is not needed to run it): it is what the ``-m gpu`` parity tests, the ``smoke()``
+check and the ``cpu_baseline`` leg of ``bench.py`` run.
 
 PINNED against the reference's own Python: ``tests/golden/make_golden.py`` runs
-the unmodified ``/root/reference`` modules (with ``oracle.ref_shims``) and
+the unmodified reference modules (with ``oracle.ref_shims``) and
 ``tests/test_oracle_golden.py`` compares this restatement with the committed
 vectors.  The hash-grid / nerfacc arithmetic underneath comes from
 ``oracle.tcnn_ref`` / ``oracle.nerfacc_ref`` (parity unpinned, see there).

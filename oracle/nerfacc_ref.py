@@ -2,8 +2,8 @@
 
 TEST INFRASTRUCTURE -- see ``oracle/__init__.py``.  **Parity unpinned** except for
 the ``importance_sampling`` docstring example: nerfacc
-(8340e19daad4bafe24125150a8c56161838086fa, README.md:50) is not under
-``/root/reference`` and cannot be installed here.  Call sites this follows:
+(8340e19daad4bafe24125150a8c56161838086fa, README.md:50) is not in the
+reference tree and is not installed in the build environment.  Call sites this follows:
 ``third_party/nerfacc_prop_net.py:11-14,148,153,165,172,349``,
 ``radiance_fields/render_utils.py:4-8,35-42,73-75,103-105,159-282``.
 

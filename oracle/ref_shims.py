@@ -1,15 +1,15 @@
 """Stand-in modules that let the reference's own Python hot path run on CPU.
 
-TEST INFRASTRUCTURE -- see ``oracle/__init__.py``.  Used ONLY in this container
-(where ``/root/reference`` exists) by ``tests/golden/make_golden.py`` and the
-reference-vs-oracle cross-check; nothing here is needed on the GPU box.
+TEST INFRASTRUCTURE -- see ``oracle/__init__.py``.  Used ONLY where a checkout of
+NVlabs/EmerNeRF is named by ``EMER_REFERENCE_ROOT``, by the fixture generators
+``tests/golden/make_golden*.py``; no test and nothing on the GPU path needs it.
 
 ``install()`` injects, *before* any reference import:
   * ``omegaconf``                    -- name-only (``render_utils.py:9,296`` type annotation)
   * ``nerfacc`` (+ ``.data_specs``, ``.estimators.base``, ``.pdf``, ``.volrend``, ``.scan``)
                                      -- ``oracle.nerfacc_ref``
   * ``third_party.tcnn_modules``     -- ``oracle.tcnn_ref.Encoding``
-and puts ``/root/reference`` on ``sys.path`` so that ``radiance_fields`` /
+and puts ``EMER_REFERENCE_ROOT`` on ``sys.path`` so that ``radiance_fields`` /
 ``third_party.nerfacc_prop_net`` resolve to the reference's files, unmodified.
 """
 from __future__ import annotations
@@ -18,7 +18,7 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("EMER_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("EMER_REFERENCE_ROOT", "")
 
 
 def reference_available() -> bool:

@@ -1,7 +1,7 @@
 """Pure-PyTorch restatement of tiny-cuda-nn's ``HashGrid`` encoding (CPU oracle).
 
 TEST INFRASTRUCTURE -- see ``oracle/__init__.py``.  **Parity unpinned**: the
-tiny-cuda-nn sources are not under ``/root/reference`` (the reference installs
+tiny-cuda-nn sources are not in the reference tree (the reference installs
 them from master, README.md:51); this file restates the published algorithm of
 ``include/tiny-cuda-nn/encodings/grid.h`` and is anchored on the reference's
 call sites ``radiance_fields/encodings.py:130-146,159-160`` and

@@ -176,10 +176,10 @@ def _r(v, m):
 
 
 def _check_tc(kred, ncols, what):
-    """linear_tc.cu launch<>: one MMA covers the output width; the resident weight panels must fit shared memory."""
-    n_pad, kred_pad = _r(ncols, 16), _r(kred, 8)
+    """linear_tc.cu launch<>: the padded output width is at most 256; the resident weight panels fit shared memory."""
+    n_pad, kred_pad = _r(ncols, 16), _r(kred, 32)
     _require(n_pad <= 256, f"{what}: output width {ncols} exceeds one MMA (256)")
-    smem = 2 * (kred_pad // 4) * n_pad * 16 + 34816 + 256 * 4 + 6 * 8 + 16
+    smem = 2 * (kred_pad // 4) * n_pad * 16 + n_pad * 4
     _require(smem <= 227 * 1024, f"{what}: layer needs {smem} B of shared memory")
 
 
@@ -240,12 +240,13 @@ def emer_linear_bwd_weight(x, ldx, dy, lddy, y, ldy, act, dw, db, n, k, n_out, s
 
 
 def _check_tc_wgrad(x, ldx, dz, lddz, k, n_out):
-    """emer_linear_tc_bwd_weight's argument checks (linear_tc.cu), restated."""
+    """The limits within which _ops sends a weight gradient to emer_linear_tc_bwd_weight (wgrad_mn.cu takes any
+    k <= 256, n_out <= 128 with aligned rows), restated independently of _ops."""
     _require(n_out <= 128 and k <= 256, f"emer_linear_tc_bwd_weight: widths k={k} n_out={n_out} out of range")
     _require(ldx % 4 == 0 and lddz % 4 == 0 and _aligned16(x, dz), "emer_linear_tc_bwd_weight: rows must be 16-byte aligned")
     _require(_r(k, 4) <= ldx and _r(n_out, 4) <= lddz, "emer_linear_tc_bwd_weight: row stride shorter than the padded width")
     m_blocks, n_pad, k4 = (k + 127) // 128, _r(n_out, 16), _r(k, 4)
-    _require(m_blocks * 2 * n_pad <= 512, "emer_linear_tc_bwd_weight: accumulator does not fit TMEM")
+    _require(m_blocks * 2 * n_pad <= 512, "emer_linear_tc_bwd_weight: accumulator does not fit")
     a_panel, b_panel = (64 if k4 <= 64 else 128) * 16 + 16, n_pad * 16 + 16
     fits = False
     for rows, nbuf, stages in ((64, 2, 2), (64, 2, 1), (32, 2, 2), (32, 2, 1), (64, 1, 2), (64, 1, 1)):

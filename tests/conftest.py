@@ -13,19 +13,13 @@ warnings.filterwarnings("ignore", category=FutureWarning)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
-    config.addinivalue_line("markers", "reference: needs /root/reference (build container only)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
 
 
 def pytest_collection_modifyitems(config, items):
     import torch
 
     has_gpu = torch.cuda.is_available()
-    from oracle import ref_shims
-
-    has_ref = ref_shims.reference_available()
     for it in items:
         if "gpu" in it.keywords and not has_gpu:
             it.add_marker(pytest.mark.skip(reason="no CUDA device"))
-        if "reference" in it.keywords and not has_ref:
-            it.add_marker(pytest.mark.skip(reason="/root/reference not present"))

@@ -1,8 +1,8 @@
 """Generate the golden vectors by running the REFERENCE's own Python hot path on CPU.
 
-Run only in the build container (needs ``/root/reference``):
+Needs a checkout of the reference (NVlabs/EmerNeRF@8c051d7):
 
-    python tests/golden/make_golden.py
+    EMER_REFERENCE_ROOT=<checkout> python tests/golden/make_golden.py
 
 For every case of ``cases.py`` this imports the unmodified reference modules
 (``radiance_fields/*``, ``third_party/nerfacc_prop_net.py``) with the stand-ins of
@@ -161,7 +161,24 @@ def run_case(case: str):
     print(f"{case}: {len(store)} arrays, {os.path.getsize(path) / 1e6:.2f} MB")
 
 
+def run_raygen():
+    """raygen.npz: the reference's get_rays (datasets/base/pixel_source.py:39-76, executed from its source file) on
+    seeded rays, per-ray and shared camera matrices (test_live_reference_variants.py)."""
+    src = open(os.path.join(ref_shims.REFERENCE_ROOT, "datasets", "base", "pixel_source.py")).read()
+    ns = {}
+    exec("from torch import Tensor\nfrom typing import Tuple\nimport torch\n"
+         + src[src.index("def get_rays("):src.index("class ScenePixelSource")], ns)
+    g = torch.Generator().manual_seed(0)
+    x, y = torch.randint(0, 960, (777,), generator=g).float(), torch.randint(0, 640, (777,), generator=g).float()
+    c2w = torch.eye(4).repeat(777, 1, 1) + torch.randn(777, 4, 4, generator=g) * 0.3
+    K = torch.tensor([[1030.0, 0, 480], [0, 1030, 320], [0, 0, 1]]).repeat(777, 1, 1)
+    out = {"x": x, "y": y, "c2w": c2w, "K": K}
+    for tag, (c, k) in (("per_ray", (c2w, K)), ("shared", (c2w[0], K[0]))):
+        out.update({f"{tag}/{i}": t for i, t in enumerate(ns["get_rays"](x, y, c, k))})
+    np.savez_compressed(os.path.join(HERE, "raygen.npz"), **{k: v.numpy() for k, v in out.items()})
+
+
 if __name__ == "__main__":
-    assert ref_shims.reference_available(), "needs /root/reference"
-    for c in (sys.argv[1:] or list(cases.CASES)):
-        run_case(c)
+    assert ref_shims.reference_available(), "set EMER_REFERENCE_ROOT to a checkout of NVlabs/EmerNeRF"
+    for c in (sys.argv[1:] or list(cases.CASES) + ["raygen"]):
+        run_raygen() if c == "raygen" else run_case(c)

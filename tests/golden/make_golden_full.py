@@ -1,8 +1,8 @@
 """Golden vectors of the BENCHMARKED configuration (full_cases.py) from the REFERENCE's own Python on CPU.
 
-Run only in the build container (needs ``/root/reference``):
+Needs a checkout of the reference (NVlabs/EmerNeRF@8c051d7):
 
-    python tests/golden/make_golden_full.py [variant ...]
+    EMER_REFERENCE_ROOT=<checkout> python tests/golden/make_golden_full.py [variant ...]
 
 Same procedure as make_golden.py -- unmodified reference modules with the stand-ins of ``oracle.ref_shims``,
 cross-checked against ``oracle.hotpath`` -- on 256 Waymo-shape rays x 64 samples with the 2^20 / 2^18-entry
@@ -181,7 +181,7 @@ def run(variant: str):
 
 
 if __name__ == "__main__":
-    assert ref_shims.reference_available(), "needs /root/reference"
+    assert ref_shims.reference_available(), "set EMER_REFERENCE_ROOT to a checkout of NVlabs/EmerNeRF"
     torch.set_num_threads(min(os.cpu_count() or 1, 16))
     for v in (sys.argv[1:] or fc.VARIANTS):
         run(v)

@@ -1,6 +1,6 @@
-"""The drop-in claim, end to end, at the REAL configuration (build container only).
+"""The drop-in claim, end to end, at the REAL configuration (needs a reference checkout in EMER_REFERENCE_ROOT).
 
-The reference's own ``builders.py`` (unmodified, imported from /root/reference) builds the model and the
+The reference's own ``builders.py`` (unmodified, imported from EMER_REFERENCE_ROOT) builds the model and the
 proposal estimator from the reference's own ``configs/default_config.yaml`` twice:
 
   ref   <file>   with the reference's classes (oracle stand-ins for tiny-cuda-nn / nerfacc)
@@ -26,7 +26,7 @@ import yaml
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.environ.get("EMER_REFERENCE_ROOT", "/root/reference")
+REF = os.environ["EMER_REFERENCE_ROOT"]
 for p in (ROOT, HERE, os.path.join(HERE, "golden")):
     if p not in sys.path:
         sys.path.insert(0, p)

@@ -1,4 +1,4 @@
-"""INTEGRATION.md's two-line claim, executed on the reference's ENTRY SCRIPT (build container only).
+"""INTEGRATION.md's two-line claim, executed on the reference's ENTRY SCRIPT (needs EMER_REFERENCE_ROOT).
 
 After ``emernerf_b200.install_dropin()`` the import block of the reference's unmodified ``train_emernerf.py``
 (lines 1-27: builders, loss, datasets, radiance_fields.render_utils, radiance_fields.video_utils,
@@ -22,7 +22,7 @@ import types
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.environ.get("EMER_REFERENCE_ROOT", "/root/reference")
+REF = os.environ["EMER_REFERENCE_ROOT"]
 
 # packages of the reference's driver / data / visualisation layers that are absent from this image
 ABSENT_OK = ("imageio", "omegaconf", "wandb", "timm", "skimage", "plotly", "matplotlib", "cv2", "lpips", "open3d",

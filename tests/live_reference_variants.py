@@ -1,12 +1,16 @@
-"""Option variants of the field / estimator, REFERENCE vs DROP-IN, live (build container only).
+"""Option variants of the field / estimator: the DROP-IN against the REFERENCE's own classes.
 
-Run as a script by tests/test_live_reference_variants.py in a subprocess (the reference's module names
-``radiance_fields`` / ``third_party`` go into ``sys.modules``).  For every variant the reference's own classes
-(with the oracle stand-ins for tiny-cuda-nn / nerfacc, oracle/ref_shims.py) and the drop-in's classes (with the
-C ABI answered by tests/cabi_emulator.py) are built with the same constructor arguments, the reference's
-state-dict is loaded into the drop-in, both render the same rays, and the maximum relative error of every
-output is printed as one JSON object.  What this covers beyond the four golden cases: the constructor options
-and data-dict shapes of SURVEY.md section 8b that the shipped configs do not exercise.
+Run by tests/test_live_reference_variants.py in a subprocess (C ABI answered by tests/cabi_emulator.py).  Built with the
+reference's constructor arguments and seeds, the drop-in holds the reference's weights exactly; the maximum relative
+error of every output, proposal loss and gradient against the reference's results stored in tests/golden/variants.npz
+(shapes and SAMPLE seeded positions per tensor) is printed as JSON.  Covers the constructor options and data-dict shapes
+of SURVEY.md section 8b that the shipped configs do not exercise.
+
+    python tests/live_reference_variants.py [variant ...]
+    EMER_REFERENCE_ROOT=<checkout of NVlabs/EmerNeRF> python tests/live_reference_variants.py --write [variant ...]
+
+``--write`` runs the reference's own classes (with the oracle stand-ins for tiny-cuda-nn / nerfacc, oracle/ref_shims.py)
+and stores what they compute.
 """
 from __future__ import annotations
 
@@ -16,6 +20,7 @@ import sys
 import types
 import warnings
 
+import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -24,18 +29,20 @@ for p in (ROOT, HERE, os.path.join(HERE, "golden")):
     if p not in sys.path:
         sys.path.insert(0, p)
 warnings.filterwarnings("ignore")
+FIXTURES = os.path.join(HERE, "golden", "variants.npz")
+WRITE = "--write" in sys.argv[1:]
 
-from oracle import ref_shims  # noqa: E402
+if WRITE:
+    from oracle import ref_shims
 
-ref_shims.install()
+    ref_shims.install()
+    from radiance_fields import RadianceField as RefField, build_density_field as ref_build_density  # noqa: E402
+    from radiance_fields.encodings import HashEncoder as RefEncoder  # noqa: E402
+    from radiance_fields.render_utils import render_rays as ref_render_rays  # noqa: E402
+    from third_party.nerfacc_prop_net import PropNetEstimator as RefEstimator  # noqa: E402
 
 import cabi_emulator  # noqa: E402
 import cases  # noqa: E402
-from radiance_fields import RadianceField as RefField, build_density_field as ref_build_density  # noqa: E402
-from radiance_fields.encodings import HashEncoder as RefEncoder  # noqa: E402
-from radiance_fields.render_utils import render_rays as ref_render_rays  # noqa: E402
-from third_party.nerfacc_prop_net import PropNetEstimator as RefEstimator  # noqa: E402
-
 from emernerf_b200.radiance_fields import RadianceField, build_density_field  # noqa: E402
 from emernerf_b200.radiance_fields.encodings import HashEncoder  # noqa: E402
 from emernerf_b200.radiance_fields.render_utils import render_rays  # noqa: E402
@@ -51,9 +58,12 @@ class _Patch:
 
 cabi_emulator.install(_Patch())
 
-REF = types.SimpleNamespace(HashEncoder=RefEncoder, RadianceField=RefField, build_density_field=ref_build_density)
 OURS = types.SimpleNamespace(HashEncoder=HashEncoder, RadianceField=RadianceField,
-                             build_density_field=build_density_field)
+                             build_density_field=build_density_field, render_rays=render_rays,
+                             PropNetEstimator=PropNetEstimator)
+if WRITE:
+    REF = types.SimpleNamespace(HashEncoder=RefEncoder, RadianceField=RefField, build_density_field=ref_build_density,
+                                render_rays=ref_render_rays, PropNetEstimator=RefEstimator)
 
 BASE = dict(geometry_feature_dim=64, base_mlp_layer_width=64, head_mlp_layer_width=64, enable_cam_embedding=False,
             enable_img_embedding=True, num_cams=cases.N_CAMS, appearance_embedding_dim=16, semantic_feature_dim=64,
@@ -124,24 +134,21 @@ def rel(a, b):
     return ((a - b).abs().max() / b.abs().max().clamp_min(1e-12)).item()
 
 
-def compare(got, want, errs, prefix=""):
-    assert set(got) == set(want), (prefix, sorted(set(got) ^ set(want)))
-    for k in want:
-        if isinstance(want[k], dict):
-            compare(got[k], want[k], errs, prefix + k + "/")
+def flatten(d, prefix, out):
+    for k, v in d.items():
+        if isinstance(v, dict):
+            flatten(v, prefix + k + "/", out)
         else:
-            assert got[k].shape == want[k].shape, (prefix + k, got[k].shape, want[k].shape)
-            errs[prefix + k] = rel(got[k], want[k])
+            out[prefix + k] = v
 
 
-def run_variant(name):
+def run_side(ns, name):
+    """Build the variant from ``ns`` (the reference's classes or the drop-in's), render, and in training mode take the
+    proposal loss and the parameter gradients.  Returns {key: tensor}, or {"raises": "<type>: <message>"} when the
+    render refuses the input (the same refusal on both sides is parity too)."""
     kwargs, dynamic, flow, edit, cfg_edit, est_kw, mode = VARIANTS[name]
-    rf, rp = build(REF, kwargs, dynamic, flow)
-    randomise(rf, rp)
-    of, op = build(OURS, kwargs, dynamic, flow)
-    of.load_state_dict(rf.state_dict())
-    for a, b in zip(op, rp):
-        a.load_state_dict(b.state_dict())
+    field, props = build(ns, kwargs, dynamic, flow)
+    randomise(field, props)
     case = "flow_feat" if edit in ("features", "features384") else "static"
     batch = cases.make_batch(case)
     if edit == "features384":
@@ -160,74 +167,98 @@ def run_variant(name):
     for k, v in cfg_edit.items():
         setattr(cfg.nerf.propnet, k, v)
     if n_props is not None:
-        # the same networks on both sides: drop one, or append a third built like the second
-        if n_props < len(rp):
-            rp, op = rp[:n_props], op[:n_props]
-        while len(rp) < n_props:
+        # drop one network, or append a third built like the second
+        props = props[:n_props]
+        while len(props) < n_props:
             e = cases.ENC_PROP[-1]
-            extra = []
-            for ns in (REF, OURS):
-                torch.manual_seed(9)
-                p = ns.build_density_field(n_input_dims=3, n_levels=e["n_levels"], max_resolution=e["max_resolution"],
-                                           log2_hashmap_size=e["log2_hashmap_size"],
-                                           n_features_per_level=e["n_features_per_level"], unbounded=True)
-                p.set_aabb(cases.AABB)
-                extra.append(p)
-            randomise(extra[0], [], seed=3)
-            extra[1].load_state_dict(extra[0].state_dict())
-            rp, op = rp + [extra[0]], op + [extra[1]]
+            torch.manual_seed(9)
+            p = ns.build_density_field(n_input_dims=3, n_levels=e["n_levels"], max_resolution=e["max_resolution"],
+                                       log2_hashmap_size=e["log2_hashmap_size"],
+                                       n_features_per_level=e["n_features_per_level"], unbounded=True)
+            p.set_aabb(cases.AABB)
+            randomise(p, [], seed=3)
+            props = props + [p]
     train = mode == "train"
-    r_est = RefEstimator(torch.optim.Adam([q for p in rp for q in p.parameters()], lr=0.01), None, **est_kw)
-    o_est = PropNetEstimator(torch.optim.Adam([q for p in op for q in p.parameters()], lr=0.01), None, **est_kw)
-    for m in (rf, of, r_est, o_est, *rp, *op):
+    est = ns.PropNetEstimator(torch.optim.Adam([q for p in props for q in p.parameters()], lr=0.01), None, **est_kw)
+    for m in (field, est, *props):
         m.train(train)
-    errs = {}
-    failures = []
     with torch.set_grad_enabled(train):
-        for fn, args in ((ref_render_rays, (rf, r_est, rp)), (render_rays, (of, o_est, op))):
-            torch.manual_seed(77)
-            try:
-                failures.append(None)
-                res = fn(*args, dict(batch), cfg, proposal_requires_grad=train, return_decomposition=not train)
-            except (AssertionError, ValueError, KeyError) as e:          # same refusal on both sides is parity too
-                failures[-1] = (type(e).__name__, str(e))
-                res = None
-            if fn is ref_render_rays:
-                want = res
-            else:
-                got = res
-    if failures[0] is not None or failures[1] is not None:
-        assert failures[0] == failures[1], failures
-        return {"raises:" + failures[0][0]: 0.0}
-    compare(got, want, errs)
+        torch.manual_seed(77)
+        try:
+            out = ns.render_rays(field, est, props, dict(batch), cfg, proposal_requires_grad=train,
+                                 return_decomposition=not train)
+        except (AssertionError, ValueError, KeyError) as e:
+            return {"raises": f"{type(e).__name__}: {e}"}
+    res = {}
+    flatten(out, "out/", res)
     if train:
-        wl = r_est.compute_loss(want["extras"]["trans"], 1024.0)
-        gl = o_est.compute_loss(got["extras"]["trans"], 1024.0)
-        errs["prop_loss"] = abs(gl.item() - wl.item()) / max(1.0, abs(wl.item()))
-        loss_w = (want["rgb"] - batch["pixels"]).square().mean() + want["depth"].mean() * 1e-2
-        loss_g = (got["rgb"] - batch["pixels"]).square().mean() + got["depth"].mean() * 1e-2
-        (loss_w + wl).backward()
-        (loss_g + gl).backward()
-        ref_grads = dict(rf.named_parameters())
-        for k, v in of.named_parameters():
-            w = ref_grads[k].grad
-            assert (v.grad is None) == (w is None), k
-            if w is not None:
-                errs["grad/" + k] = rel(v.grad, w)
-        for i, (a, b) in enumerate(zip(op, rp)):
-            rg = dict(b.named_parameters())
-            for k, v in a.named_parameters():
-                w = rg[k].grad
-                assert (v.grad is None) == (w is None), (i, k)
-                if w is not None:
-                    errs[f"grad/prop{i}/" + k] = rel(v.grad, w)
+        ploss = est.compute_loss(out["extras"]["trans"], 1024.0)
+        res["prop_loss"] = ploss.detach().reshape(1)
+        loss = (out["rgb"] - batch["pixels"]).square().mean() + out["depth"].mean() * 1e-2
+        (loss + ploss).backward()
+        for k, v in field.named_parameters():
+            if v.grad is not None:
+                res["grad/" + k] = v.grad
+        for i, p in enumerate(props):
+            for k, v in p.named_parameters():
+                if v.grad is not None:
+                    res[f"grad/prop{i}/" + k] = v.grad
+    return res
+
+
+SAMPLE = 256
+
+
+def sample(res):
+    """{key: tensor} -> {key: values at SAMPLE fixed seeded positions (all of them for smaller tensors), shape/key: shape}"""
+    out = {}
+    for k, v in res.items():
+        if isinstance(v, str):
+            out[k] = v
+            continue
+        flat = v.detach().reshape(-1)
+        if flat.numel() > SAMPLE:
+            flat = flat[torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:SAMPLE]]
+        out[k] = flat
+        out["shape/" + k] = torch.tensor(v.shape, dtype=torch.int64)
+    return out
+
+
+def compare_variant(name):
+    """Errors of the drop-in against the stored reference results of one variant."""
+    z = np.load(FIXTURES)
+    want = {k[len(name) + 1:]: (str(z[k]) if z[k].dtype.kind == "U" else torch.from_numpy(z[k]))
+            for k in z.files if k.startswith(name + "/")}
+    got = sample(run_side(OURS, name))
+    if "raises" in want or "raises" in got:
+        assert str(want.get("raises")) == got.get("raises"), (name, want.get("raises"), got.get("raises"))
+        return {"raises:" + got["raises"].split(":")[0]: 0.0}
+    assert set(got) == set(want), (name, sorted(set(got) ^ set(want)))
+    errs = {}
+    for k, w in want.items():
+        g = got[k]
+        assert g.shape == w.shape, (name, k, g.shape, w.shape)
+        if k.startswith("shape/"):
+            assert torch.equal(g, w), (name, k, g, w)
+        elif k == "prop_loss":
+            errs[k] = abs(g.item() - w.item()) / max(1.0, abs(w.item()))
+        else:
+            errs[k[len("out/"):] if k.startswith("out/") else k] = rel(g, w)
     return errs
 
 
 if __name__ == "__main__":
-    assert ref_shims.reference_available(), "needs /root/reference"
+    names = [a for a in sys.argv[1:] if a != "--write"] or list(VARIANTS)
+    if WRITE:
+        assert ref_shims.reference_available(), "set EMER_REFERENCE_ROOT to a checkout of NVlabs/EmerNeRF"
+        arrays = dict(np.load(FIXTURES)) if os.path.exists(FIXTURES) else {}
+        for name in names:
+            for k, v in sample(run_side(REF, name)).items():
+                arrays[f"{name}/{k}"] = np.array(v) if isinstance(v, str) else v.numpy()
+        np.savez_compressed(FIXTURES, **arrays)
+        sys.exit(0)
     out = {}
-    for name in (sys.argv[1:] or list(VARIANTS)):
+    for name in names:
         del cabi_emulator.CALLS[:]
-        out[name] = {"errors": run_variant(name), "calls": sorted(set(cabi_emulator.CALLS))}
+        out[name] = {"errors": compare_variant(name), "calls": sorted(set(cabi_emulator.CALLS))}
     print("JSON:" + json.dumps(out))

@@ -164,7 +164,7 @@ def test_sorted_interp_quad_searchsorted_equals_dense_mask():
 
 
 def test_tensor_core_eligibility_mirrors_the_library_limits():
-    """_ops only sends a layer to the tcgen05 kernels when the library can take it (csrc/linear_tc.cu launch<>,
+    """_ops only sends a layer to the tensor-core kernels when the library can take it (csrc/linear_tc.cu launch<>,
     emer_linear_tc_bwd_weight); the emulator carries an independent restatement of the same limits, so a
     disagreement between the two shows up here before it can on the GPU."""
     import ctypes

@@ -1,4 +1,4 @@
-"""bench.py's two arms compute the same workload: one training step of the B200 arm (``Trainer._step_body`` --
+"""bench.py's two arms compute the same workload: one training step of the GPU arm (``Trainer._step_body`` --
 render_rays + proposal update + pixel losses + backward + Adam, here on CPU with the C ABI answered by
 tests/cabi_emulator.py) against the step the reference arm times (``cpu_baseline``: oracle render_rays +
 the same losses + backward), on the same full-size default configuration, tables, batch and random draws."""
@@ -49,7 +49,7 @@ def test_training_step_of_both_arms_is_the_same_computation(monkeypatch, variant
     names = [k for k, v in fsd.items() if v.requires_grad]
     grads_o = dict(zip(names, torch.autograd.grad(loss_o * 1024.0, [fsd[k] for k in names], allow_unused=True)))
 
-    # ---- B200 arm's step body, unmodified
+    # ---- GPU arm's step body, unmodified
     tr = bench.Trainer.__new__(bench.Trainer)
     tr.args = types.SimpleNamespace(variant=variant, rays=n_rays, samples=samples)
     tr.rank, tr.world, tr.device, tr.cfg = 0, 1, "cpu", cfg

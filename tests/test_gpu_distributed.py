@@ -1,6 +1,6 @@
-"""Two B200s, NCCL: the ray-sharded data-parallel step of emernerf_b200.distributed (flat-bucket all-reduce, and
-reduce-scatter -> sharded FusedAdam -> all-gather) equals the one-GPU full-batch step.  Needs >= 2 GPUs
-(``gpurun --gpus 2``); skipped otherwise."""
+"""Two GPUs, NCCL: the ray-sharded data-parallel step of emernerf_b200.distributed (flat-bucket all-reduce, and
+reduce-scatter -> sharded FusedAdam -> all-gather) equals the one-GPU full-batch step.  Needs >= 2 GPUs; skipped
+otherwise."""
 import pytest
 import torch
 

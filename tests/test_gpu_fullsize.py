@@ -2,8 +2,8 @@
 own Python produced for the full-size model (tests/golden/make_golden_full.py): 2^20-entry static grid, 2^18-entry
 4-D grids, 8x1 proposal grids, 64 samples, proposal samples [128, 64], 256 Waymo-shape rays.
 
-16 384 rows per head and 32 768 / 16 384 proposal samples: the tcgen05 layers (``tc_linear_kernel`` /
-``tc_wgrad_kernel``), ``prop_level_kernel<8>`` and the 10-level gather / scatter kernels -- exactly what ``bench.py``
+16 384 rows per head and 32 768 / 16 384 proposal samples: the tensor-core layers (``tc_linear_kernel`` /
+``wgrad_kernel``), ``prop_level_kernel<8>`` and the 10-level gather / scatter kernels -- exactly what ``bench.py``
 times -- are the code under test here (the miniature fixtures of test_gpu_golden.py stay below ``TC_MIN_ROWS``).
 
 Bars: every rendered (per-ray) output within 1e-4 relative of the reference (BASELINE.json), PSNR of the rendered
@@ -188,7 +188,7 @@ def test_full_size_render_matches_reference(variant, mode):
 
 @pytest.mark.parametrize("variant", fc.VARIANTS)
 def test_full_size_field_and_compositing_at_reference_samples(variant):
-    """The field (hash grids, fused chain / tcgen05 layers, heads) and the compositing kernels on the REFERENCE's own
+    """The field (hash grids, fused chain / tensor-core layers, heads) and the compositing kernels on the REFERENCE's own
     sample intervals (rebuilt from its t_vals -+ t_dist / 2), without the resampling chain in front: every rendered
     output within 1e-4, per-sample densities / flows within 5e-5, on ALL rays."""
     from emernerf_b200.radiance_fields.render_utils import rendering

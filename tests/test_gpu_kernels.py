@@ -145,7 +145,7 @@ def test_contract_forward_backward_vs_oracle():
                                         (116, 64, 1), (180, 64, 1), (40, 192, 0)])
 def test_linear_forward_backward_vs_fp32_reference(k, n_out, act, impl, monkeypatch):
     """Plain PyTorch fp32 (CPU) reference of the same layer; tolerance 2e-5 relative (fp32 sums of up
-    to 180 terms in a different order).  ``tc`` = tcgen05 3xTF32 kernels, ``simt`` = FFMA kernels."""
+    to 180 terms in a different order).  ``tc`` = wgmma 3xTF32 kernels, ``simt`` = FFMA kernels."""
     from emernerf_b200 import _ops
 
     monkeypatch.setattr(_ops, "LINEAR_IMPL", impl)
@@ -187,7 +187,7 @@ def test_linear_strided_input_rows(impl, monkeypatch):
 
 
 def test_linear_wgrad_tc_matches_simt(monkeypatch):
-    """tcgen05 weight gradient (dW^T accumulated in TMEM over many row tiles) vs the FFMA kernel."""
+    """wgmma weight gradient (dW^T accumulated in registers over many row tiles) vs the FFMA kernel."""
     from emernerf_b200 import _ops
 
     g = torch.Generator(device=DEV).manual_seed(3)
@@ -208,7 +208,7 @@ def test_linear_wgrad_tc_matches_simt(monkeypatch):
 
 
 def test_linear_tc_many_tiles_and_ragged_tail():
-    """More tiles than CTAs (persistent loop, ring phases wrap) and a ragged last tile."""
+    """More tiles than CTAs (persistent loop over several tiles per CTA) and a ragged last tile."""
     from emernerf_b200 import _ops
 
     g = torch.Generator(device=DEV).manual_seed(11)
@@ -502,7 +502,9 @@ def test_colour_head_chain_skip_variants(impl, shared, n, monkeypatch):
     """The colour head (113 -> 64 -> [64 | 113] -> 64 -> 3, sigmoid; radiance_fields/mlp.py:38-46) through the
     chain in its four bookkeeping variants -- stacked / two-product skip gradient, shared / copied
     concatenation buffer -- against fp64 autograd.  n = 300 runs the CUDA-core layers, the larger n the
-    tcgen05 ones (3xTF32: ~1e-6)."""
+    tensor-core ones (3xTF32: ~1e-6).  Rows with a ReLU input within 1e-5 of zero get no upstream gradient:
+    there the mask is decided by fp32 rounding, which differs with any summation order (the data has an
+    input of 3e-7 against ~1e-6 of rounding in its row)."""
     from emernerf_b200 import _ops
 
     monkeypatch.setattr(_ops, "SKIP_BWD_IMPL", impl)
@@ -517,9 +519,14 @@ def test_colour_head_chain_skip_variants(impl, shared, n, monkeypatch):
     wd = [w.double().requires_grad_() for w in ws]
     bd = [b.double().requires_grad_() for b in bs]
     xd = x.double().requires_grad_()
-    h1 = torch.relu(xd @ wd[0].t() + bd[0])
-    h2 = torch.relu(torch.cat([h1, xd], -1) @ wd[1].t() + bd[1])
+    z1 = xd @ wd[0].t() + bd[0]
+    h1 = torch.relu(z1)
+    z2 = torch.cat([h1, xd], -1) @ wd[1].t() + bd[1]
+    h2 = torch.relu(z2)
     yd = torch.sigmoid(h2 @ wd[2].t() + bd[2])
+    ill = (z1.detach().abs() < 1e-5).any(-1) | (z2.detach().abs() < 1e-5).any(-1)
+    assert int(ill.sum()) <= 16
+    up = up * (~ill).float()[:, None]
     (yd * up.double()).sum().backward()
 
     wg = [w.to(DEV).requires_grad_() for w in ws]
@@ -542,7 +549,7 @@ def test_colour_head_chain_skip_variants(impl, shared, n, monkeypatch):
         assert rel_err(a.grad, b.grad) < 2e-5
 
 
-# ----------------------------------------------------------------------------- fused field chain (tcgen05, TMEM-resident)
+# ----------------------------------------------------------------------------- fused field chain (wgmma, register-resident)
 def _chain_reference(enc, rb, S, wb0, bb0, wb1, bb1, w0, w1, w2, b2, c, masks=None):
     """fp64 restatement of the chain.  ``masks`` = the ReLU masks of the kernel's own (saved) activations: with 10^6+
     pre-activations a handful sit within rounding distance of zero, where the fp32 kernel and fp64 disagree about
@@ -563,7 +570,7 @@ def _chain_reference(enc, rb, S, wb0, bb0, wb1, bb1, w0, w1, w2, b2, c, masks=No
 @pytest.mark.parametrize("k_enc,n_feat,n,S,c", [(40, 64, 128 * 6 + 37, 64, 49), (40, 128, 4096, 48, 49), (32, 64, 333, 16, 33),
                                                 (64, 64, 128 * 300, 64, 49)])
 def test_field_chain_forward_backward_vs_fp64(k_enc, n_feat, n, S, c):
-    """emer_field_fwd (csrc/field_fused.cu): outputs within 2e-5 of an fp64 restatement of the chain (3xTF32 in TMEM),
+    """emer_field_fwd (csrc/field_fused.cu): outputs within 2e-5 of an fp64 restatement of the chain (3xTF32),
     ragged last tile / last ray, both warpgroups and many tiles per CTA; gradients of every input through the op's
     backward within 2e-4 of fp64 autograd."""
     from emernerf_b200 import _ops
@@ -691,8 +698,8 @@ def test_gen_rays_matches_the_reference_formula():
 @pytest.mark.parametrize("k,n,ldx,lddz", [(64, 64 * 1500 + 21, 64, 64), (40, 128 * 700 + 5, 40, 64), (128, 64 * 900 + 63, 128, 64),
                                           (64, 37, 128, 128), (100, 64 * 400, 104, 64), (64, 524288, 128, 128)])
 def test_weight_gradient_mn_major_operands(k, n, ldx, lddz):
-    """emer_linear_tc_bwd_weight_mn (csrc/wgrad_mn.cu: operands as they lie in memory, MN-major SWIZZLE_128B_BASE32B,
-    elementwise hi / lo split) against fp64: dW and db within 2e-5 of the sum over all rows; ragged last tile, strided
+    """emer_linear_tc_bwd_weight_mn (csrc/wgrad_mn.cu: operands read as they lie in memory, row-major X and dZ)
+    against fp64: dW and db within 2e-5 of the sum over all rows; ragged last tile, strided
     rows, k not a multiple of 32, accumulation into a non-zero buffer."""
     import ctypes
 
@@ -709,7 +716,7 @@ def test_weight_gradient_mn_major_operands(k, n, ldx, lddz):
               _ops._stream())
     want_w = dw0.double() + dz.double().T @ x.double()
     want_b = db0.double() + dz.double().sum(0)
-    tol = 2e-5 if n < 200000 else 5e-5               # fp32 accumulation over 8192 tiles in TMEM + 148 partial sums
+    tol = 2e-5 if n < 200000 else 5e-5               # fp32 accumulation over thousands of row tiles in registers + one partial sum per CTA
     assert rel_err(dw, want_w) < tol, rel_err(dw, want_w)
     assert rel_err(db, want_b) < tol, rel_err(db, want_b)
 

@@ -2,7 +2,7 @@
 ``PropNetEstimator``) and the autograd wrappers of ``emernerf_b200/_ops.py`` run unmodified on CPU tensors, with
 the shared library's entry points answered by ``tests/cabi_emulator.py`` (oracle arithmetic behind the same
 pointers / strides / sizes), and are compared with the golden vectors produced by the reference's own Python
-(tests/golden/make_golden.py) -- the same comparisons tests/test_gpu_golden.py makes on the B200, at the same
+(tests/golden/make_golden.py) -- the same comparisons tests/test_gpu_golden.py makes on the GPU, at the same
 tolerances.  What this pins without a GPU: closure plumbing, per-sample expand views, fused-path selection,
 weight-column permutations of the colour head, buffer / stride / padding bookkeeping, gradient routing, the
 proposal cache and the interlevel loss.

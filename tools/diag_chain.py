@@ -1,4 +1,4 @@
-"""Per-tensor errors of the fused chain's forward saves and backward against fp64 (run on the GPU box)."""
+"""Per-tensor errors of the fused chain's forward saves and backward against fp64 (needs a CUDA device)."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden")):

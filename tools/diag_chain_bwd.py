@@ -1,4 +1,4 @@
-"""Step through _FieldChain.backward's kernel sequence, comparing every intermediate with fp64 (run on the GPU box)."""
+"""Step through _FieldChain.backward's kernel sequence, comparing every intermediate with fp64 (needs a CUDA device)."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden")):

@@ -1,4 +1,4 @@
-"""Where does the end-to-end difference at the benchmarked configuration come from?  (run on the GPU box)
+"""Where does the end-to-end difference at the benchmarked configuration come from?  (needs a CUDA device)
 
 Stage-by-stage comparison of the drop-in on cuda:0 with the CPU oracle for the full-size static model
 (tests/golden/full_cases.py), evaluation mode: every proposal level in isolation (fed with the ORACLE's previous

@@ -1,4 +1,4 @@
-"""Per-level timing of the hash-grid forward / backward kernels on ray-coherent points (B200).
+"""Per-level timing of the hash-grid forward / backward kernels on ray-coherent points.
 
     python tools/microbench_grid.py [--rays 8192] [--samples 64]
 

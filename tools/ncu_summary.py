@@ -1,6 +1,6 @@
 """Condense an .ncu-rep (read with `ncu -i ... --page raw --csv`) into the table the docs cite.
 
-    python tools/ncu_summary.py gpurun_out/r2_chain.ncu-rep > profiles/r2_chain_ncu_summary.md
+    python tools/ncu_summary.py <report>.ncu-rep > <summary>.md
 """
 import csv
 import io

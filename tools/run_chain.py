@@ -1,4 +1,4 @@
-"""Launch the fused field chain (forward + backward) at the benchmark's shapes, for ncu captures and CUDA-event timing.
+"""Launch the fused field chain (forward + backward) at the benchmark's shapes, for profiler captures and CUDA-event timing.
 
     python tools/run_chain.py [n_points] [reps]
 """

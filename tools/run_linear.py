@@ -1,4 +1,4 @@
-"""Launch the dense-layer kernels once at bench shapes (for ncu captures)."""
+"""Launch the dense-layer kernels once at bench shapes (for profiler captures)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""Time the two tcgen05 weight-gradient kernels at the benchmark's shapes (CUDA events, 5 repetitions)."""
+"""Time the two wgmma weight-gradient entry points at the benchmark's shapes (CUDA events, 5 repetitions)."""
 import os
 import sys
 

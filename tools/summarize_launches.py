@@ -1,6 +1,6 @@
 """Summarise an ncu launch list (``--metrics gpu__time_duration.sum --csv``) into a markdown table.
 
-    python tools/summarize_launches.py gpurun_out/launches.csv "title" > profiles/<name>.md
+    python tools/summarize_launches.py <launches>.csv "title" > <summary>.md
 """
 import collections
 import csv
