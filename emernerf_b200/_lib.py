@@ -47,6 +47,8 @@ _SIGNATURES = {
                        _P, _P, _P, c_int64, _P],
     "emer_field_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, c_int, _P, c_int64, _P, _P, c_int64, _P, _P, _P, _P,
                        _P, _P, c_int64, _P, c_int, c_int64, _P],
+    "emer_field_wgrad": [_P, c_int64, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, _P, c_int64, _P, _P,
+                         c_int64, _P, _P, c_int64, _P],
     "emer_gen_rays": [_P, _P, _P, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P, c_int64, _P],
     "emer_adam_step": [_P, _P, c_int, c_int64, _P, c_float, c_float, c_float, c_float, c_int, _P],
     "emer_composite_fwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, _P],
@@ -123,6 +125,8 @@ def tag_of(name: str, args) -> str:
             return f"k{args[10]}_o{args[11]}_N{args[9]}"
         if name == "emer_field_bwd":
             return f"k{args[10]}_f{args[12]}_N{args[27]}"
+        if name == "emer_field_wgrad":
+            return f"k{args[2]}_f{args[11]}_N{args[23]}"
         if name == "emer_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("_save" if args[19].value else "")
     except Exception:

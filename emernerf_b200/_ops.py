@@ -674,6 +674,13 @@ CHAIN_BWD = os.environ.get("EMER_CHAIN_BWD", "fused")          # "layers": data 
 CHAIN_K_ENC = (32, 40, 64)
 
 
+def _field_wgrad_usable(t: Tensor) -> bool:
+    """Whether the fused chain's weight gradients take the one-launch ``emer_field_wgrad``: tensors on the GPU.  The CPU
+    harness of the C ABI (tests/cabi_emulator.py) runs the same data path on host memory; there they go through the
+    per-layer weight-gradient entry points it answers."""
+    return t.is_cuda
+
+
 def _tc_bwd_data_acc(dz: Tensor, lddz: int, w: Tensor, dx: Tensor, lddx: int, n: int) -> None:
     """dx[n, k] += dz[n, n_out] @ w on the tensor-core layer kernel (accumulating form)."""
     n_out, k = w.shape
@@ -793,62 +800,89 @@ class _FieldChain(torch.autograd.Function):
             if d_sigma is not None:
                 # trunc_exp backward (nerf_utils.py:72-75): g * exp(clamp(x, max=15)), x = feats[:, 0] - 1 = log(sigma)
                 dgeo[:, 0] += _f32c(d_sigma).reshape(n) * torch.clamp(sigma, max=3269017.25)
-            dzb = None
-        if n_feat == 128:
-            dfe = torch.cat([D1[:, 64:], torch.zeros((n, 64), **f32) if d_sem is None else d_sem], dim=1)
-            ldf = 128
-        else:
-            dfe, ldf = D1[:, 64:], 128
-        if dzb is None:
+        one_launch = fused_data and _field_wgrad_usable(enc2)
+        if not one_launch:
+            # [dF | d_sem]: the gradient of the base MLP's output (zeros for an absent semantic half)
+            if n_feat == 128:
+                dfe = torch.cat([D1[:, 64:], torch.zeros((n, 64), **f32) if d_sem is None else d_sem], dim=1)
+            else:
+                dfe = D1[:, 64:]
+        if not fused_data:
             dzb = torch.empty((n, 64), **f32)
-            _layer_bwd_data(dfe, ldf, wb1, dzb, 64, n, hb, 64, 64)
+            _layer_bwd_data(dfe, 128, wb1, dzb, 64, n, hb, 64, 64)
             if ctx.needs_input_grad[0]:
                 d_enc = torch.empty((n, _pad4(k_enc)), **f32)
                 _layer_bwd_data(dzb, 64, wb0, d_enc, d_enc.shape[1], n, None, 0, 0)
                 d_enc = d_enc[:, :k_enc]
 
-        res = {}
-
-        def weight_gradients(deferred=None):
-            """X^T dZ over all rows for the five layers (+ the column-block bookkeeping of the head's weights; on the
-            side stream those few adds are deferred to the join: autograd adds the per-ray columns' gradient to the same
-            tensors on the main stream)."""
-            dw0 = dw1 = dw2_ = db2_ = None
-            add = (lambda dst, src: dst.add_(src)) if deferred is None else (lambda dst, src: deferred.append(lambda: dst.add_(src)))
+        if not one_launch:
+            # X^T dZ layer by layer; the head's geo / hidden column blocks, its per-ray columns get their gradient
+            # through ray_bias
+            if fused_data and d_rgb is not None:
+                dw2, db2 = _layer_bwd_weight(h1, 64, dz2, 3, w2, True, n, sk["w2"], sk["b2"])
+                dw1hg, _ = _layer_bwd_weight(hg, 128, dz1, 64, w1hg, False, n)
+                dw0g, _ = _layer_bwd_weight(hg[:, 64:], 128, D1[:, :64], 128, w0g, False, n)
+            dw0 = dw1 = None
             if d_rgb is not None:
-                if fused_data:
-                    dw2_, db2_ = _layer_bwd_weight(h1, 64, dz2, 3, w2, True, n, sk["w2"], sk["b2"])
-                    dw1hg_ = _layer_bwd_weight(hg, 128, dz1, 64, w1hg, False, n)[0]
-                    dw0g_ = _layer_bwd_weight(hg[:, 64:], 128, D1[:, :64], 128, w0g, False, n)[0]
-                else:
-                    dw2_, db2_, dw1hg_, dw0g_ = dw2, db2, dw1hg, dw0g
-                # the head's geo / hidden column blocks; its per-ray columns get their gradient through ray_bias
                 if sk["w0"] is not None:
-                    add(sk["w0"][0][:, n_ray_cols:], dw0g_)
+                    sk["w0"][0][:, n_ray_cols:].add_(dw0g)
                     sk["w0"][1]()
                 else:
                     dw0 = torch.zeros_like(w0)
-                    dw0[:, n_ray_cols:] = dw0g_
+                    dw0[:, n_ray_cols:] = dw0g
                 if sk["w1"] is not None:
-                    add(sk["w1"][0][:, :64], dw1hg_[:, :64])
-                    add(sk["w1"][0][:, 64 + n_ray_cols:], dw1hg_[:, 64:])
+                    sk["w1"][0][:, :64].add_(dw1hg[:, :64])
+                    sk["w1"][0][:, 64 + n_ray_cols:].add_(dw1hg[:, 64:])
                     sk["w1"][1]()
                 else:
                     dw1 = torch.zeros_like(w1)
-                    dw1[:, :64] = dw1hg_[:, :64]
-                    dw1[:, 64 + n_ray_cols:] = dw1hg_[:, 64:]
-            dwb1, dbb1 = _layer_bwd_weight(hb, 64, dfe, ldf, wb1, True, n, sk["wb1"], sk["bb1"])
+                    dw1[:, :64] = dw1hg[:, :64]
+                    dw1[:, 64 + n_ray_cols:] = dw1hg[:, 64:]
+            dwb1, dbb1 = _layer_bwd_weight(hb, 64, dfe, 128, wb1, True, n, sk["wb1"], sk["bb1"])
             dwb0, dbb0 = _layer_bwd_weight(enc2, ld_enc, dzb, 64, wb0, True, n, sk["wb0"], sk["bb0"])
-            res["g"] = (dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2_, db2_)
-
-        if WGRAD_STREAM and fused_data and all(v is not None for v in sk.values()) and enc2.is_cuda:
-            # every weight gradient lands in the optimizer's buffers: nothing autograd waits for, so the kernels may run
-            # beside the hash-grid scatter / the table's reduce-scatter (joined by FusedAdam.step / DataParallel.reduce)
-            with _on_side_stream(dev, enc2, hb, hg, h1, dz2, dz1, D1, dzb, dfe, w1hg, w0g):
-                weight_gradients(_AFTER_JOIN)
         else:
-            weight_gradients()
-        dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = res["g"]
+            shapes = dict(wb0=wb0.shape, bb0=(64,), wb1=wb1.shape, bb1=(n_feat,), w0=w0.shape, w1=w1.shape, w2=w2.shape,
+                          b2=(3,))
+            keys = list(shapes) if dz2 is not None else ["wb0", "bb0", "wb1", "bb1"]
+            side = WGRAD_STREAM and all(v is not None for v in sk.values()) and enc2.is_cuda
+
+            def weight_gradients(deferred):
+                """The five layers' X^T dZ in one emer_field_wgrad launch, accumulated into the optimizer's buffers (or
+                into zeros shaped like the parameters, returned to autograd).  ``deferred``: the side stream's list of
+                updates to run after the join -- the head's w0 / w1 gradients then go to zeros and are added there,
+                because autograd adds the per-ray columns' gradient to the same buffers on the main stream with an
+                in-place add of the whole tensor, which would race the kernel's atomics."""
+                out, grads = {}, {}
+                for k in keys:
+                    s = sk[k]
+                    if s is None:
+                        out[k] = grads[k] = torch.zeros(shapes[k], **f32)
+                    elif deferred is not None and k in ("w0", "w1"):
+                        out[k] = torch.zeros(shapes[k], **f32)
+                        deferred.append(lambda dst=s[0], src=out[k]: dst.add_(src))
+                    else:
+                        out[k] = s[0]
+                o = lambda k: _ptr(out[k]) if k in out else None
+                if dz2 is not None:        # the head's geo / hidden column blocks; the per-ray ones come through ray_bias
+                    w0g_d, ld_w0, w1g_d, ld_w1 = out["w0"][:, n_ray_cols:], out["w0"].stride(0), out["w1"][:, 64 + n_ray_cols:], out["w1"].stride(0)
+                else:
+                    w0g_d, ld_w0, w1g_d, ld_w1 = None, 0, None, 0
+                _lib.call("emer_field_wgrad", _ptr(enc2), ld_enc, k_enc, _ptr(hb), _ptr(hg), _ptr(h1), _ptr(dz2),
+                          _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_sem), n_feat, o("wb0"), o("bb0"), o("wb1"), o("bb1"),
+                          _ptr(w0g_d), ld_w0, o("w1"), _ptr(w1g_d), ld_w1, o("w2"), o("b2"), n, _stream())
+                for k in keys:
+                    if sk[k] is not None:
+                        sk[k][1]()
+                return tuple(grads.get(k) for k in ("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"))
+
+            if side:
+                # every weight gradient lands in the optimizer's buffers: nothing autograd waits for, so the kernel may
+                # run beside the hash-grid scatter / the table's reduce-scatter (joined by FusedAdam.step /
+                # DataParallel.reduce)
+                with _on_side_stream(dev, enc2, hb, hg, h1, dz2, dz1, D1, dzb, d_sem):
+                    dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(_AFTER_JOIN)
+            else:
+                dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(None)
         if d_enc is not None:
             d_enc = d_enc.reshape(enc_shape)
         return d_enc, d_rb, None, None, dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2

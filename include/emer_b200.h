@@ -216,13 +216,29 @@ int emer_field_fwd(const float* enc, int64_t ld_enc, int k_enc, const float* wb0
  *   d_ray_bias[R,128] += per-ray sums of [dz0 | dz1]   (caller zeroes; needs samples % 32 == 0; may be NULL)
  * hb / hg / h1 / rgb / sigma are emer_field_fwd's saves and outputs.  d_rgb, d_sigma, d_geo, d_sem, d_enc, dz2 may be
  * NULL.  Row buffers 32-byte aligned, ld_denc % 8 == 0.  The weight gradients are X^T dZ products over dz2 / dz1 / d1 /
- * dzb (emer_linear_tc_bwd_weight_mn). */
+ * dzb (emer_field_wgrad). */
 int emer_field_bwd(const float* d_rgb, const float* rgb, const float* d_sigma, const float* sigma,
                    const float* d_geo, const float* d_sem, const float* hb, const float* hg, const float* h1,
                    const float* wb0, int k_enc, const float* wb1, int n_feat, const float* w0g, int64_t ld_w0,
                    const float* w1h, const float* w1g, int64_t ld_w1, const float* w2, float* dz2, float* dz1,
                    float* d1, float* dzb, float* d_enc, int64_t ld_denc, float* d_ray_bias, int samples,
                    int64_t n, void* stream);
+
+/* Weight gradients of the fused field chain from emer_field_bwd's buffers, in one launch that reads every row buffer
+ * once (csrc/field_wgrad.cu).  All outputs accumulate (+=; the caller zeroes):
+ *   dwb0 [64, k_enc] += dzb^T enc,                 dbb0 [64]     += column sums of dzb
+ *   dwb1 [n_feat, 64] += [dF | d_sem]^T hb,         dbb1 [n_feat] += column sums of [dF | d_sem]
+ *   dw0g [64, 64] (row stride ld_w0) += dZ0^T geo
+ *   dw1h, dw1g [64, 64] (row stride ld_w1) += dz1^T h0, dz1^T geo
+ *   dw2 [3, 64] += dz2^T h1,                        db2 [3]       += column sums of dz2
+ * with hg = [h0 | geo] [N,128] and d1 = [dZ0 | dF] [N,128].  enc [N, k_enc] has row stride ld_enc (% 4 == 0);
+ * hb, h1, dz1, dzb, d_sem [N,64] and dz2 [N,3] are dense.  d_sem (n_feat = 128 only) may be NULL: dWb1's rows 64.. and
+ * dbb1[64:] are then left as they are.  dz2 NULL (no colour gradient): only dwb0 / dbb0 / dwb1 / dbb1 are computed,
+ * and hg, h1, dz1 and the head's outputs may be NULL.  Row buffers 16-byte aligned. */
+int emer_field_wgrad(const float* enc, int64_t ld_enc, int k_enc, const float* hb, const float* hg, const float* h1,
+                     const float* dz2, const float* dz1, const float* d1, const float* dzb, const float* d_sem,
+                     int n_feat, float* dwb0, float* dbb0, float* dwb1, float* dbb1, float* dw0g, int64_t ld_w0,
+                     float* dw1h, float* dw1g, int64_t ld_w1, float* dw2, float* db2, int64_t n, void* stream);
 
 /* ---- volume rendering along rays (replaces nerfacc.render_transmittance_from_density /
  *      render_weight_from_density / accumulate_along_rays and the torch cumsum/searchsorted of
