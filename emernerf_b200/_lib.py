@@ -55,6 +55,11 @@ _SIGNATURES = {
     "emer_composite_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, _P],
     "emer_accumulate_fwd": [_P, _P, _P, c_int64, c_int, c_int, _P],
     "emer_accumulate_bwd": [_P, _P, _P, _P, _P, c_int64, c_int, c_int, _P],
+    "emer_pointwise_loss_fwd": [c_int, _P, _P, c_int64, c_float, c_float, c_float, c_float, _P, _P, _P],
+    "emer_pointwise_loss_bwd": [c_int, _P, _P, c_int64, c_float, c_float, c_float, c_float, _P, _P, _P, _P, _P],
+    "emer_ray_loss_fwd": [c_int, _P, _P, _P, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, _P, _P, _P],
+    "emer_ray_loss_bwd": [c_int, _P, _P, _P, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, _P, _P, _P,
+                          _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])
@@ -127,6 +132,10 @@ def tag_of(name: str, args) -> str:
             return f"k{args[10]}_f{args[12]}_N{args[27]}"
         if name == "emer_field_wgrad":
             return f"k{args[2]}_f{args[11]}_N{args[23]}"
+        if name in ("emer_pointwise_loss_fwd", "emer_pointwise_loss_bwd"):
+            return f"kind{args[0]}_N{args[3]}"
+        if name in ("emer_ray_loss_fwd", "emer_ray_loss_bwd"):
+            return f"kind{args[0]}_R{args[4]}_S{args[5]}"
         if name == "emer_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("_save" if args[19].value else "")
     except Exception:

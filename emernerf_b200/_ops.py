@@ -8,6 +8,7 @@ tensors must live on a CUDA device -- there is no CPU path.
 from __future__ import annotations
 
 import ctypes
+import math
 import weakref
 from typing import Callable, Dict, Optional, Sequence, Tuple
 
@@ -1181,3 +1182,125 @@ def accumulate(w: Tensor, v: Tensor) -> Tensor:
         return torch.cat([_Accumulate.apply(w, v[..., c:c + ACC_MAX_CHANNELS])
                           for c in range(0, v.shape[-1], ACC_MAX_CHANNELS)], dim=-1)
     return _Accumulate.apply(w, v)
+
+
+# ----------------------------------------------------------------------------- training losses (csrc/losses.cu)
+LOSS_KINDS = {"l1": 0, "l2": 1, "smooth_l1": 2, "depth_l1": 3, "depth_l2": 4, "depth_smooth_l1": 5, "sky_bce": 6,
+              "sparsity": 7, "entropy": 8}
+RAY_LOSS_KINDS = {"line_of_sight": 0, "sky_weights": 1, "sight": 2}
+LOSS_WORKSPACE_BYTES = 16384    # EMER_LOSS_WORKSPACE_BYTES
+_LOSS_WS: Dict[object, Tensor] = {}
+
+
+def _loss_workspace(dev: torch.device) -> Tensor:
+    """The device's loss workspace: zeroed once, left zeroed by every call (the last CTA resets its ticket), so it is
+    shared by all loss calls on the device's stream and by graph replays.  Created outside graph capture."""
+    ws = _LOSS_WS.get(dev)
+    if ws is None:
+        if dev.type == "cuda" and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("emernerf_b200 losses: run each loss once before capturing it in a CUDA graph")
+        ws = torch.zeros(LOSS_WORKSPACE_BYTES // 4, dtype=torch.int32, device=dev)
+        _LOSS_WS[dev] = ws
+    return ws
+
+
+class _PointwiseLoss(torch.autograd.Function):
+    """post * mean(pre * term(a, b)) for one of LOSS_KINDS; b is a constant (target / mask) except for the entropy
+    loss, where it is the static density and gets a gradient."""
+
+    @staticmethod
+    def forward(ctx, a: Tensor, b: Optional[Tensor], kind: int, p0: float, p1: float, pre: float, post: float):
+        ctx.set_materialize_grads(False)
+        _need_cuda(a, b)
+        ac = _f32c(a)
+        bc = None if b is None else _f32c(b)
+        if bc is not None and bc.numel() != ac.numel():
+            raise ValueError(f"pointwise loss: {tuple(a.shape)} vs {tuple(b.shape)}")
+        out = torch.empty(2, dtype=torch.float32, device=ac.device)
+        _lib.call("emer_pointwise_loss_fwd", kind, _ptr(ac), _ptr(bc), ac.numel(), p0, p1, pre, post, _ptr(out),
+                  _ptr(_loss_workspace(ac.device)), _stream())
+        ctx.save_for_backward(ac, bc, out)
+        ctx.args = (kind, p0, p1, pre, post)
+        ctx.shapes = (a.shape, None if b is None else b.shape)
+        return out[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        need_a = ctx.needs_input_grad[0]
+        need_b = ctx.needs_input_grad[1] and ctx.args[0] == LOSS_KINDS["entropy"]
+        if g is None or not (need_a or need_b):
+            return None, None, None, None, None, None, None
+        a, b, out = ctx.saved_tensors
+        kind, p0, p1, pre, post = ctx.args
+        da = torch.empty_like(a) if need_a else None
+        db = torch.empty_like(b) if need_b else None
+        _lib.call("emer_pointwise_loss_bwd", kind, _ptr(a), _ptr(b), a.numel(), p0, p1, pre, post, _ptr(out),
+                  _ptr(_f32c(g)), _ptr(da), _ptr(db), _stream())
+        return (None if da is None else da.view(ctx.shapes[0]), None if db is None else db.view(ctx.shapes[1]),
+                None, None, None, None, None)
+
+
+def pointwise_loss(kind: str, a: Tensor, b: Optional[Tensor], p0: float = 0.0, p1: float = 0.0, pre: float = 1.0,
+                   post: float = 1.0) -> Tensor:
+    """0-d loss value; see EMER_LOSS_* in include/emer_b200.h for what ``kind`` computes and what p0 / p1 are."""
+    return _PointwiseLoss.apply(a, b, LOSS_KINDS[kind], float(p0), float(p1), float(pre), float(post))
+
+
+class _RayLoss(torch.autograd.Function):
+    """Per-ray sums over [R, S] rows (EMER_RAY_LOSS_*); differentiable w.r.t. the weights only."""
+
+    @staticmethod
+    def forward(ctx, w: Tensor, t: Optional[Tensor], gt: Tensor, kind: int, consts: Tuple[float, float, float],
+                pre: float, post: float):
+        ctx.set_materialize_grads(False)
+        _need_cuda(w, t, gt)
+        wc, gc = _f32c(w), _f32c(gt)
+        tc = None if t is None else _f32c(t)
+        r, s = wc.shape
+        if gc.numel() != r or (tc is not None and tc.shape != wc.shape):
+            raise ValueError(f"ray loss: weights {tuple(w.shape)}, t {None if t is None else tuple(t.shape)}, "
+                             f"per-ray {tuple(gt.shape)}")
+        out = torch.empty(2, dtype=torch.float32, device=wc.device)
+        _lib.call("emer_ray_loss_fwd", kind, _ptr(wc), _ptr(tc), _ptr(gc), r, s, *consts, pre, post, _ptr(out),
+                  _ptr(_loss_workspace(wc.device)), _stream())
+        ctx.save_for_backward(wc, tc, gc, out)
+        ctx.args = (kind, consts, pre, post)
+        return out[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        if g is None or not ctx.needs_input_grad[0]:
+            return None, None, None, None, None, None, None
+        w, t, gt, out = ctx.saved_tensors
+        kind, consts, pre, post = ctx.args
+        dw = torch.empty_like(w)
+        _lib.call("emer_ray_loss_bwd", kind, _ptr(w), _ptr(t), _ptr(gt), w.shape[0], w.shape[1], *consts, pre, post,
+                  _ptr(out), _ptr(_f32c(g)), _ptr(dw), _stream())
+        return dw, None, None, None, None, None, None
+
+
+def _sight_consts(epsilon: float) -> Tuple[float, float, float]:
+    """(epsilon, 2 sigma^2, 1 / sqrt(2 pi sigma^2)), sigma = epsilon / 3, in double as the reference's Python forms
+    them; ctypes rounds each once to fp32, as torch rounds a Python scalar."""
+    sigma = float(epsilon) / 3
+    return float(epsilon), 2 * sigma**2, 1 / (math.sqrt(2 * math.pi * sigma**2))
+
+
+def line_of_sight_loss(weights: Tensor, t_vals: Tensor, gt_depth: Tensor, epsilon: float, pre: float = 1.0,
+                       post: float = 1.0) -> Tensor:
+    """post * mean(pre * compute_line_of_sight_loss(gt_depth, weights, t_vals, epsilon)); t_vals and gt_depth are
+    constants."""
+    return _RayLoss.apply(weights, t_vals.detach(), gt_depth.detach(), RAY_LOSS_KINDS["line_of_sight"],
+                          _sight_consts(epsilon), float(pre), float(post))
+
+
+def line_of_sight_sum(weights: Tensor, t_vals: Tensor, gt_depth: Tensor, epsilon: float) -> Tensor:
+    """mean_r empty_r + mean_r near_r of compute_line_of_sight_loss (before its ray mask), a 0-d tensor."""
+    return _RayLoss.apply(weights, t_vals.detach(), gt_depth.detach(), RAY_LOSS_KINDS["sight"], _sight_consts(epsilon),
+                          1.0, 1.0)
+
+
+def sky_weights_loss(weights: Tensor, sky_mask: Tensor, post: float = 1.0) -> Tensor:
+    """post * mean_r(sum_s weights^2 * sky_mask_r)."""
+    return _RayLoss.apply(weights, None, sky_mask.detach(), RAY_LOSS_KINDS["sky_weights"], (0.0, 0.0, 0.0), 1.0,
+                          float(post))

@@ -288,6 +288,44 @@ int emer_adam_step(const emer_adam_block* blocks, const int64_t* prefix, int n_b
                    const float* hyper, float beta1, float beta2, float eps, float weight_decay, int zero_grad,
                    void* stream);
 
+/* ---- training losses (replaces the op-by-op torch of loss/base.py: RealValueLoss :83-146, SkyLoss :149-185,
+ *      DepthLoss :188-269, LineOfSightLoss :272-335 with compute_line_of_sight_loss :430-464,
+ *      DynamicRegularizationLoss :338-410), csrc/losses.cu ------------------------------------------------------------
+ * Forward: ONE launch, no host sync.  out [2] (caller-owned, per call) receives out[0] = the loss value and out[1] = the
+ * count its mean divides by (elements, valid rays, or rays with gt > 0), which the backward reads.  workspace: at least
+ * EMER_LOSS_WORKSPACE_BYTES of device memory, zeroed once by its owner; the kernel leaves it zeroed again, so it is
+ * reused by every call (and every CUDA-graph replay) on one stream -- calls that may run concurrently need separate
+ * workspaces.  Sums are per CTA, then over CTAs in a fixed order (no float atomics): bit-identical on one device.
+ * Backward: ONE launch; g is the upstream gradient (a device scalar); the gradients are WRITTEN (not accumulated).
+ * pre: per-element factor before the mean; post: factor after it (the loss's coef). */
+#define EMER_LOSS_WORKSPACE_BYTES 16384
+enum {
+    EMER_LOSS_L1 = 0, EMER_LOSS_L2 = 1, EMER_LOSS_SMOOTH_L1 = 2,    /* a = pred, b = target [n]; mean over n        */
+    EMER_LOSS_DEPTH_L1 = 3, EMER_LOSS_DEPTH_L2 = 4,                 /* a = pred, b = gt depth [n]; p0 = max depth:  */
+    EMER_LOSS_DEPTH_SMOOTH_L1 = 5,                                  /*   clamp(d / p0, 0, 1), mean over 0.01 < gt < p0 */
+    EMER_LOSS_SKY_BCE = 6,                                          /* a = opacity, b = sky mask: BCE(a, 1 - b)     */
+    EMER_LOSS_SPARSITY = 7,                                         /* a = density (b unused): mean(a)              */
+    EMER_LOSS_ENTROPY = 8                                           /* a = dynamic, b = static density; p0 = skewness
+                                                                       k, p1 = k - 1; da and/or db                  */
+};
+int emer_pointwise_loss_fwd(int kind, const float* a, const float* b, int64_t n, float p0, float p1, float pre,
+                            float post, float* out, void* workspace, void* stream);
+int emer_pointwise_loss_bwd(int kind, const float* a, const float* b, int64_t n, float p0, float p1, float pre,
+                            float post, const float* fwd_out, const float* g, float* da, float* db, void* stream);
+
+/* Per-ray sums over the S samples of [R, S] rows.
+ *   LINE_OF_SIGHT: w = weights, t = t_vals [R, S], gt = gt depth [R]; eps, two_sigma_sq = 2 (eps/3)^2,
+ *                  amp = 1 / sqrt(2 pi (eps/3)^2):  post * mean_r(pre * (mean_r empty_r + mean_r near_r) * [gt_r > 0])
+ *   SKY_WEIGHTS:   w = weights, t unused, gt = sky mask [R]:  post * mean_r(sum_s w^2 * sky_r)
+ *   SIGHT:         as LINE_OF_SIGHT without the ray mask and its mean: post * pre * (mean_r empty_r + mean_r near_r)
+ * dw [R, S] is d loss / d w. */
+enum { EMER_RAY_LOSS_LINE_OF_SIGHT = 0, EMER_RAY_LOSS_SKY_WEIGHTS = 1, EMER_RAY_LOSS_SIGHT = 2 };
+int emer_ray_loss_fwd(int kind, const float* w, const float* t, const float* gt, int64_t n_rays, int n_samples, float eps,
+                      float two_sigma_sq, float amp, float pre, float post, float* out, void* workspace, void* stream);
+int emer_ray_loss_bwd(int kind, const float* w, const float* t, const float* gt, int64_t n_rays, int n_samples, float eps,
+                      float two_sigma_sq, float amp, float pre, float post, const float* fwd_out, const float* g,
+                      float* dw, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
