@@ -12,9 +12,14 @@
 //   L * 2^D * F * 4 (corner reads) + D*4 (position) + L*F*4 (output)
 //   = 1452 B (3-D 10x4), 2736 B (4-D 10x4), 300 B (3-D 8x1).
 //
-// Mapping (forward): one thread per point, all levels in the thread.  A point's L*F outputs are
-// contiguous (160 B for 10x4), so a warp writes one dense 5 KB span; all 2^D corner gathers of a
-// level are issued back to back (16-byte LDG for F=4) before the first use.
+// Mapping (forward and table scatter): level-group-major, see level_group() below.  One thread per
+// (point, group of G levels); the launch is ordered so that the resident CTAs work on one group at
+// a time, and each hashed level's table (or its gradient slice) is read from HBM about once and
+// then served from L2.  The static 122 MB grid runs one level per group: 0.52 -> 0.35 ms (gather)
+// and 0.90 -> 0.49 ms (scatter) per 524 288 ray-coherent points against the point-major order
+// (H100 80GB HBM3, 400 W power limit).  All 2^D corner gathers of a level are issued back to back
+// (16-byte LDG for F=4) before the first use.  The input gradient (never needed in training) stays
+// one thread per point, all levels.
 #include "common.cuh"
 
 namespace emer {
@@ -47,14 +52,15 @@ __device__ __forceinline__ uint32_t grid_index(const uint32_t (&c)[D], uint32_t 
     return idx;
 }
 
+// Positions are streamed (evict-first), so they do not push table lines out of L2.
 template <int D>
 __device__ __forceinline__ void load_point(const float* __restrict__ x, int64_t i, float (&p)[D]) {
     if constexpr (D == 4) {
-        float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
+        float4 v = __ldcs(reinterpret_cast<const float4*>(x) + i);
         p[0] = v.x; p[1] = v.y; p[2] = v.z; p[3] = v.w;
     } else {
 #pragma unroll
-        for (int d = 0; d < D; ++d) p[d] = __ldg(x + i * D + d);
+        for (int d = 0; d < D; ++d) p[d] = __ldcs(x + i * D + d);
     }
 }
 
@@ -110,7 +116,22 @@ __device__ __forceinline__ void locate(const float (&p)[D], float scale, uint32_
     }
 }
 
-template <int D, int F>
+// Level-group schedule of the forward and the table scatter: a thread handles one point and G
+// consecutive levels, blockIdx.x is the point block and blockIdx.y the level group.  CTAs are
+// dispatched x-fastest, so the CTAs resident at any moment work on one group (two at a boundary),
+// and only those levels' tables compete for L2 instead of the whole grid.
+//
+// G: with F = 4 a hashed level of a 2^20-entry map is 16 MiB, and two such levels already thrash
+// H100's L2 (a pair of fine levels takes 1.2x the time of its two levels alone), so each level is
+// its own group, although a thread then writes half of a 32-byte output sector.  Narrower
+// features keep G*F = 8 floats, one whole sector per thread: the F = 1 proposal grids (8 levels,
+// 19-22 MB in all) fit L2 as a whole and run as a single group.
+template <int F>
+constexpr int level_group() {
+    return F == 4 ? 1 : 8 / F;
+}
+
+template <int D, int F, int G>
 __global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd,
                                                        const float* __restrict__ x,
                                                        const float* __restrict__ table,
@@ -119,10 +140,14 @@ __global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd,
     if (i >= n) return;
     const emer_grid_desc& g = gd.g;
     const int L = g.n_levels;
+    const int l0 = blockIdx.y * G;
     float p[D];
     load_point<D>(x, i, p);
     float* yo = y + i * (int64_t)(L * F);
-    for (int l = 0; l < L; ++l) {
+#pragma unroll
+    for (int j = 0; j < G; ++j) {
+        const int l = l0 + j;
+        if (l >= L) break;
         const float scale = g.scale[l];
         const uint32_t res = g.resolution[l];
         const uint32_t off = g.offset[l];
@@ -158,13 +183,14 @@ __global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd,
         for (int c = 0; c < (1 << D); ++c)
 #pragma unroll
             for (int f = 0; f < F; ++f) acc[f] = fmaf(wt[c], val[c].v[f], acc[f]);
+        // outputs are streamed: evict-first, so they do not push table lines out of L2
         if constexpr (F == 4) {
-            reinterpret_cast<float4*>(yo)[l] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+            __stcs(reinterpret_cast<float4*>(yo) + l, make_float4(acc[0], acc[1], acc[2], acc[3]));
         } else if constexpr (F == 2) {
-            reinterpret_cast<float2*>(yo)[l] = make_float2(acc[0], acc[1]);
+            __stcs(reinterpret_cast<float2*>(yo) + l, make_float2(acc[0], acc[1]));
         } else {
 #pragma unroll
-            for (int f = 0; f < F; ++f) yo[l * F + f] = acc[f];
+            for (int f = 0; f < F; ++f) __stcs(yo + l * F + f, acc[f]);
         }
     }
 }
@@ -194,48 +220,49 @@ __global__ void grid_indices_kernel(const GridDescDev gd, const float* __restric
     }
 }
 
-// Backward: one thread per point, all levels.  dtable is accumulated with vector reductions
-// (red.global.add.v4.f32 for F=4: one 16-byte L2 atomic per corner); dx is summed in registers.
+// Table gradient, on the level-group schedule of the forward.  dtable is accumulated with vector
+// reductions (red.global.add.v4.f32 for F=4: one 16-byte L2 atomic per corner) into the caller's
+// buffer, which is added to and never overwritten; the resident CTAs' reductions then land in
+// one group's gradient slices, which stay in L2.
 //
 // Ray-coherent batches put consecutive samples of a ray in consecutive lanes, and at the coarse
 // levels those samples share a cell, and same-address L2 reductions serialise.  So each
 // warp first looks for runs of adjacent lanes in the SAME cell; where there are any, the 2^D*F
 // partial sums of a run are combined with a segmented shuffle reduction and only the run's first
 // lane issues the reductions.
-template <int D, int F, bool WITH_TABLE, bool WITH_DX>
-__global__ void __launch_bounds__(256) grid_bwd_kernel(const GridDescDev gd,
-                                                       const float* __restrict__ x,
-                                                       const float* __restrict__ table,
-                                                       const float* __restrict__ dy,
-                                                       float* __restrict__ dtable,
-                                                       float* __restrict__ dx, int64_t n) {
+template <int D, int F, int G>
+__global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev gd,
+                                                             const float* __restrict__ x,
+                                                             const float* __restrict__ dy,
+                                                             float* __restrict__ dtable, int64_t n) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = i < n;                  // no early exit: warp collectives below
     const int lane = threadIdx.x & 31;
     const emer_grid_desc& g = gd.g;
     const int L = g.n_levels;
+    const int l0 = blockIdx.y * G;
     float p[D];
 #pragma unroll
     for (int d = 0; d < D; ++d) p[d] = 0.0f;
     if (active) load_point<D>(x, i, p);
     const float* dyo = dy + (active ? i : 0) * (int64_t)(L * F);
-    float gx[D];
 #pragma unroll
-    for (int d = 0; d < D; ++d) gx[d] = 0.0f;
-    for (int l = 0; l < L; ++l) {
+    for (int j = 0; j < G; ++j) {
+        const int l = l0 + j;
+        if (l >= L) break;                      // uniform over the grid
         float g_out[F];
 #pragma unroll
         for (int f = 0; f < F; ++f) g_out[f] = 0.0f;
-        if (active) {
+        if (active) {                           // streamed: evict-first
             if constexpr (F == 4) {
-                float4 t = __ldg(reinterpret_cast<const float4*>(dyo) + l);
+                float4 t = __ldcs(reinterpret_cast<const float4*>(dyo) + l);
                 g_out[0] = t.x; g_out[1] = t.y; g_out[2] = t.z; g_out[3] = t.w;
             } else if constexpr (F == 2) {
-                float2 t = __ldg(reinterpret_cast<const float2*>(dyo) + l);
+                float2 t = __ldcs(reinterpret_cast<const float2*>(dyo) + l);
                 g_out[0] = t.x; g_out[1] = t.y;
             } else {
 #pragma unroll
-                for (int f = 0; f < F; ++f) g_out[f] = __ldg(dyo + l * F + f);
+                for (int f = 0; f < F; ++f) g_out[f] = __ldcs(dyo + l * F + f);
             }
         }
         bool any = false;
@@ -257,102 +284,140 @@ __global__ void __launch_bounds__(256) grid_bwd_kernel(const GridDescDev gd,
             for (int d = 0; d < D; ++d) cc[d] = c0[d] + ((c >> d) & 1);
             idx[c] = grid_index<D>(cc, res, size, hashed);
         }
-        if constexpr (WITH_DX) {
-            if (any) {
-                const float* lt = table + (size_t)off * F;
-                // s[c] = <dy, table[corner c]>
-                float s[1 << D];
+        float* lt = dtable + (size_t)off * F;
+        // cell key, injective while (res+1)^D fits 32 bits (the coarse levels, where it matters)
+        const uint64_t radix = (uint64_t)res + 1u;
+        uint64_t span = 1;
 #pragma unroll
-                for (int c = 0; c < (1 << D); ++c) {
-                    Vec<F> v = load_entry<F>(lt, idx[c]);
-                    float t = 0.0f;
+        for (int d = 0; d < D; ++d) span *= radix;
+        const bool keyable = span < 0xFFFFFFFFull;
+        uint32_t key = 0xFFFFFFFFu;
+        if (active && keyable) {
+            key = 0;
 #pragma unroll
-                    for (int f = 0; f < F; ++f) t = fmaf(g_out[f], v.v[f], t);
-                    s[c] = t;
-                }
-#pragma unroll
-                for (int gdim = 0; gdim < D; ++gdim) {
-                    float acc = 0.0f;
-#pragma unroll
-                    for (int c = 0; c < (1 << D); ++c) {
-                        if ((c >> gdim) & 1) continue;     // c = "left" corner along gdim
-                        float t = scale;
-#pragma unroll
-                        for (int d = 0; d < D; ++d) {
-                            if (d == gdim) continue;
-                            t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
-                        }
-                        acc = fmaf(t, s[c | (1 << gdim)] - s[c], acc);
-                    }
-                    gx[gdim] += acc;
-                }
-            }
+            for (int d = D - 1; d >= 0; --d) key = key * (uint32_t)radix + c0[d];
         }
-        if constexpr (WITH_TABLE) {
-            float* lt = dtable + (size_t)off * F;
-            // cell key, injective while (res+1)^D fits 32 bits (the coarse levels, where it matters)
-            const uint64_t radix = (uint64_t)res + 1u;
-            uint64_t span = 1;
+        const uint32_t prev = __shfl_up_sync(0xffffffffu, key, 1);
+        const bool head = (lane == 0) || (key != prev) || !keyable;
+        const unsigned heads = __ballot_sync(0xffffffffu, head);
+        if (heads != 0xffffffffu) {
+            // at least one run of >= 2 lanes in the same cell: segmented suffix reduction
+            const unsigned later = (lane == 31) ? 0u : (heads >> (lane + 1));
+            const int run_end = later ? (lane + __ffs(later) - 1) : 31;
 #pragma unroll
-            for (int d = 0; d < D; ++d) span *= radix;
-            const bool keyable = span < 0xFFFFFFFFull;
-            uint32_t key = 0xFFFFFFFFu;
-            if (active && keyable) {
-                key = 0;
+            for (int c = 0; c < (1 << D); ++c) {
+                float t = 1.0f;
 #pragma unroll
-                for (int d = D - 1; d >= 0; --d) key = key * (uint32_t)radix + c0[d];
-            }
-            const uint32_t prev = __shfl_up_sync(0xffffffffu, key, 1);
-            const bool head = (lane == 0) || (key != prev) || !keyable;
-            const unsigned heads = __ballot_sync(0xffffffffu, head);
-            if (heads != 0xffffffffu) {
-                // at least one run of >= 2 lanes in the same cell: segmented suffix reduction
-                const unsigned later = (lane == 31) ? 0u : (heads >> (lane + 1));
-                const int run_end = later ? (lane + __ffs(later) - 1) : 31;
+                for (int d = 0; d < D; ++d) t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
+                float v[F];
 #pragma unroll
-                for (int c = 0; c < (1 << D); ++c) {
-                    float t = 1.0f;
+                for (int f = 0; f < F; ++f) v[f] = t * g_out[f];
 #pragma unroll
-                    for (int d = 0; d < D; ++d) t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
-                    float v[F];
+                for (int o = 1; o < 32; o <<= 1) {
 #pragma unroll
-                    for (int f = 0; f < F; ++f) v[f] = t * g_out[f];
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) {
-#pragma unroll
-                        for (int f = 0; f < F; ++f) {
-                            const float u = __shfl_down_sync(0xffffffffu, v[f], o);
-                            if (lane + o <= run_end) v[f] += u;
-                        }
+                    for (int f = 0; f < F; ++f) {
+                        const float u = __shfl_down_sync(0xffffffffu, v[f], o);
+                        if (lane + o <= run_end) v[f] += u;
                     }
-                    bool nz = false;
-#pragma unroll
-                    for (int f = 0; f < F; ++f) nz |= (v[f] != 0.0f);
-                    if (head && active && nz) red_add_entry<F>(lt, idx[c], v);
                 }
-            } else if (any) {
+                bool nz = false;
 #pragma unroll
-                for (int c = 0; c < (1 << D); ++c) {
-                    float t = 1.0f;
+                for (int f = 0; f < F; ++f) nz |= (v[f] != 0.0f);
+                if (head && active && nz) red_add_entry<F>(lt, idx[c], v);
+            }
+        } else if (any) {
 #pragma unroll
-                    for (int d = 0; d < D; ++d) t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
-                    float v[F];
+            for (int c = 0; c < (1 << D); ++c) {
+                float t = 1.0f;
 #pragma unroll
-                    for (int f = 0; f < F; ++f) v[f] = t * g_out[f];
-                    red_add_entry<F>(lt, idx[c], v);
-                }
+                for (int d = 0; d < D; ++d) t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
+                float v[F];
+#pragma unroll
+                for (int f = 0; f < F; ++f) v[f] = t * g_out[f];
+                red_add_entry<F>(lt, idx[c], v);
             }
         }
     }
-    if constexpr (WITH_DX) {
-        if (active) {
-            if constexpr (D == 4) {
-                reinterpret_cast<float4*>(dx)[i] = make_float4(gx[0], gx[1], gx[2], gx[3]);
-            } else {
+}
+
+// Input gradient: one thread per point, all levels, summed in registers (tcnn's dy/dx: the
+// derivative of the D-linear weights times the level's scale).
+template <int D, int F>
+__global__ void __launch_bounds__(256) grid_bwd_dx_kernel(const GridDescDev gd,
+                                                          const float* __restrict__ x,
+                                                          const float* __restrict__ table,
+                                                          const float* __restrict__ dy,
+                                                          float* __restrict__ dx, int64_t n) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const emer_grid_desc& g = gd.g;
+    const int L = g.n_levels;
+    float p[D];
+    load_point<D>(x, i, p);
+    const float* dyo = dy + i * (int64_t)(L * F);
+    float gx[D];
 #pragma unroll
-                for (int d = 0; d < D; ++d) dx[i * D + d] = gx[d];
-            }
+    for (int d = 0; d < D; ++d) gx[d] = 0.0f;
+    for (int l = 0; l < L; ++l) {
+        float g_out[F];
+        if constexpr (F == 4) {
+            float4 t = __ldg(reinterpret_cast<const float4*>(dyo) + l);
+            g_out[0] = t.x; g_out[1] = t.y; g_out[2] = t.z; g_out[3] = t.w;
+        } else if constexpr (F == 2) {
+            float2 t = __ldg(reinterpret_cast<const float2*>(dyo) + l);
+            g_out[0] = t.x; g_out[1] = t.y;
+        } else {
+#pragma unroll
+            for (int f = 0; f < F; ++f) g_out[f] = __ldg(dyo + l * F + f);
         }
+        bool any = false;
+#pragma unroll
+        for (int f = 0; f < F; ++f) any |= (g_out[f] != 0.0f);
+        if (!any) continue;
+        const float scale = g.scale[l];
+        const uint32_t res = g.resolution[l];
+        const uint32_t off = g.offset[l];
+        const uint32_t size = g.offset[l + 1] - off;
+        const bool hashed = g.hashed[l] != 0;
+        const float* lt = table + (size_t)off * F;
+        uint32_t c0[D];
+        float w[D];
+        locate<D>(p, scale, c0, w);
+        // s[c] = <dy, table[corner c]>
+        float s[1 << D];
+#pragma unroll
+        for (int c = 0; c < (1 << D); ++c) {
+            uint32_t cc[D];
+#pragma unroll
+            for (int d = 0; d < D; ++d) cc[d] = c0[d] + ((c >> d) & 1);
+            Vec<F> v = load_entry<F>(lt, grid_index<D>(cc, res, size, hashed));
+            float t = 0.0f;
+#pragma unroll
+            for (int f = 0; f < F; ++f) t = fmaf(g_out[f], v.v[f], t);
+            s[c] = t;
+        }
+#pragma unroll
+        for (int gdim = 0; gdim < D; ++gdim) {
+            float acc = 0.0f;
+#pragma unroll
+            for (int c = 0; c < (1 << D); ++c) {
+                if ((c >> gdim) & 1) continue;     // c = "left" corner along gdim
+                float t = scale;
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    if (d == gdim) continue;
+                    t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
+                }
+                acc = fmaf(t, s[c | (1 << gdim)] - s[c], acc);
+            }
+            gx[gdim] += acc;
+        }
+    }
+    if constexpr (D == 4) {
+        reinterpret_cast<float4*>(dx)[i] = make_float4(gx[0], gx[1], gx[2], gx[3]);
+    } else {
+#pragma unroll
+        for (int d = 0; d < D; ++d) dx[i * D + d] = gx[d];
     }
 }
 
@@ -383,6 +448,14 @@ static int validate(const emer_grid_desc* g) {
 
 using namespace emer;
 
+template <int D, int F>
+static void launch_fwd(const GridDescDev& gd, const float* x, const float* table, float* y, int64_t n,
+                       cudaStream_t st) {
+    constexpr int G = level_group<F>();
+    const dim3 blocks((unsigned)ceil_div(n, 256), (unsigned)ceil_div(gd.g.n_levels, G));
+    grid_fwd_kernel<D, F, G><<<blocks, 256, 0, st>>>(gd, x, table, y, n);
+}
+
 extern "C" int emer_grid_fwd(const emer_grid_desc* g, const float* x, const float* table, float* y,
                              int64_t n, void* stream) {
     if (int e = validate(g)) return e;
@@ -392,14 +465,12 @@ extern "C" int emer_grid_fwd(const emer_grid_desc* g, const float* x, const floa
                  "emer_grid_fwd: pointers must be 16-byte aligned");
     GridDescDev gd{*g};
     cudaStream_t st = (cudaStream_t)stream;
-    const int threads = 256;
-    const unsigned blocks = (unsigned)ceil_div(n, threads);
-    DISPATCH_DF(3, 1, (grid_fwd_kernel<D, F><<<blocks, threads, 0, st>>>(gd, x, table, y, n)))
-    DISPATCH_DF(3, 2, (grid_fwd_kernel<D, F><<<blocks, threads, 0, st>>>(gd, x, table, y, n)))
-    DISPATCH_DF(3, 4, (grid_fwd_kernel<D, F><<<blocks, threads, 0, st>>>(gd, x, table, y, n)))
-    DISPATCH_DF(4, 1, (grid_fwd_kernel<D, F><<<blocks, threads, 0, st>>>(gd, x, table, y, n)))
-    DISPATCH_DF(4, 2, (grid_fwd_kernel<D, F><<<blocks, threads, 0, st>>>(gd, x, table, y, n)))
-    DISPATCH_DF(4, 4, (grid_fwd_kernel<D, F><<<blocks, threads, 0, st>>>(gd, x, table, y, n)))
+    DISPATCH_DF(3, 1, (launch_fwd<D, F>(gd, x, table, y, n, st)))
+    DISPATCH_DF(3, 2, (launch_fwd<D, F>(gd, x, table, y, n, st)))
+    DISPATCH_DF(3, 4, (launch_fwd<D, F>(gd, x, table, y, n, st)))
+    DISPATCH_DF(4, 1, (launch_fwd<D, F>(gd, x, table, y, n, st)))
+    DISPATCH_DF(4, 2, (launch_fwd<D, F>(gd, x, table, y, n, st)))
+    DISPATCH_DF(4, 4, (launch_fwd<D, F>(gd, x, table, y, n, st)))
     return check_launch("emer_grid_fwd");
 }
 
@@ -415,14 +486,17 @@ extern "C" int emer_grid_indices(const emer_grid_desc* g, const float* x, int32_
     return check_launch("emer_grid_indices");
 }
 
+// Both gradients requested: two launches, the table scatter then the input gradient.
 template <int D, int F>
 static void launch_bwd(const GridDescDev& gd, const float* x, const float* table, const float* dy,
                        float* dtable, float* dx, int64_t n, cudaStream_t st) {
-    const int threads = 256;
-    const unsigned blocks = (unsigned)ceil_div(n, threads);
-    if (dtable && dx) grid_bwd_kernel<D, F, true, true><<<blocks, threads, 0, st>>>(gd, x, table, dy, dtable, dx, n);
-    else if (dtable) grid_bwd_kernel<D, F, true, false><<<blocks, threads, 0, st>>>(gd, x, table, dy, dtable, dx, n);
-    else grid_bwd_kernel<D, F, false, true><<<blocks, threads, 0, st>>>(gd, x, table, dy, dtable, dx, n);
+    const unsigned blocks = (unsigned)ceil_div(n, 256);
+    if (dtable) {
+        constexpr int G = level_group<F>();
+        const dim3 grid(blocks, (unsigned)ceil_div(gd.g.n_levels, G));
+        grid_bwd_table_kernel<D, F, G><<<grid, 256, 0, st>>>(gd, x, dy, dtable, n);
+    }
+    if (dx) grid_bwd_dx_kernel<D, F><<<blocks, 256, 0, st>>>(gd, x, table, dy, dx, n);
 }
 
 extern "C" int emer_grid_bwd(const emer_grid_desc* g, const float* x, const float* table,

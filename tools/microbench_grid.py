@@ -4,7 +4,8 @@
 
 Points are the real sample positions of one render pass of the bench model (proposal-resampled, so
 consecutive lanes of a warp are consecutive samples of a ray).  Each level is timed alone through a
-one-level descriptor, then the full grid; CUDA events, 20 repetitions after 3 warm-ups."""
+one-level descriptor, then a few consecutive-level pairs (whether two hashed levels still share L2),
+then the full grid; CUDA events, 20 repetitions after 3 warm-ups."""
 import argparse
 import ctypes
 import os
@@ -30,15 +31,18 @@ def timeit(fn, reps=20, warm=3):
     return e0.elapsed_time(e1) / reps
 
 
-def one_level(desc: GridDesc, l: int) -> GridDesc:
+def sub_desc(desc: GridDesc, l0: int, l1: int) -> GridDesc:
+    """Levels l0 .. l1-1 of ``desc``, addressing the same table storage."""
     d = GridDesc.__new__(GridDesc)
-    d.n_dims, d.n_levels, d.n_feat = desc.n_dims, 1, desc.n_feat
-    d.scales, d.resolutions = [desc.scales[l]], [desc.resolutions[l]]
-    d.offsets, d.hashed = [desc.offsets[l], desc.offsets[l + 1]], [desc.hashed[l]]
+    d.n_dims, d.n_levels, d.n_feat = desc.n_dims, l1 - l0, desc.n_feat
+    d.scales, d.resolutions = desc.scales[l0:l1], desc.resolutions[l0:l1]
+    d.offsets, d.hashed = desc.offsets[l0:l1 + 1], desc.hashed[l0:l1]
     c = type(desc.c)()
-    c.n_dims, c.n_levels, c.n_feat = desc.n_dims, 1, desc.n_feat
-    c.scale[0], c.resolution[0], c.hashed[0] = desc.scales[l], desc.resolutions[l], int(desc.hashed[l])
-    c.offset[0], c.offset[1] = desc.offsets[l], desc.offsets[l + 1]
+    c.n_dims, c.n_levels, c.n_feat = desc.n_dims, l1 - l0, desc.n_feat
+    for j, l in enumerate(range(l0, l1)):
+        c.scale[j], c.resolution[j], c.hashed[j] = desc.scales[l], desc.resolutions[l], int(desc.hashed[l])
+        c.offset[j] = desc.offsets[l]
+    c.offset[l1 - l0] = desc.offsets[l1]
     d.c = c
     return d
 
@@ -67,8 +71,11 @@ def main():
     print(f"points {n}, inside-cube fraction {inside:.3f}")
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     P = lambda t_: ctypes.c_void_p(t_.data_ptr())
-    for l in list(range(desc.n_levels)) + [-1]:
-        d = desc if l < 0 else one_level(desc, l)
+    spans = [(l, l + 1) for l in range(desc.n_levels)]
+    spans += [(l, l + 2) for l in (3, 5, 7) if l + 2 <= desc.n_levels]
+    sums = [0.0, 0.0]
+    for l0, l1 in spans + [(0, desc.n_levels)]:
+        d = sub_desc(desc, l0, l1)
         y = torch.empty(n, d.n_output_dims, device=dev)
         dy = torch.randn(n, d.n_output_dims, device=dev)
         dt = torch.zeros_like(table)
@@ -76,7 +83,15 @@ def main():
         b = timeit(lambda: _lib.call("emer_grid_bwd", ctypes.byref(d.c), P(x), P(table), P(dy), P(dt), None, n, st))
         xr = torch.rand_like(x)
         br = timeit(lambda: _lib.call("emer_grid_bwd", ctypes.byref(d.c), P(xr), P(table), P(dy), P(dt), None, n, st))
-        name = "all" if l < 0 else f"L{l} res={desc.resolutions[l]:5d} {'hash' if desc.hashed[l] else 'dense'}"
+        if l1 - l0 == 1:
+            sums[0] += f
+            sums[1] += b
+            name = f"L{l0} res={desc.resolutions[l0]:5d} {'hash' if desc.hashed[l0] else 'dense'}"
+        elif l1 - l0 == desc.n_levels:
+            print(f"{'sum of single levels':22s} fwd {sums[0] * 1e3:8.1f} us   bwd(table) {sums[1] * 1e3:8.1f} us")
+            name = "all"
+        else:
+            name = f"L{l0}+L{l1 - 1}"
         print(f"{name:22s} fwd {f * 1e3:8.1f} us   bwd(table) {b * 1e3:8.1f} us   bwd on uniform-random points {br * 1e3:8.1f} us")
 
 
