@@ -34,7 +34,6 @@ _SIGNATURES = {
     "emer_linear_tc_bwd_data": [_P, c_int64, _P, c_int64, c_int, _P, _P, c_int64, _P, c_int64, c_int, c_int64, c_int,
                                 c_int, c_int, _P],
     "emer_linear_tc_bwd_weight": [_P, c_int64, _P, c_int64, _P, _P, c_int64, c_int, c_int, _P],
-    "emer_linear_tc_bwd_weight_mn": [_P, c_int64, _P, c_int64, _P, _P, c_int64, c_int, c_int, _P],
     "emer_pdf_resample": [_P, _P, c_int, c_int, _P, c_float, c_float, c_int, _P, _P, _P, c_int64, _P],
     "emer_prop_level": [POINTER(EmerGridDesc), _P, _P, c_int, c_int, _P, c_float, c_float, c_int, _P, _P, _P, c_int, _P,
                         _P, _P, _P, _P, _P, _P, _P, _P, c_int64, _P],
@@ -124,7 +123,7 @@ def tag_of(name: str, args) -> str:
             return f"k{args[7]}_o{args[8]}_N{args[6]}"
         if name == "emer_linear_bwd_data":
             return f"k{args[9]}_o{args[10]}_N{args[8]}"
-        if name in ("emer_linear_tc_bwd_weight", "emer_linear_tc_bwd_weight_mn"):
+        if name == "emer_linear_tc_bwd_weight":
             return f"k{args[7]}_o{args[8]}_N{args[6]}"
         if name == "emer_linear_bwd_weight":
             return f"k{args[10]}_o{args[11]}_N{args[9]}"

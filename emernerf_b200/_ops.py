@@ -25,8 +25,8 @@ ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
 # fp32 CUDA-core kernels of linear_simt.cu (the bit-faithful checker); both are sm_90a code in the
 # same library -- this is a debugging switch, not a backend dispatch.
 LINEAR_IMPL = os.environ.get("EMER_LINEAR", "tc")
-LINEAR_WGRAD_IMPL = os.environ.get("EMER_LINEAR_WGRAD", "mn")      # "mn" / "tc": the tensor-core weight gradient (csrc/wgrad_mn.cu,
-                                                                   # through either entry point); "simt"
+LINEAR_WGRAD_IMPL = os.environ.get("EMER_LINEAR_WGRAD", "tc")      # "simt": the FFMA weight gradient; anything else: the
+                                                                   # tensor-core one (csrc/wgrad_mn.cu)
 SKIP_BWD_IMPL = os.environ.get("EMER_SKIP_BWD", "stack")   # "stack": one stacked product; "add": two + add
 TC_MIN_ROWS = int(os.environ.get("EMER_TC_MIN_ROWS", "1024"))   # below: the FP32-FMA kernels (tiny per-ray heads are launch-bound either way)
 STOT_KINDS = {"uniform": 0, "lindisp": 1, "sqrt": 2, "log": 3, "uniform_lindisp": 4, "uniform_lindisp_0": 5}
@@ -330,21 +330,8 @@ def _tc_fits(kred: int, ncols: int) -> bool:
 
 
 def _tc_wgrad_fits(k: int, n_out: int) -> bool:
-    """Same for the tensor-core weight gradient (emer_linear_tc_bwd_weight): the layer widths it is used for.  (The
-    kernel takes any k <= 256, n_out <= 128; this keeps the routing the library has always had.)"""
-    if n_out > 128 or k > 256:
-        return False
-    k_pad4, n_pad, m_blocks = _round_up(k, 4), _round_up(n_out, 16), (k + 127) // 128
-    if m_blocks * 2 * n_pad > 512:
-        return False
-    a_rows = 64 if k_pad4 <= 64 else 128
-    for w_rows, nbuf, raw_stages in ((64, 2, 2), (64, 2, 1), (32, 2, 2), (32, 2, 1), (64, 1, 2), (64, 1, 1)):
-        rq = w_rows // 4
-        ops1 = 2 * (m_blocks * rq * (a_rows * 16 + 16)) + 2 * (rq * (n_pad * 16 + 16))
-        raw1 = w_rows * (k_pad4 + n_pad) * 4
-        if nbuf * ops1 + raw_stages * raw1 + 4 * 8 + 16 + 2048 <= _SMEM_MAX:
-            return True
-    return False
+    """Same for the tensor-core weight gradient (emer_linear_tc_bwd_weight, csrc/wgrad_mn.cu)."""
+    return k <= 256 and n_out <= 128
 
 
 def _tc_rows_ok(n: int) -> bool:
@@ -397,14 +384,10 @@ def _layer_bwd_weight(x2: Tensor, ldx: int, dz: Tensor, lddz: int, w: Tensor, ha
         db = b_sink[0]
     else:
         db = torch.zeros(n_out, dtype=torch.float32, device=w.device)
-    tc = (_tc_rows_ok(n) and LINEAR_WGRAD_IMPL in ("tc", "mn") and _tc_wgrad_fits(k, n_out) and n_out % 4 == 0
+    tc = (_tc_rows_ok(n) and LINEAR_WGRAD_IMPL != "simt" and _tc_wgrad_fits(k, n_out) and n_out % 4 == 0
           and _aligned(x2, ldx) and _aligned(dz, lddz) and _pad4(k) <= ldx)
     if _narrow_ok(k, n_out):
         _lib.call("emer_linear_narrow_bwd_weight", _ptr(x2), ldx, _ptr(dz), lddz, _ptr(dw), _ptr(db), n, k, n_out,
-                  _stream())
-    elif tc and LINEAR_WGRAD_IMPL == "mn" and n_out == 64 and 4 <= k <= 128:
-        # the field chain's 64-wide layers (csrc/wgrad_mn.cu)
-        _lib.call("emer_linear_tc_bwd_weight_mn", _ptr(x2), ldx, _ptr(dz), lddz, _ptr(dw), _ptr(db), n, k, n_out,
                   _stream())
     elif tc:
         _lib.call("emer_linear_tc_bwd_weight", _ptr(x2), ldx, _ptr(dz), lddz, _ptr(dw), _ptr(db), n, k, n_out,
@@ -675,13 +658,6 @@ CHAIN_BWD = os.environ.get("EMER_CHAIN_BWD", "fused")          # "layers": data 
 CHAIN_K_ENC = (32, 40, 64)
 
 
-def _field_wgrad_usable(t: Tensor) -> bool:
-    """Whether the fused chain's weight gradients take the one-launch ``emer_field_wgrad``: tensors on the GPU.  The CPU
-    harness of the C ABI (tests/cabi_emulator.py) runs the same data path on host memory; there they go through the
-    per-layer weight-gradient entry points it answers."""
-    return t.is_cuda
-
-
 def _tc_bwd_data_acc(dz: Tensor, lddz: int, w: Tensor, dx: Tensor, lddx: int, n: int) -> None:
     """dx[n, k] += dz[n, n_out] @ w on the tensor-core layer kernel (accumulating form)."""
     n_out, k = w.shape
@@ -694,10 +670,12 @@ class _FieldChain(torch.autograd.Function):
     colour head in one kernel (``emer_field_fwd``, csrc/field_fused.cu).  ``ray_bias`` [R, 128] carries the per-ray
     input columns of the colour head and its first two biases (see :func:`field_chain`).
 
-    Backward: the data gradients walk the chain with the tensor-core layer kernels on the saved activations
+    Backward: the data gradients come from one kernel (``emer_field_bwd``) or -- ragged rays, batches below
+    ``TC_MIN_ROWS``, ``EMER_CHAIN_BWD=layers`` -- from a walk over the saved activations with the layer kernels
     ([h0 | geo] side by side, so layer 1 of the head is one 64 -> 128 product and the skip gradient accumulates in
-    place); ``d_ray_bias`` is the per-ray sum of the two hidden-layer gradients, which hands the per-ray weight
-    columns, the biases and the embedding their gradients through ordinary autograd."""
+    place).  Either way the five layers' weight gradients then come from one ``emer_field_wgrad`` launch over the
+    buffers the data path left.  ``d_ray_bias`` is the per-ray sum of the two hidden-layer gradients, which hands the
+    per-ray weight columns, the biases and the embedding their gradients through ordinary autograd."""
 
     @staticmethod
     def forward(ctx, enc: Tensor, ray_bias: Tensor, samples: int, want_geo: bool, wb0: Tensor, bb0: Tensor, wb1: Tensor,
@@ -751,8 +729,7 @@ class _FieldChain(torch.autograd.Function):
         w1hg = torch.cat([w1[:, :64], w1[:, 64 + n_ray_cols:]], dim=1)            # [64, 128] = [hidden | geo] columns
         w0g = w0[:, n_ray_cols:].contiguous()
         D1 = torch.empty((n, 128), **f32)          # [dZ0 | dF] side by side (row stride 128)
-        dw2 = db2 = dw1hg = dw0g = dz2 = dz1 = d_rb = d_enc = None
-        fused_data = False
+        dz2 = dz1 = d_rb = d_enc = None
         c = lambda g, w: None if g is None else _f32c(g.reshape(n, w))
         d_geo, d_sem = c(d_geo, 64), c(d_sem, 64)
         if CHAIN_BWD == "fused" and samples % 32 == 0 and _tc_rows_ok(n):
@@ -769,18 +746,14 @@ class _FieldChain(torch.autograd.Function):
                       _ptr(hg), _ptr(h1), _ptr(wb0), k_enc, _ptr(wb1), n_feat, _ptr(w0g), 64, _ptr(w1hg), _ptr(w1hg[:, 64:]),
                       128, _ptr(w2), _ptr(dz2), _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_enc), k_enc, _ptr(d_rb), samples, n,
                       _stream())
-            fused_data = True
         else:
             # ---- layer by layer on the same buffers (ragged rays, tiny batches, EMER_CHAIN_BWD=layers)
             if d_rgb is not None:
                 dz2 = _f32c(d_rgb.reshape(n, 3)) * (rgb * (1.0 - rgb))
-                dw2, db2 = _layer_bwd_weight(h1, 64, dz2, 3, w2, True, n, sk["w2"], sk["b2"])
                 dz1 = torch.empty((n, 64), **f32)
                 _layer_bwd_data(dz2, 3, w2, dz1, 64, n, h1, 64, 64)                   # relu'(h1) applied
-                dw1hg, _ = _layer_bwd_weight(hg, 128, dz1, 64, w1hg, False, n)
                 _layer_bwd_data(dz1, 64, w1hg, D1, 128, n, hg, 128, 64)               # [relu'(h0) dH0 | dGeo(layer 1)]
                 dz0 = D1[:, :64]
-                dw0g, _ = _layer_bwd_weight(hg[:, 64:], 128, dz0, 128, w0g, False, n)
                 if _tc_rows_ok(n):
                     _tc_bwd_data_acc(dz0, 128, w0g, D1[:, 64:], 128, n)              # dGeo += dZ0 W0g
                 else:
@@ -801,14 +774,11 @@ class _FieldChain(torch.autograd.Function):
             if d_sigma is not None:
                 # trunc_exp backward (nerf_utils.py:72-75): g * exp(clamp(x, max=15)), x = feats[:, 0] - 1 = log(sigma)
                 dgeo[:, 0] += _f32c(d_sigma).reshape(n) * torch.clamp(sigma, max=3269017.25)
-        one_launch = fused_data and _field_wgrad_usable(enc2)
-        if not one_launch:
             # [dF | d_sem]: the gradient of the base MLP's output (zeros for an absent semantic half)
             if n_feat == 128:
                 dfe = torch.cat([D1[:, 64:], torch.zeros((n, 64), **f32) if d_sem is None else d_sem], dim=1)
             else:
                 dfe = D1[:, 64:]
-        if not fused_data:
             dzb = torch.empty((n, 64), **f32)
             _layer_bwd_data(dfe, 128, wb1, dzb, 64, n, hb, 64, 64)
             if ctx.needs_input_grad[0]:
@@ -816,74 +786,48 @@ class _FieldChain(torch.autograd.Function):
                 _layer_bwd_data(dzb, 64, wb0, d_enc, d_enc.shape[1], n, None, 0, 0)
                 d_enc = d_enc[:, :k_enc]
 
-        if not one_launch:
-            # X^T dZ layer by layer; the head's geo / hidden column blocks, its per-ray columns get their gradient
-            # through ray_bias
-            if fused_data and d_rgb is not None:
-                dw2, db2 = _layer_bwd_weight(h1, 64, dz2, 3, w2, True, n, sk["w2"], sk["b2"])
-                dw1hg, _ = _layer_bwd_weight(hg, 128, dz1, 64, w1hg, False, n)
-                dw0g, _ = _layer_bwd_weight(hg[:, 64:], 128, D1[:, :64], 128, w0g, False, n)
-            dw0 = dw1 = None
-            if d_rgb is not None:
-                if sk["w0"] is not None:
-                    sk["w0"][0][:, n_ray_cols:].add_(dw0g)
-                    sk["w0"][1]()
-                else:
-                    dw0 = torch.zeros_like(w0)
-                    dw0[:, n_ray_cols:] = dw0g
-                if sk["w1"] is not None:
-                    sk["w1"][0][:, :64].add_(dw1hg[:, :64])
-                    sk["w1"][0][:, 64 + n_ray_cols:].add_(dw1hg[:, 64:])
-                    sk["w1"][1]()
-                else:
-                    dw1 = torch.zeros_like(w1)
-                    dw1[:, :64] = dw1hg[:, :64]
-                    dw1[:, 64 + n_ray_cols:] = dw1hg[:, 64:]
-            dwb1, dbb1 = _layer_bwd_weight(hb, 64, dfe, 128, wb1, True, n, sk["wb1"], sk["bb1"])
-            dwb0, dbb0 = _layer_bwd_weight(enc2, ld_enc, dzb, 64, wb0, True, n, sk["wb0"], sk["bb0"])
-        else:
-            shapes = dict(wb0=wb0.shape, bb0=(64,), wb1=wb1.shape, bb1=(n_feat,), w0=w0.shape, w1=w1.shape, w2=w2.shape,
-                          b2=(3,))
-            keys = list(shapes) if dz2 is not None else ["wb0", "bb0", "wb1", "bb1"]
-            side = WGRAD_STREAM and all(v is not None for v in sk.values()) and enc2.is_cuda
+        shapes = dict(wb0=wb0.shape, bb0=(64,), wb1=wb1.shape, bb1=(n_feat,), w0=w0.shape, w1=w1.shape, w2=w2.shape,
+                      b2=(3,))
+        keys = list(shapes) if dz2 is not None else ["wb0", "bb0", "wb1", "bb1"]
+        side = WGRAD_STREAM and all(v is not None for v in sk.values())
 
-            def weight_gradients(deferred):
-                """The five layers' X^T dZ in one emer_field_wgrad launch, accumulated into the optimizer's buffers (or
-                into zeros shaped like the parameters, returned to autograd).  ``deferred``: the side stream's list of
-                updates to run after the join -- the head's w0 / w1 gradients then go to zeros and are added there,
-                because autograd adds the per-ray columns' gradient to the same buffers on the main stream with an
-                in-place add of the whole tensor, which would race the kernel's atomics."""
-                out, grads = {}, {}
-                for k in keys:
-                    s = sk[k]
-                    if s is None:
-                        out[k] = grads[k] = torch.zeros(shapes[k], **f32)
-                    elif deferred is not None and k in ("w0", "w1"):
-                        out[k] = torch.zeros(shapes[k], **f32)
-                        deferred.append(lambda dst=s[0], src=out[k]: dst.add_(src))
-                    else:
-                        out[k] = s[0]
-                o = lambda k: _ptr(out[k]) if k in out else None
-                if dz2 is not None:        # the head's geo / hidden column blocks; the per-ray ones come through ray_bias
-                    w0g_d, ld_w0, w1g_d, ld_w1 = out["w0"][:, n_ray_cols:], out["w0"].stride(0), out["w1"][:, 64 + n_ray_cols:], out["w1"].stride(0)
+        def weight_gradients(deferred):
+            """The five layers' X^T dZ in one emer_field_wgrad launch, accumulated into the optimizer's buffers (or
+            into zeros shaped like the parameters, returned to autograd).  ``deferred``: the side stream's list of
+            updates to run after the join -- the head's w0 / w1 gradients then go to zeros and are added there,
+            because autograd adds the per-ray columns' gradient to the same buffers on the main stream with an
+            in-place add of the whole tensor, which would race the kernel's atomics."""
+            out, grads = {}, {}
+            for k in keys:
+                s = sk[k]
+                if s is None:
+                    out[k] = grads[k] = torch.zeros(shapes[k], **f32)
+                elif deferred is not None and k in ("w0", "w1"):
+                    out[k] = torch.zeros(shapes[k], **f32)
+                    deferred.append(lambda dst=s[0], src=out[k]: dst.add_(src))
                 else:
-                    w0g_d, ld_w0, w1g_d, ld_w1 = None, 0, None, 0
-                _lib.call("emer_field_wgrad", _ptr(enc2), ld_enc, k_enc, _ptr(hb), _ptr(hg), _ptr(h1), _ptr(dz2),
-                          _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_sem), n_feat, o("wb0"), o("bb0"), o("wb1"), o("bb1"),
-                          _ptr(w0g_d), ld_w0, o("w1"), _ptr(w1g_d), ld_w1, o("w2"), o("b2"), n, _stream())
-                for k in keys:
-                    if sk[k] is not None:
-                        sk[k][1]()
-                return tuple(grads.get(k) for k in ("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"))
-
-            if side:
-                # every weight gradient lands in the optimizer's buffers: nothing autograd waits for, so the kernel may
-                # run beside the hash-grid scatter / the table's reduce-scatter (joined by FusedAdam.step /
-                # DataParallel.reduce)
-                with _on_side_stream(dev, enc2, hb, hg, h1, dz2, dz1, D1, dzb, d_sem):
-                    dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(_AFTER_JOIN)
+                    out[k] = s[0]
+            o = lambda k: _ptr(out[k]) if k in out else None
+            if dz2 is not None:        # the head's geo / hidden column blocks; the per-ray ones come through ray_bias
+                w0g_d, ld_w0, w1g_d, ld_w1 = out["w0"][:, n_ray_cols:], out["w0"].stride(0), out["w1"][:, 64 + n_ray_cols:], out["w1"].stride(0)
             else:
-                dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(None)
+                w0g_d, ld_w0, w1g_d, ld_w1 = None, 0, None, 0
+            _lib.call("emer_field_wgrad", _ptr(enc2), ld_enc, k_enc, _ptr(hb), _ptr(hg), _ptr(h1), _ptr(dz2),
+                      _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_sem), n_feat, o("wb0"), o("bb0"), o("wb1"), o("bb1"),
+                      _ptr(w0g_d), ld_w0, o("w1"), _ptr(w1g_d), ld_w1, o("w2"), o("b2"), n, _stream())
+            for k in keys:
+                if sk[k] is not None:
+                    sk[k][1]()
+            return tuple(grads.get(k) for k in ("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"))
+
+        if side:
+            # every weight gradient lands in the optimizer's buffers: nothing autograd waits for, so the kernel may
+            # run beside the hash-grid scatter / the table's reduce-scatter (joined by FusedAdam.step /
+            # DataParallel.reduce)
+            with _on_side_stream(dev, enc2, hb, hg, h1, dz2, dz1, D1, dzb, d_sem):
+                dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(_AFTER_JOIN)
+        else:
+            dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(None)
         if d_enc is not None:
             d_enc = d_enc.reshape(enc_shape)
         return d_enc, d_rb, None, None, dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2

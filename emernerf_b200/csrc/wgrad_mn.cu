@@ -1,6 +1,5 @@
 // Weight gradients  dW[n_out, k] += dZ^T X,  db += column sums of dZ,  on Hopper warpgroup MMA (3xTF32, tc_common.cuh).
-// Entry points: emer_linear_tc_bwd_weight (any n_out <= 128, k <= 256) and emer_linear_tc_bwd_weight_mn (the 64-wide
-// layers of the field chain, read as they lie in memory: row-major X and dZ); both run wgrad_kernel.
+// Entry point: emer_linear_tc_bwd_weight (any k <= 256, n_out <= 128; X and dZ read row-major, as they lie in memory).
 // D[k x n_out] = X^T dZ: A = X^T straight from the row-major X (the 8 lanes with the same q read one 32-byte sector of
 // a row), B = dZ^T staged per tile into K-major panels; D stays in registers across the persistent CTA's tiles and is
 // flushed once with atomics (DESIGN.md §5.3).  HBM-bound: (k + n_out) * 4 B per row.
@@ -147,15 +146,4 @@ extern "C" int emer_linear_tc_bwd_weight(const float* x, int64_t ldx, const floa
     EMER_REQUIRE((n_out + 3) / 4 * 4 <= lddz, "emer_linear_tc_bwd_weight: dZ rows too short");
     emer::wg::Params p{x, ldx, k, dz, lddz, n_out, dw, db, n};
     return emer::wg::launch(p, (cudaStream_t)stream, "emer_linear_tc_bwd_weight");
-}
-
-extern "C" int emer_linear_tc_bwd_weight_mn(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw, float* db,
-                                            int64_t n, int k, int n_out, void* stream) {
-    if (n == 0) return 0;
-    EMER_REQUIRE(x && dz && dw, "emer_linear_tc_bwd_weight_mn: NULL pointer");
-    EMER_REQUIRE(n_out == 64 && k >= 4 && k <= 128, "emer_linear_tc_bwd_weight_mn: shape k=%d n_out=%d (need n_out = 64, k <= 128)", k, n_out);
-    EMER_REQUIRE(ldx % 4 == 0 && lddz % 4 == 0 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)dz & 15) == 0 && (k + 3) / 4 * 4 <= ldx,
-                 "emer_linear_tc_bwd_weight_mn: rows must be 16-byte aligned");
-    emer::wg::Params p{x, ldx, k, dz, lddz, n_out, dw, db, n};
-    return emer::wg::launch(p, (cudaStream_t)stream, "emer_linear_tc_bwd_weight_mn");
 }

@@ -181,11 +181,6 @@ int emer_field_tail_bwd(const float* feats, int64_t ld_feats, float* d_out, int6
                         const float* d_sigma, const int64_t* idx, float* d_emb, int e_dim, int64_t n_rays,
                         int n_samples, void* stream);
 
-/* Same contract and kernel as emer_linear_tc_bwd_weight, for the field chain's layers: n_out == 64, k <= 128
- * (csrc/wgrad_mn.cu). */
-int emer_linear_tc_bwd_weight_mn(const float* x, int64_t ldx, const float* dz, int64_t lddz, float* dw, float* db,
-                                 int64_t n, int k, int n_out, void* stream);
-
 /* ---- the fused field chain (csrc/field_fused.cu): base MLP -> density + colour head in ONE wgmma kernel with the
  *      activations in registers.  Replaces the chain of nn.Linear / torch.cat / trunc_exp / sigmoid calls of
  *      radiance_fields/radiance_field.py:74-80,314-318 (base_mlp), :422 (density), :131-143,622-658 (query_rgb) and

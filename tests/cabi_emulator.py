@@ -240,34 +240,17 @@ def emer_linear_bwd_weight(x, ldx, dy, lddy, y, ldy, act, dw, db, n, k, n_out, s
 
 
 def _check_tc_wgrad(x, ldx, dz, lddz, k, n_out):
-    """The limits within which _ops sends a weight gradient to emer_linear_tc_bwd_weight (wgrad_mn.cu takes any
-    k <= 256, n_out <= 128 with aligned rows), restated independently of _ops."""
+    """emer_linear_tc_bwd_weight's EMER_REQUIREs (csrc/wgrad_mn.cu), restated independently of _ops."""
     _require(n_out <= 128 and k <= 256, f"emer_linear_tc_bwd_weight: widths k={k} n_out={n_out} out of range")
     _require(ldx % 4 == 0 and lddz % 4 == 0 and _aligned16(x, dz), "emer_linear_tc_bwd_weight: rows must be 16-byte aligned")
-    _require(_r(k, 4) <= ldx and _r(n_out, 4) <= lddz, "emer_linear_tc_bwd_weight: row stride shorter than the padded width")
-    m_blocks, n_pad, k4 = (k + 127) // 128, _r(n_out, 16), _r(k, 4)
-    _require(m_blocks * 2 * n_pad <= 512, "emer_linear_tc_bwd_weight: accumulator does not fit")
-    a_panel, b_panel = (64 if k4 <= 64 else 128) * 16 + 16, n_pad * 16 + 16
-    fits = False
-    for rows, nbuf, stages in ((64, 2, 2), (64, 2, 1), (32, 2, 2), (32, 2, 1), (64, 1, 2), (64, 1, 1)):
-        ops = 2 * m_blocks * (rows // 4) * a_panel + 2 * (rows // 4) * b_panel           # hi + lo of A and of B
-        fits = fits or nbuf * ops + stages * rows * (k4 + n_pad) * 4 + 48 + 2048 <= 227 * 1024
-    _require(fits, f"emer_linear_tc_bwd_weight: layer {k}x{n_out} does not fit shared memory")
+    _require(_r(k, 4) <= ldx, "emer_linear_tc_bwd_weight: row stride shorter than the padded width")
+    _require(_r(n_out, 4) <= lddz, "emer_linear_tc_bwd_weight: dZ rows too short")
 
 
 def emer_linear_tc_bwd_weight(x, ldx, dz, lddz, dw, db, n, k, n_out, stream):
     if n == 0:
         return
     _check_tc_wgrad(x, ldx, dz, lddz, k, n_out)
-    _bwd_weight(_view(x, n, k, ldx), _view(dz, n, n_out, lddz), _view(dw, n_out, k), _vec(db, n_out))
-
-
-def emer_linear_tc_bwd_weight_mn(x, ldx, dz, lddz, dw, db, n, k, n_out, stream):
-    if n == 0:
-        return
-    _require(n_out == 64 and 4 <= k <= 128, f"emer_linear_tc_bwd_weight_mn: shape k={k} n_out={n_out} (need n_out = 64, k <= 128)")
-    _require(ldx % 4 == 0 and lddz % 4 == 0 and _aligned16(x, dz) and (k + 3) // 4 * 4 <= ldx,
-             "emer_linear_tc_bwd_weight_mn: rows must be 16-byte aligned")
     _bwd_weight(_view(x, n, k, ldx), _view(dz, n, n_out, lddz), _view(dw, n_out, k), _vec(db, n_out))
 
 
@@ -572,6 +555,31 @@ def emer_field_bwd(d_rgb, rgb, d_sigma, sigma, d_geo, d_sem, hb, hg, h1, wb0, k_
             acc[:, 64:].index_add_(0, ray, z1)
 
 
+def emer_field_wgrad(enc, ld_enc, k_enc, hb, hg, h1, dz2, dz1, d1, dzb, d_sem, n_feat, dwb0, dbb0, dwb1, dbb1, dw0g, ld_w0,
+                     dw1h, dw1g, ld_w1, dw2, db2, n, stream):
+    if n == 0:
+        return
+    _require(all(_addr(p) for p in (enc, hb, d1, dzb, dwb0, dbb0, dwb1, dbb1)), "emer_field_wgrad: NULL pointer")
+    _require(not _addr(dz2) or all(_addr(p) for p in (hg, h1, dz1, dw0g, dw1h, dw1g, dw2, db2)),
+             "emer_field_wgrad: NULL pointer among the colour head's buffers")
+    _require(k_enc in (32, 40, 64) and n_feat in (64, 128), "emer_field_wgrad: bad shape")
+    _require(not _addr(d_sem) or n_feat == 128, "emer_field_wgrad: d_sem needs n_feat = 128")
+    _require(ld_enc % 4 == 0 and ld_enc >= k_enc, "emer_field_wgrad: ld_enc")
+    _require(not _addr(dz2) or (ld_w0 >= 64 and ld_w1 >= 64), "emer_field_wgrad: ld_w0 / ld_w1 shorter than a block")
+    _require(_aligned16(enc, hb, hg, h1, dz2, dz1, d1, dzb, d_sem), "emer_field_wgrad: row buffers must be 16-byte aligned")
+    D1, hb_ = _view(d1, n, 128), _view(hb, n, 64)
+    _bwd_weight(_view(enc, n, k_enc, ld_enc), _view(dzb, n, 64), _view(dwb0, 64, k_enc), _vec(dbb0, 64))
+    _bwd_weight(hb_, D1[:, 64:], _view(dwb1, 64, 64), _vec(dbb1, 64))
+    if _addr(d_sem):
+        _bwd_weight(hb_, _view(d_sem, n, 64), _view(_addr(dwb1) + 64 * 64 * 4, 64, 64), _vec(_addr(dbb1) + 64 * 4, 64))
+    if _addr(dz2):
+        h0, geo, z1 = _view(hg, n, 64, 128), _view(_addr(hg) + 64 * 4, n, 64, 128), _view(dz1, n, 64)
+        _bwd_weight(geo, D1[:, :64], _view(dw0g, 64, 64, ld_w0), None)
+        _bwd_weight(h0, z1, _view(dw1h, 64, 64, ld_w1), None)
+        _bwd_weight(geo, z1, _view(dw1g, 64, 64, ld_w1), None)
+        _bwd_weight(_view(h1, n, 64), _view(dz2, n, 3), _view(dw2, 3, 64), _vec(db2, 3))
+
+
 # ----------------------------------------------------------------------------- ray generation
 def emer_gen_rays(img_idx, x, y, c2w, intrinsics, per_ray_mats, timestamps, height, width, origins, viewdirs, norms,
                   pixel_coords, out_times, n, stream):
@@ -640,4 +648,5 @@ def install(monkeypatch) -> None:
     monkeypatch.setattr(_ops, "_stream", lambda: None)
     monkeypatch.setattr(_ops, "on_device", lambda t: True)
     monkeypatch.setattr(_ops, "TC_MIN_ROWS", 64)       # send the larger layers through the tensor-core entry points
+    monkeypatch.setattr(_ops, "WGRAD_STREAM", False)   # host memory has no side stream
     del CALLS[:]

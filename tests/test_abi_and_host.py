@@ -163,7 +163,7 @@ def test_sorted_interp_quad_searchsorted_equals_dense_mask():
             #  network only through w_prop)
 
 
-def test_tensor_core_eligibility_mirrors_the_library_limits():
+def test_tensor_core_eligibility_matches_the_library_limits():
     """_ops only sends a layer to the tensor-core kernels when the library can take it (csrc/linear_tc.cu launch<>,
     emer_linear_tc_bwd_weight); the emulator carries an independent restatement of the same limits, so a
     disagreement between the two shows up here before it can on the GPU."""
@@ -176,9 +176,10 @@ def test_tensor_core_eligibility_mirrors_the_library_limits():
     for k, n_out in ((40, 64), (64, 64), (64, 128), (113, 64), (177, 64), (49, 64), (32, 64)):
         assert _ops._tc_fits(k, n_out) and _ops._tc_fits(n_out, k) and _ops._tc_wgrad_fits(k, n_out), (k, n_out)
     assert _ops._tc_fits(128, 113)                       # stacked skip gradient [dZ0 | dZ1] [W0 ; W1[:, h:]]
+    assert _ops._tc_wgrad_fits(256, 128)                # the widest weight gradient the library takes
     # layers the resident weight panels / accumulators cannot hold
     assert not _ops._tc_fits(256, 256) and not _ops._tc_fits(113, 256) and not _ops._tc_fits(64, 384)
-    assert not _ops._tc_wgrad_fits(256, 128) and not _ops._tc_wgrad_fits(64, 256) and not _ops._tc_wgrad_fits(369, 64)
+    assert not _ops._tc_wgrad_fits(64, 256) and not _ops._tc_wgrad_fits(369, 64) and not _ops._tc_wgrad_fits(300, 64)
 
     buf = (ctypes.c_float * 64)()
     ptr = ctypes.c_void_p((ctypes.addressof(buf) + 15) // 16 * 16)

@@ -1,5 +1,5 @@
 """emer_field_wgrad (csrc/field_wgrad.cu): the fused field chain's five weight gradients in one launch, against fp64
-dZ^T X and column sums, with the bars of test_gpu_kernels.py::test_weight_gradient_mn_major_operands."""
+dZ^T X and column sums, with the bars of test_gpu_kernels.py::test_tc_weight_gradient_row_major_operands."""
 import pytest
 import torch
 

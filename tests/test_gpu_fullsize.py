@@ -263,7 +263,7 @@ def test_full_size_gradients_and_proposal_loss(variant):
     loss = adapters.parity_loss(fc.mask_rays(out, keep))
     assert abs(loss.item() - g.scalar("train/loss")) < 1e-4 * max(1.0, abs(g.scalar("train/loss")))
     (_, names) = _launch_names(loss.backward)
-    assert "emer_linear_tc_bwd_weight" in names or "emer_field_bwd" in names, names
+    assert ("emer_linear_tc_bwd_weight" in names or "emer_field_bwd" in names) and "emer_field_wgrad" in names, names
     want, want_proj = g.tensors("train/grad/field"), g.tensors("train/gradproj/field")
     checked = 0
     for k, v in field.named_parameters():
@@ -293,7 +293,7 @@ def _check_projection(grad, want, name):
 
 def test_full_size_training_steps_fused_optimizer_and_side_stream(monkeypatch):
     """Three training steps of the full-size static model, twice from the same start: (A) torch.optim.Adam with ordinary
-    autograd gradients, (B) FusedAdam with the gradient sinks, the fused backward kernel, MN-major weight gradients and
+    autograd gradients, (B) FusedAdam with the gradient sinks, the fused backward kernel and
     the weight gradients on the side stream.  Adam with eps = 1e-15 turns every non-zero gradient into a +-lr step, so
     the trajectories are compared robustly: identical update support, > 99.9 % of the entries within 1e-4 of each other
     (an entry whose gradient is rounding noise may step the other way), losses equal to 1e-5."""
@@ -316,12 +316,10 @@ def test_full_size_training_steps_fused_optimizer_and_side_stream(monkeypatch):
             p.grad = None
         if fused:
             monkeypatch.setattr(_ops, "CHAIN_BWD", "fused")
-            monkeypatch.setattr(_ops, "LINEAR_WGRAD_IMPL", "mn")
             monkeypatch.setattr(_ops, "WGRAD_STREAM", True)
             opt = FusedAdam(field.parameters(), **adam)
         else:
             monkeypatch.setattr(_ops, "CHAIN_BWD", "layers")
-            monkeypatch.setattr(_ops, "LINEAR_WGRAD_IMPL", "tc")
             monkeypatch.setattr(_ops, "WGRAD_STREAM", False)
             opt = torch.optim.Adam(field.parameters(), **adam)
         losses = []

@@ -191,7 +191,7 @@ def test_linear_wgrad_tc_matches_simt(monkeypatch):
     from emernerf_b200 import _ops
 
     g = torch.Generator(device=DEV).manual_seed(3)
-    for k, n_out, act in ((177, 64, 1), (64, 128, 0), (40, 64, 1), (64, 3, 2)):
+    for k, n_out, act in ((177, 64, 1), (64, 128, 0), (40, 64, 1), (64, 3, 2), (256, 128, 0)):
         n = 64 * 1500 + 21
         x = torch.randn(n, k, device=DEV, generator=g)
         w = (torch.randn(n_out, k, device=DEV, generator=g) / k ** 0.5)
@@ -697,8 +697,8 @@ def test_gen_rays_matches_the_reference_formula():
 
 @pytest.mark.parametrize("k,n,ldx,lddz", [(64, 64 * 1500 + 21, 64, 64), (40, 128 * 700 + 5, 40, 64), (128, 64 * 900 + 63, 128, 64),
                                           (64, 37, 128, 128), (100, 64 * 400, 104, 64), (64, 524288, 128, 128)])
-def test_weight_gradient_mn_major_operands(k, n, ldx, lddz):
-    """emer_linear_tc_bwd_weight_mn (csrc/wgrad_mn.cu: operands read as they lie in memory, row-major X and dZ)
+def test_tc_weight_gradient_row_major_operands(k, n, ldx, lddz):
+    """emer_linear_tc_bwd_weight (csrc/wgrad_mn.cu: operands read as they lie in memory, row-major X and dZ)
     against fp64: dW and db within 2e-5 of the sum over all rows; ragged last tile, strided
     rows, k not a multiple of 32, accumulation into a non-zero buffer."""
     import ctypes
@@ -712,7 +712,7 @@ def test_weight_gradient_mn_major_operands(k, n, ldx, lddz):
     dw0, db0 = torch.randn(64, k, device=DEV, generator=g), torch.randn(64, device=DEV, generator=g)
     dw, db = dw0.clone(), db0.clone()
     _ops._need_cuda(x)
-    _lib.call("emer_linear_tc_bwd_weight_mn", _ops._ptr(x), ldx, _ops._ptr(dz), lddz, _ops._ptr(dw), _ops._ptr(db), n, k, 64,
+    _lib.call("emer_linear_tc_bwd_weight", _ops._ptr(x), ldx, _ops._ptr(dz), lddz, _ops._ptr(dw), _ops._ptr(db), n, k, 64,
               _ops._stream())
     want_w = dw0.double() + dz.double().T @ x.double()
     want_b = db0.double() + dz.double().sum(0)
