@@ -210,7 +210,7 @@ int emer_field_fwd(const float* enc, int64_t ld_enc, int k_enc, const float* wb0
  *   dzb[N,64] = (dF wb1[:64] + d_sem wb1[64:]) * (hb > 0);  d_enc[N, k_enc] = dzb wb0   (row stride ld_denc)
  *   d_ray_bias[R,128] += per-ray sums of [dz0 | dz1]   (caller zeroes; needs samples % 32 == 0; may be NULL)
  * hb / hg / h1 / rgb / sigma are emer_field_fwd's saves and outputs.  d_rgb, d_sigma, d_geo, d_sem, d_enc, dz2 may be
- * NULL.  Row buffers 32-byte aligned, ld_denc % 8 == 0.  The weight gradients are X^T dZ products over dz2 / dz1 / d1 /
+ * NULL; without d_rgb, dz2 is not written.  Row buffers 32-byte aligned, ld_denc % 8 == 0.  The weight gradients are X^T dZ products over dz2 / dz1 / d1 /
  * dzb (emer_field_wgrad). */
 int emer_field_bwd(const float* d_rgb, const float* rgb, const float* d_sigma, const float* sigma,
                    const float* d_geo, const float* d_sem, const float* hb, const float* hg, const float* h1,

@@ -514,6 +514,8 @@ def emer_field_fwd(enc, ld_enc, k_enc, wb0, bb0, wb1, bb1, n_feat, w0g, ld_w0, w
 
 def emer_field_bwd(d_rgb, rgb, d_sigma, sigma, d_geo, d_sem, hb, hg, h1, wb0, k_enc, wb1, n_feat, w0g, ld_w0, w1h, w1g,
                    ld_w1, w2, dz2, dz1, d1, dzb, d_enc, ld_denc, d_ray_bias, samples, n, stream):
+    _require(all(_addr(p) for p in (rgb, sigma, hb, hg, h1, wb0, wb1, w0g, w1h, w1g, w2, dz1, d1, dzb)),
+             "emer_field_bwd: NULL pointer")
     _require(k_enc in (32, 40, 64) and n_feat in (64, 128) and samples > 0, "emer_field_bwd: bad shape")
     _require(not _addr(d_enc) or (ld_denc % 8 == 0 and ld_denc >= k_enc), "emer_field_bwd: d_enc rows must be 32-byte aligned")
     _require(_aligned32(hb, hg, h1, dz1, d1, dzb, d_enc, d_geo, d_sem), "emer_field_bwd: row buffers must be 32-byte aligned")
@@ -525,8 +527,8 @@ def emer_field_bwd(d_rgb, rgb, d_sigma, sigma, d_geo, d_sem, hb, hg, h1, wb0, k_
         if _addr(d_rgb):
             y = _view(rgb, n, 3)
             z2 = _view(d_rgb, n, 3) * (y * (1.0 - y))
-        if _addr(dz2):
-            _view(dz2, n, 3).copy_(z2)
+            if _addr(dz2):                  # (without d_rgb the library leaves dz2 as it is)
+                _view(dz2, n, 3).copy_(z2)
         z1 = (z2 @ _view(w2, 3, 64)) * (_view(h1, n, 64) > 0)
         _view(dz1, n, 64).copy_(z1)
         h0 = _view(hg, n, 64, 128)
