@@ -59,6 +59,8 @@ _SIGNATURES = {
     "emer_ray_loss_fwd": [c_int, _P, _P, _P, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, _P, _P, _P],
     "emer_ray_loss_bwd": [c_int, _P, _P, _P, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, _P, _P, _P,
                           _P],
+    "emer_cycle_loss_fwd": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, _P, _P, _P],
+    "emer_cycle_loss_bwd": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, _P, _P, _P, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])
@@ -135,6 +137,8 @@ def tag_of(name: str, args) -> str:
             return f"kind{args[0]}_N{args[3]}"
         if name in ("emer_ray_loss_fwd", "emer_ray_loss_bwd"):
             return f"kind{args[0]}_R{args[4]}_S{args[5]}"
+        if name in ("emer_cycle_loss_fwd", "emer_cycle_loss_bwd"):
+            return f"N{args[8]}"
         if name == "emer_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("_save" if args[19].value else "")
     except Exception:

@@ -1248,3 +1248,51 @@ def sky_weights_loss(weights: Tensor, sky_mask: Tensor, post: float = 1.0) -> Te
     """post * mean_r(sum_s weights^2 * sky_mask_r)."""
     return _RayLoss.apply(weights, None, sky_mask.detach(), RAY_LOSS_KINDS["sky_weights"], (0.0, 0.0, 0.0), 1.0,
                           float(post))
+
+
+class _CycleLoss(torch.autograd.Function):
+    """coef * 0.5 * mean((f + fpb)^2 + (b + bpf)^2) over [..., 3] flows, and the four maximum row norms
+    (emer_cycle_loss_*).  Column slices of wider rows are read in place; f and b are constants."""
+
+    @staticmethod
+    def forward(ctx, f: Tensor, b: Tensor, fpb: Tensor, bpf: Tensor, coef: float):
+        ctx.set_materialize_grads(False)
+        _need_cuda(f, b, fpb, bpf)
+        if not (f.shape == b.shape == fpb.shape == bpf.shape) or f.dim() == 0 or f.shape[-1] != 3:
+            raise ValueError(f"flow cycle loss: flows of shapes {tuple(f.shape)}, {tuple(b.shape)}, "
+                             f"{tuple(fpb.shape)}, {tuple(bpf.shape)}; all must be the same [..., 3]")
+        if f.numel() == 0:
+            raise ValueError("flow cycle loss: no samples (the maximum flow norms of an empty batch are undefined)")
+        rows = [_rows(t, 3) for t in (f, b, fpb, bpf)]
+        args = [a for r in rows for a in (_ptr(r[0]), r[1])]
+        n = rows[0][0].shape[0]
+        out = torch.empty(6, dtype=torch.float32, device=rows[0][0].device)
+        _lib.call("emer_cycle_loss_fwd", *args, n, coef, _ptr(out), _ptr(_loss_workspace(out.device)), _stream())
+        ctx.save_for_backward(*(r[0] for r in rows), out)
+        ctx.lds = [r[1] for r in rows]
+        ctx.coef, ctx.shape = coef, fpb.shape
+        stats = out[2:]
+        ctx.mark_non_differentiable(stats)
+        return out[0], stats
+
+    @staticmethod
+    def backward(ctx, g, _g_stats):
+        need_fpb, need_bpf = ctx.needs_input_grad[2], ctx.needs_input_grad[3]
+        if g is None or not (need_fpb or need_bpf):
+            return None, None, None, None, None
+        f, b, fpb, bpf, out = ctx.saved_tensors
+        n = f.shape[0]
+        d_fpb = torch.empty(n, 3, dtype=torch.float32, device=f.device) if need_fpb else None
+        d_bpf = torch.empty(n, 3, dtype=torch.float32, device=f.device) if need_bpf else None
+        args = [a for t, ld in zip((f, b, fpb, bpf), ctx.lds) for a in (_ptr(t), ld)]
+        _lib.call("emer_cycle_loss_bwd", *args, n, ctx.coef, _ptr(out), _ptr(_f32c(g)), _ptr(d_fpb), _ptr(d_bpf),
+                  _stream())
+        view = lambda d: None if d is None else d.view(ctx.shape)
+        return None, None, view(d_fpb), view(d_bpf), None
+
+
+def cycle_loss(forward_flow: Tensor, backward_flow: Tensor, forward_pred_backward_flow: Tensor,
+               backward_pred_forward_flow: Tensor, coef: float) -> Tuple[Tensor, Tensor]:
+    """(0-d loss value, [4] maximum row norms of the four flows in argument order; no gradient)."""
+    return _CycleLoss.apply(forward_flow.detach(), backward_flow.detach(), forward_pred_backward_flow,
+                            backward_pred_forward_flow, float(coef))

@@ -1,7 +1,8 @@
 // The training losses of the reference's loss/base.py, value and gradient, one launch each way per loss call.
 //
 // Reference: RealValueLoss (:83-146), SkyLoss (:149-185), DepthLoss (:188-269), LineOfSightLoss (:272-335) with
-// compute_line_of_sight_loss (:430-464), DynamicRegularizationLoss (:338-410).  Op by op those are elementwise torch
+// compute_line_of_sight_loss (:430-464), DynamicRegularizationLoss (:338-410), and the flow variants' cycle loss with
+// its four flow statistics (train_emernerf.py:700-740).  Op by op those are elementwise torch
 // calls, masks, boolean indexing (DepthLoss: a nonzero and a device-to-host sync) and means; the line-of-sight loss
 // alone is ~30 launches each way.  Here:
 //   forward : grid-stride pass over the elements (pointwise) or one warp per ray (per-ray sums over the S samples);
@@ -23,8 +24,13 @@ struct LossWorkspace {
     unsigned int ticket;             // zero between calls: the last CTA resets it
     unsigned int pad[15];
     float sum_a[LOSS_MAX_CTAS];
-    float sum_b[LOSS_MAX_CTAS];
-    long long count[LOSS_MAX_CTAS];
+    union {
+        struct {
+            float sum_b[LOSS_MAX_CTAS];
+            long long count[LOSS_MAX_CTAS];
+        };
+        unsigned int norm_max[4][LOSS_MAX_CTAS];     // the cycle loss's four statistics (it needs no sum_b / count)
+    };
 };
 static_assert(sizeof(LossWorkspace) <= EMER_LOSS_WORKSPACE_BYTES, "workspace layout exceeds the ABI size");
 
@@ -113,12 +119,38 @@ __device__ __forceinline__ T block_sum(T v, T* sh) {
     return t;
 }
 
+// Maximum of one CTA; valid in thread 0.
+__device__ __forceinline__ unsigned int block_max(unsigned int v, unsigned int* sh) {
+    v = __reduce_max_sync(0xffffffffu, v);
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    __syncthreads();
+    if (lane == 0) sh[wid] = v;
+    __syncthreads();
+    unsigned int t = 0u;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < LOSS_WARPS; ++w) t = max(t, sh[w]);
+    return t;
+}
+
+// Called by every thread after thread 0 has stored its CTA's partials: true in every thread of the CTA that takes the
+// last ticket, which then sees all partials.
+__device__ bool last_cta(LossWorkspace* ws) {
+    __shared__ bool last;
+    if (threadIdx.x == 0) {
+        __threadfence();
+        last = atomicAdd(&ws->ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return false;
+    __threadfence();
+    return true;
+}
+
 // Every CTA publishes its partials; the one that takes the last ticket adds them up in CTA order.  Returns true in
 // thread 0 of that CTA, with the totals in a / b / c.
 __device__ bool reduce_across_ctas(LossWorkspace* ws, float& a, float& b, long long& c) {
     __shared__ float shf[LOSS_WARPS];
     __shared__ long long shc[LOSS_WARPS];
-    __shared__ bool last;
     a = block_sum(a, shf);
     b = block_sum(b, shf);
     c = block_sum(c, shc);
@@ -126,12 +158,8 @@ __device__ bool reduce_across_ctas(LossWorkspace* ws, float& a, float& b, long l
         ws->sum_a[blockIdx.x] = a;
         ws->sum_b[blockIdx.x] = b;
         ws->count[blockIdx.x] = c;
-        __threadfence();
-        last = atomicAdd(&ws->ticket, 1u) == gridDim.x - 1;
     }
-    __syncthreads();
-    if (!last) return false;
-    __threadfence();
+    if (!last_cta(ws)) return false;
     a = 0.0f; b = 0.0f; c = 0;
     for (int i = threadIdx.x; i < (int)gridDim.x; i += LOSS_THREADS) {
         a += __ldcg(ws->sum_a + i);
@@ -291,6 +319,107 @@ __global__ void __launch_bounds__(LOSS_THREADS) ray_loss_bwd_kernel(const LossPa
     }
 }
 
+// ---------------------------------------------------------------------------------------------- flow cycle loss
+// train_emernerf.py:700-740 of the reference, over n rows of 3 (R * S samples):
+//   value = coef * (0.5 * mean((f + fpb)^2 + (b + bpf)^2)), the mean over all 3n elements
+//   stats = max_row |f|, |b|, |fpb|, |bpf|
+// Each input is a [n, 3] view with its own row stride (a column slice of the flow MLP's output rows).
+enum { CYC_F = 0, CYC_B = 1, CYC_FPB = 2, CYC_BPF = 3 };
+
+struct CycleParams {
+    const float* x[4];       // forward flow, backward flow, forward-predicted backward, backward-predicted forward
+    int64_t ld[4];
+    int64_t n;
+    float coef;
+    float* out;              // [6]: value, count, the four maxima in the order of x
+    LossWorkspace* ws;
+    const float* g;          // backward: upstream gradient (device scalar)
+    float* d_fpb;            // backward: [n, 3] contiguous, or null
+    float* d_bpf;
+};
+
+__device__ __forceinline__ float3 cycle_row(const CycleParams& p, int k, int64_t i) {
+    const float* r = p.x[k] + i * p.ld[k];
+    return make_float3(__ldg(r), __ldg(r + 1), __ldg(r + 2));
+}
+
+// |v| as an unsigned key with the order of the floats: a non-negative float orders as its bits, and clearing the
+// sign bit sends every NaN above +inf, so the maximum is NaN when any row is (as torch.max)
+__device__ __forceinline__ unsigned int norm_key(float3 v) {
+    return __float_as_uint(sqrtf(v.x * v.x + v.y * v.y + v.z * v.z)) & 0x7fffffffu;
+}
+
+__device__ __forceinline__ float cycle_term(float f, float p, float b, float q) {
+    const float u = f + p, w = b + q;
+    return u * u + w * w;
+}
+
+__global__ void __launch_bounds__(LOSS_THREADS) cycle_loss_fwd_kernel(const CycleParams p) {
+    __shared__ float shf[LOSS_WARPS];
+    __shared__ unsigned int shu[LOSS_WARPS];
+    float sum = 0.0f;
+    unsigned int mx[4] = {0u, 0u, 0u, 0u};
+    for (int64_t i = (int64_t)blockIdx.x * LOSS_THREADS + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * LOSS_THREADS) {
+        const float3 f = cycle_row(p, CYC_F, i), b = cycle_row(p, CYC_B, i);
+        const float3 fp = cycle_row(p, CYC_FPB, i), bp = cycle_row(p, CYC_BPF, i);
+        sum += cycle_term(f.x, fp.x, b.x, bp.x);
+        sum += cycle_term(f.y, fp.y, b.y, bp.y);
+        sum += cycle_term(f.z, fp.z, b.z, bp.z);
+        mx[CYC_F] = max(mx[CYC_F], norm_key(f));
+        mx[CYC_B] = max(mx[CYC_B], norm_key(b));
+        mx[CYC_FPB] = max(mx[CYC_FPB], norm_key(fp));
+        mx[CYC_BPF] = max(mx[CYC_BPF], norm_key(bp));
+    }
+    sum = block_sum(sum, shf);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) mx[k] = block_max(mx[k], shu);
+    if (threadIdx.x == 0) {
+        p.ws->sum_a[blockIdx.x] = sum;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) p.ws->norm_max[k][blockIdx.x] = mx[k];
+    }
+    if (!last_cta(p.ws)) return;
+    sum = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) mx[k] = 0u;
+    for (int c = threadIdx.x; c < (int)gridDim.x; c += LOSS_THREADS) {
+        sum += __ldcg(p.ws->sum_a + c);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) mx[k] = max(mx[k], __ldcg(p.ws->norm_max[k] + c));
+    }
+    sum = block_sum(sum, shf);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) mx[k] = block_max(mx[k], shu);
+    if (threadIdx.x == 0) {
+        p.ws->ticket = 0u;
+        const float count = (float)(p.n * 3);
+        p.out[0] = 0.5f * (sum / count) * p.coef;
+        p.out[1] = count;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) p.out[2 + k] = __uint_as_float(mx[k]);
+    }
+}
+
+__global__ void __launch_bounds__(LOSS_THREADS) cycle_loss_bwd_kernel(const CycleParams p) {
+    const float gs = __ldg(p.g) * p.coef * 0.5f / __ldg(p.out + 1);         // torch's chain: coef, 0.5, the mean
+    for (int64_t i = (int64_t)blockIdx.x * LOSS_THREADS + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * LOSS_THREADS) {
+        if (p.d_fpb) {
+            const float3 f = cycle_row(p, CYC_F, i), fp = cycle_row(p, CYC_FPB, i);
+            float* d = p.d_fpb + i * 3;
+            d[0] = 2.0f * (f.x + fp.x) * gs;
+            d[1] = 2.0f * (f.y + fp.y) * gs;
+            d[2] = 2.0f * (f.z + fp.z) * gs;
+        }
+        if (p.d_bpf) {
+            const float3 b = cycle_row(p, CYC_B, i), bp = cycle_row(p, CYC_BPF, i);
+            float* d = p.d_bpf + i * 3;
+            d[0] = 2.0f * (b.x + bp.x) * gs;
+            d[1] = 2.0f * (b.y + bp.y) * gs;
+            d[2] = 2.0f * (b.z + bp.z) * gs;
+        }
+    }
+}
+
 // persistent grid: at most two CTAs per SM (and the workspace's LOSS_MAX_CTAS partials)
 static int loss_grid(int64_t work_items, int per_cta) {
     int64_t blocks = ceil_div(work_items, per_cta);
@@ -352,4 +481,43 @@ extern "C" int emer_ray_loss_bwd(int kind, const float* w, const float* t, const
                  nullptr};
     ray_loss_bwd_kernel<<<loss_grid(n_rays * n_samples, LOSS_THREADS), LOSS_THREADS, 0, (cudaStream_t)stream>>>(p);
     return check_launch("emer_ray_loss_bwd");
+}
+
+static CycleParams cycle_params(const float* f, int64_t ld_f, const float* b, int64_t ld_b, const float* fpb,
+                                int64_t ld_fpb, const float* bpf, int64_t ld_bpf, int64_t n, float coef) {
+    CycleParams p{};
+    p.x[CYC_F] = f; p.x[CYC_B] = b; p.x[CYC_FPB] = fpb; p.x[CYC_BPF] = bpf;
+    p.ld[CYC_F] = ld_f; p.ld[CYC_B] = ld_b; p.ld[CYC_FPB] = ld_fpb; p.ld[CYC_BPF] = ld_bpf;
+    p.n = n;
+    p.coef = coef;
+    return p;
+}
+
+extern "C" int emer_cycle_loss_fwd(const float* f, int64_t ld_f, const float* b, int64_t ld_b, const float* fpb,
+                                   int64_t ld_fpb, const float* bpf, int64_t ld_bpf, int64_t n, float coef, float* out,
+                                   void* workspace, void* stream) {
+    EMER_REQUIRE(f && b && fpb && bpf && out && workspace, "emer_cycle_loss_fwd: NULL pointer");
+    EMER_REQUIRE(n >= 1, "emer_cycle_loss_fwd: no rows");        // the maxima of nothing are undefined
+    EMER_REQUIRE(ld_f >= 3 && ld_b >= 3 && ld_fpb >= 3 && ld_bpf >= 3, "emer_cycle_loss_fwd: row stride below 3");
+    CycleParams p = cycle_params(f, ld_f, b, ld_b, fpb, ld_fpb, bpf, ld_bpf, n, coef);
+    p.out = out;
+    p.ws = (LossWorkspace*)workspace;
+    cycle_loss_fwd_kernel<<<loss_grid(n, LOSS_THREADS), LOSS_THREADS, 0, (cudaStream_t)stream>>>(p);
+    return check_launch("emer_cycle_loss_fwd");
+}
+
+extern "C" int emer_cycle_loss_bwd(const float* f, int64_t ld_f, const float* b, int64_t ld_b, const float* fpb,
+                                   int64_t ld_fpb, const float* bpf, int64_t ld_bpf, int64_t n, float coef,
+                                   const float* fwd_out, const float* g, float* d_fpb, float* d_bpf, void* stream) {
+    EMER_REQUIRE(f && b && fpb && bpf && fwd_out && g, "emer_cycle_loss_bwd: NULL pointer");
+    EMER_REQUIRE(d_fpb || d_bpf, "emer_cycle_loss_bwd: no gradient requested");
+    EMER_REQUIRE(n >= 1, "emer_cycle_loss_bwd: no rows");
+    EMER_REQUIRE(ld_f >= 3 && ld_b >= 3 && ld_fpb >= 3 && ld_bpf >= 3, "emer_cycle_loss_bwd: row stride below 3");
+    CycleParams p = cycle_params(f, ld_f, b, ld_b, fpb, ld_fpb, bpf, ld_bpf, n, coef);
+    p.out = (float*)fwd_out;
+    p.g = g;
+    p.d_fpb = d_fpb;
+    p.d_bpf = d_bpf;
+    cycle_loss_bwd_kernel<<<loss_grid(n, LOSS_THREADS), LOSS_THREADS, 0, (cudaStream_t)stream>>>(p);
+    return check_launch("emer_cycle_loss_bwd");
 }

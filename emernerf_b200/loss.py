@@ -2,7 +2,9 @@
 defaults, ``__call__`` signatures and returned ``{name: value}`` keys, each loss one CUDA launch forward and one
 backward (csrc/losses.cu), with no host synchronisation and no data-dependent shapes.
 
-Drop-in for ``train_emernerf.py``: replace ``import loss`` with ``from emernerf_b200 import loss``.
+Drop-in for ``train_emernerf.py``: replace ``import loss`` with ``from emernerf_b200 import loss``.  The flow variants'
+cycle loss and flow statistics, inline in ``train_emernerf.py:700-740`` rather than in ``loss/base.py``, are
+``flow_cycle_loss`` here.
 
 Differences from the op-by-op reference, all deliberate:
   * ``DepthLoss`` averages over the valid rays (0.01 < gt < upper_bound) with a count kept on the device instead of
@@ -20,7 +22,7 @@ Differences from the op-by-op reference, all deliberate:
 from __future__ import annotations
 
 import math
-from typing import Literal
+from typing import Dict, Literal, Tuple
 
 import torch
 import torch.nn as nn
@@ -29,7 +31,7 @@ from torch import Tensor
 from . import _ops
 
 __all__ = ["normalize_depth", "Loss", "RealValueLoss", "SkyLoss", "DepthLoss", "LineOfSightLoss",
-           "DynamicRegularizationLoss", "dirac_delta_approx", "compute_line_of_sight_loss"]
+           "DynamicRegularizationLoss", "dirac_delta_approx", "compute_line_of_sight_loss", "flow_cycle_loss"]
 
 
 def _unsupported(what: str):
@@ -251,6 +253,27 @@ class DynamicRegularizationLoss(Loss):
             k = float(self.entropy_skewness)
             value = _ops.pointwise_loss("entropy", dynamic_density, static_density, p0=k, p1=k - 1, post=self.coef)
         return self._result(name, value)
+
+
+FLOW_STAT_KEYS = ("max_forward_flow_norm", "max_backward_flow_norm", "max_forward_pred_backward_flow_norm",
+                  "max_backward_pred_forward_flow_norm")
+
+
+def flow_cycle_loss(extras: Dict[str, Tensor], coef: float = 0.01,
+                    name: str = "cycle_loss") -> Tuple[Dict[str, Tensor], Dict[str, Tensor]]:
+    """The flow variants' cycle-consistency loss and flow statistics of the reference's pixel pass
+    (train_emernerf.py:700-740), in one launch each way:
+
+        {name: coef * 0.5 * mean((forward_flow + forward_pred_backward_flow) ** 2
+                                 + (backward_flow + backward_pred_forward_flow) ** 2)},
+        {"max_forward_flow_norm": max |forward_flow|, ... for the four flows}
+
+    ``extras`` is ``render_results["extras"]``, each flow ``[R, S, 3]``.  Only the two predicted flows receive a
+    gradient; the statistics are 0-d device tensors without one, NaN when a row of their flow is.  An empty batch
+    raises ``ValueError``, as the reference's ``.max()`` does."""
+    value, stats = _ops.cycle_loss(extras["forward_flow"], extras["backward_flow"],
+                                   extras["forward_pred_backward_flow"], extras["backward_pred_forward_flow"], coef)
+    return {name: value}, dict(zip(FLOW_STAT_KEYS, stats.unbind(0)))
 
 
 def dirac_delta_approx(x, mu=0, sigma=1e-5):

@@ -321,6 +321,22 @@ int emer_ray_loss_bwd(int kind, const float* w, const float* t, const float* gt,
                       float two_sigma_sq, float amp, float pre, float post, const float* fwd_out, const float* g,
                       float* dw, void* stream);
 
+/* ---- the flow variants' cycle loss and flow statistics (replaces the inline block of train_emernerf.py:700-740)
+ * f = forward_flow, b = backward_flow, fpb = forward_pred_backward_flow, bpf = backward_pred_forward_flow: each n rows
+ * of 3 floats (n = R * S samples), row i at x + i * ld_x (ld_x >= 3: a column slice of a wider row is read in place).
+ *   value = coef * (0.5 * mean((f + fpb)^2 + (b + bpf)^2)), the mean over all 3n elements
+ * Forward: ONE launch, no host sync, n >= 1.  out [6] (caller-owned): out[0] = value, out[1] = 3n (the count the mean
+ * divides by, read by the backward), out[2..5] = the maximum row norm of f, b, fpb, bpf (NaN if any row of that input
+ * holds a NaN).  workspace as for the losses above.  The sum is per CTA, then over CTAs in a fixed order.
+ * Backward: ONE launch; f and b are constants.  d_fpb, d_bpf: [n, 3] contiguous, WRITTEN; either may be NULL.
+ *   d = 2 (f + fpb) * (g * coef * 0.5 / out[1])  (and likewise for b, bpf) */
+int emer_cycle_loss_fwd(const float* f, int64_t ld_f, const float* b, int64_t ld_b, const float* fpb, int64_t ld_fpb,
+                        const float* bpf, int64_t ld_bpf, int64_t n, float coef, float* out, void* workspace,
+                        void* stream);
+int emer_cycle_loss_bwd(const float* f, int64_t ld_f, const float* b, int64_t ld_b, const float* fpb, int64_t ld_fpb,
+                        const float* bpf, int64_t ld_bpf, int64_t n, float coef, const float* fwd_out, const float* g,
+                        float* d_fpb, float* d_bpf, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

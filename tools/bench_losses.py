@@ -7,6 +7,8 @@ Workloads (R = 8192 rays, S = 64 samples, seeded; targets from emernerf_b200.syn
   static     rgb l2 + opacity-based sky                                                 -- the pixel pass, by config
   dynamic    static + dynamic sparsity + shadow
   flow_feat  dynamic + feature l2 (64 channels)
+  cycle      the flow variants' cycle loss (coef 0.01) and its four flow statistics (train_emernerf.py:700-740), the
+             flows 3-wide column slices of [R, S, 6] rows as the flow MLP writes them
 Each set runs two ways, alternating in the same process: ``torch`` -- the reference's arithmetic restated op by op
 (boolean indexing in the range loss, as the reference) -- and ``fused`` -- the emernerf_b200.loss classes.
 Reported per set and way: device time (CUDA events), host wall time (ending in a synchronize), CUDA kernel launches
@@ -41,8 +43,10 @@ SETS = {
     "static": ("rgb", "sky"),
     "dynamic": ("rgb", "sky", "dynamic", "shadow"),
     "flow_feat": ("rgb", "sky", "dynamic", "shadow", "feature"),
+    "cycle": ("cycle",),
 }
-LEAVES = ("rgb", "opacity", "depth", "weights", "dynamic_density", "shadow_ratio", "dino_feat")
+LEAVES = ("rgb", "opacity", "depth", "weights", "dynamic_density", "shadow_ratio", "dino_feat", "flow_fwd_query",
+          "flow_bwd_query")
 
 
 def make_inputs(dev):
@@ -57,13 +61,32 @@ def make_inputs(dev):
         "weights": rnd(R, S) * 0.05, "t_vals": torch.sort(rnd(R, S) * 100.0, -1).values,
         "dynamic_density": rnd(R, S) * 2.0, "shadow_ratio": rnd(R, 1), "dino_feat": rnd(R, 64),
     }
+    # the flow MLP's [R, S, 6] outputs at the samples and at the two warped queries
+    x["flow"] = rnd(R, S, 6) * 2.0 - 1.0
+    x["flow_fwd_query"] = rnd(R, S, 6) * 2.0 - 1.0
+    x["flow_bwd_query"] = rnd(R, S, 6) * 2.0 - 1.0
     for k in LEAVES:
         x[k].requires_grad_()
     return x
 
 
 # ------------------------------------------------------------------ the reference's arithmetic, eager torch, fp32
+def flow_extras(x):
+    return {"forward_flow": x["flow"][..., :3], "backward_flow": x["flow"][..., 3:],
+            "forward_pred_backward_flow": x["flow_fwd_query"][..., 3:],
+            "backward_pred_forward_flow": x["flow_bwd_query"][..., :3]}
+
+
 def torch_term(name, x):
+    if name == "cycle":
+        ex = flow_extras(x)
+        cycle = 0.5 * ((ex["forward_flow"].detach() + ex["forward_pred_backward_flow"]) ** 2
+                       + (ex["backward_flow"].detach() + ex["backward_pred_forward_flow"]) ** 2).mean()
+        x["stats"] = {"max_forward_flow_norm": ex["forward_flow"].detach().norm(dim=-1).max(),
+                      "max_backward_flow_norm": ex["backward_flow"].detach().norm(dim=-1).max(),
+                      "max_forward_pred_backward_flow_norm": ex["forward_pred_backward_flow"].norm(dim=-1).max(),
+                      "max_backward_pred_forward_flow_norm": ex["backward_pred_forward_flow"].norm(dim=-1).max()}
+        return cycle * 0.01
     if name == "rgb":
         return F.mse_loss(x["rgb"].squeeze(), x["pixels"].squeeze(), reduction="none").mul(1.0).mean() * 1.0
     if name == "sky":
@@ -101,10 +124,14 @@ FUSED = {
     "shadow": lambda: fused_loss.DynamicRegularizationLoss(name="shadow", loss_type="sparsity", coef=0.01),
     "range": lambda: fused_loss.DepthLoss(loss_type="l2", coef=1.0),
     "line_of_sight": lambda: fused_loss.LineOfSightLoss(coef=0.1),
+    "cycle": lambda: None,
 }
 
 
 def fused_term(fn, name, x):
+    if name == "cycle":
+        cycle, x["stats"] = fused_loss.flow_cycle_loss(flow_extras(x))
+        return cycle
     if name == "rgb":
         return fn(x["rgb"], x["pixels"])
     if name == "sky":
@@ -126,6 +153,7 @@ def fused_term(fn, name, x):
 def step(way, names, x, fns):
     for k in LEAVES:
         x[k].grad = None
+    x.pop("stats", None)
     if way == "torch":
         total = sum(torch_term(n, x) for n in names)
     else:
@@ -193,7 +221,7 @@ def main():
                 step(way, names, x, fns)
         dev_ms = {"torch": [], "fused": []}
         host_ms = {"torch": [], "fused": []}
-        values = {}
+        values, stats = {}, {}
         torch.cuda.synchronize()
         for it in range(args.iters):
             for way in (("torch", "fused") if it % 2 == 0 else ("fused", "torch")):
@@ -206,6 +234,8 @@ def main():
                 host_ms[way].append((time.perf_counter() - t0) * 1e3)
                 dev_ms[way].append(e0.elapsed_time(e1))
                 values[way] = total.item()
+                if "stats" in x:
+                    stats[way] = {k: v.item() for k, v in x["stats"].items()}
         entry = {}
         for way in ("torch", "fused"):
             kernels, copies = count_launches(way, names, x, fns)
@@ -216,6 +246,9 @@ def main():
                 "host_syncs": count_syncs(way, names, x, fns), "loss": values[way],
             }
         entry["loss_rel_diff"] = abs(values["fused"] - values["torch"]) / max(abs(values["torch"]), 1e-30)
+        if stats:
+            entry["stats_max_rel_diff"] = max(abs(stats["fused"][k] - v) / max(abs(v), 1e-30)
+                                              for k, v in stats["torch"].items())
         result["sets"][set_name] = entry
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "bench_losses.json"), "w") as fh:
