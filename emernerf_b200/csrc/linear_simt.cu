@@ -332,7 +332,8 @@ __global__ void __launch_bounds__(256) narrow_bwd_data_kernel(const float* __res
         v[j] = a;
     }
     float* out = dx + row * lddx + c0;
-    if ((lddx % 4 == 0) && ((reinterpret_cast<uintptr_t>(dx) & 15) == 0) && c0 + 3 < lddx) {
+    // only columns < k are ours: the caller's row may go on behind them (a view of a wider buffer)
+    if ((lddx % 4 == 0) && ((reinterpret_cast<uintptr_t>(dx) & 15) == 0) && c0 + 4 <= k) {
         *reinterpret_cast<float4*>(out) = make_float4(v[0], v[1], v[2], v[3]);
     } else {
 #pragma unroll
