@@ -164,10 +164,14 @@ __global__ void __launch_bounds__(THREADS, 1) field_fwd_kernel(const FwdParams p
         uint32_t ahi[8][4], alo[8][4];
 
         // ---- stage 0: Hb = relu(enc Wb0^T + bb0)
+        // Rows past n read row n - 1 instead: a per-lane conditional load feeding the A operand makes ptxas serialize
+        // every wgmma of the kernel (C7520).  Rows of a tile are independent and rows >= n are never stored.
+        const float* x0p = p.enc + (ok0 ? row0 : p.n - 1) * p.ld_enc + 2 * q;
+        const float* x1p = p.enc + (ok1 ? row1 : p.n - 1) * p.ld_enc + 2 * q;
 #pragma unroll
         for (int j = 0; j < K_ENC / 8; ++j) {
-            const float2 x0 = ld2(p.enc + row0 * p.ld_enc + 8 * j + 2 * q, ok0);
-            const float2 x1 = ld2(p.enc + row1 * p.ld_enc + 8 * j + 2 * q, ok1);
+            const float2 x0 = __ldg(reinterpret_cast<const float2*>(x0p + 8 * j));
+            const float2 x1 = __ldg(reinterpret_cast<const float2*>(x1p + 8 * j));
             frag_split(x0.x, x0.y, x1.x, x1.y, ahi[j], alo[j]);
         }
         float acc[32];
@@ -190,14 +194,27 @@ __global__ void __launch_bounds__(THREADS, 1) field_fwd_kernel(const FwdParams p
         }
 
         // ---- stage 1: feats = Hb Wb1^T + bb1; sigma = exp(feats[0] - 1); geo -> operand; semantic half -> HBM
-        float geo[32], sem[NF > H ? 32 : 1];
+        // The semantic half goes first, on its own: with both halves in flight at once <k,128> spills.
+        if constexpr (NF > H) {
+            float sem[32];
+            wg_fence();
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks)
+                mma3<64>(sem, ahi[ks], alo[ks], b_desc(sb + m.wb1_hi, NF, ks, H), b_desc(sb + m.wb1_lo, NF, ks, H), ks > 0);
+            wg_commit();
+            wg_wait0();
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int c = 8 * j + 2 * q;
+                st2(p.save_sem + row0 * H + c, sem[4 * j] + bb1_s[H + c], sem[4 * j + 1] + bb1_s[H + c + 1], ok0);
+                st2(p.save_sem + row1 * H + c, sem[4 * j + 2] + bb1_s[H + c], sem[4 * j + 3] + bb1_s[H + c + 1], ok1);
+            }
+        }
+        float geo[32];
         wg_fence();
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {
+        for (int ks = 0; ks < 8; ++ks)
             mma3<64>(geo, ahi[ks], alo[ks], b_desc(sb + m.wb1_hi, NF, ks, 0), b_desc(sb + m.wb1_lo, NF, ks, 0), ks > 0);
-            if constexpr (NF > H)
-                mma3<64>(sem, ahi[ks], alo[ks], b_desc(sb + m.wb1_hi, NF, ks, H), b_desc(sb + m.wb1_lo, NF, ks, H), ks > 0);
-        }
         wg_commit();
         wg_wait0();
 #pragma unroll
@@ -214,14 +231,6 @@ __global__ void __launch_bounds__(THREADS, 1) field_fwd_kernel(const FwdParams p
                 st2(p.save_hg + row1 * 128 + H + c, v2, v3, ok1);
             }
             frag_split(v0, v1, v2, v3, ahi[j], alo[j]);
-        }
-        if constexpr (NF > H) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int c = 8 * j + 2 * q;
-                st2(p.save_sem + row0 * H + c, sem[4 * j] + bb1_s[H + c], sem[4 * j + 1] + bb1_s[H + c + 1], ok0);
-                st2(p.save_sem + row1 * H + c, sem[4 * j + 2] + bb1_s[H + c], sem[4 * j + 3] + bb1_s[H + c + 1], ok1);
-            }
         }
 
         // ---- stage 2: [pre-h0 | partial h1] = G [W0g; W1g]^T;  H0 = relu(pre-h0 + ray_bias0)

@@ -2,14 +2,18 @@
 // field_bwd_kernel leaves in HBM is read once, and the five products dW += dZ^T X of the chain's layers accumulate in
 // registers with the 3xTF32 warpgroup MMA of tc_common.cuh (the arithmetic of wgrad_mn.cu, summed in another order).
 //
-// Per 16-row tile, cp.async copies enc, hb, hg = [h0 | geo], h1, dz1, d1 = [dZ0 | dF], dzb, d_sem and dz2 into a
-// STAGES-deep shared-memory ring, so tiles t+1 .. t+STAGES-1 are in flight while tile t is computed.  Every dZ column
-// is split once into K-major hi / lo panels (the B operands, shared by the products that use them) and summed into its
-// bias; each warpgroup reads its X^T fragments (the A operands) out of the landed tile:
-//   warpgroup 0:  enc x dzb -> dWb0,  hb x dF -> dWb1[:64]
-//   warpgroup 1:  geo x dZ0 -> dW0g,  geo x dz1 -> dW1g,  h1 x dz2 -> dW2
-//   warpgroup 2:  h0 x dz1 -> dW1h,   hb x d_sem -> dWb1[64:]
-// The accumulators stay in registers across the CTA's tiles and are flushed once with atomics (DESIGN.md §5.3).
+// Warp-specialized, one CTA per SM, tiles of 16 rows:
+//   producer  (warpgroup 0)  cp.async copies enc, hb, hg = [h0 | geo], h1, dz1, d1 = [dZ0 | dF], dzb, d_sem and dz2 of
+//                            tile t+2 into a STAGES-deep ring, and splits every dZ column of tile t+1 into K-major hi / lo
+//                            panels (the B operands, shared by the products that use them) of one of two panel buffers,
+//                            summing it into its bias;
+//   consumers (warpgroups 1, 2) read their X^T fragments (the A operands) of tile t out of the ring and run its MMAs on
+//                            the other panel buffer:
+//     warpgroup 1:  enc x dzb -> dWb0,  geo x dZ0 -> dW0g,  geo x dz1 -> dW1g
+//     warpgroup 2:  hb x dF -> dWb1[:64],  h0 x dz1 -> dW1h,  h1 x dz2 -> dW2,  hb x d_sem -> dWb1[64:]
+// Hand-offs are named barriers (full / empty per panel buffer, free per ring slot), so staging, copies and MMAs
+// overlap; setmaxnreg gives the consumers' accumulators the producer's registers.  The accumulators stay in registers
+// across the CTA's tiles and are flushed once with atomics (DESIGN.md §5.3).
 // HBM-bound: (k_enc + 64 + 128 + 64 + 3 + 64 + 128 + 64 [+ 64 with d_sem]) * 4 B per row.
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -20,9 +24,13 @@ namespace fw {
 using namespace emer::tc;
 
 constexpr int TR = 16;               // rows per tile = 2 k steps
-constexpr int STAGES = 4;            // ring depth
-constexpr int THREADS = 384;         // three warpgroups
+constexpr int STAGES = 3;            // row ring: tile t (A operands), t+1 (being split), t+2 (landing)
+constexpr int THREADS = 384;         // producer warpgroup + two consumer warpgroups
+constexpr int PROD_REGS = 56, CONS_REGS = 224;   // setmaxnreg: 128 * 56 + 256 * 224 <= 64 K; the producer spills at 40
 constexpr int MIN_TILES = 4;         // per CTA: each CTA ends with ~25 K atomics onto the same addresses
+
+// named barriers (0 is __syncthreads): panel buffer b full / empty, ring slot s free, the producer warpgroup alone
+constexpr int BAR_FULL = 1, BAR_EMPTY = 3, BAR_RING = 5, BAR_PROD = 5 + STAGES;
 
 // B panels (hi, then lo right behind it) of one tile: TR rows of 64 (dz2: 8) columns
 constexpr int PANEL64 = TR * 64 * 4, PANEL8 = TR * 8 * 4;
@@ -56,16 +64,57 @@ __device__ __forceinline__ void cp_async16(float* dst, const float* src, int byt
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+// bar.arrive orders the caller's earlier memory accesses before the bar.sync of the threads that wait on the barrier
+__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
 
-// rows [row0, row0 + TR) of a row buffer with stride ld, W floats each, into a slot of row stride W + 4; rows past n
-// are zero-filled
+// rows [row0, row0 + TR) of a row buffer with stride ld, W floats each, into a slot of row stride W + 4; rows >= rows_left
+// are zero-filled.  Producer thread t (0 .. 127) copies the 16-byte chunks t, t + 128, ...: the trip count and each
+// chunk's place in the tile are compile-time in all but t, which keeps the producer's issue cost per tile low.
 template <int W>
-__device__ __forceinline__ void copy_rows(float* dst, const float* src, int64_t ld, int64_t row0, int64_t n) {
-    constexpr int CPR = W / 4;
-    for (int c = threadIdx.x; c < TR * CPR; c += THREADS) {
-        const int r = c / CPR, j = c % CPR;
-        const bool ok = row0 + r < n;
-        cp_async16(dst + r * (W + 4) + 4 * j, ok ? src + (row0 + r) * ld + 4 * j : src, ok ? 16 : 0);
+__device__ __forceinline__ void copy_rows(float* dst, const float* src, int64_t ld, int64_t row0, int rows_left, int t) {
+    constexpr int CPR = W / 4, CHUNKS = TR * CPR;
+    const float* s = src + row0 * ld;
+#pragma unroll
+    for (int k = 0; k < (CHUNKS + 127) / 128; ++k) {
+        const int c = t + 128 * k;
+        if (CHUNKS % 128 == 0 || c < CHUNKS) {
+            const int r = c / CPR, j = c % CPR;
+            const bool ok = r < rows_left;
+            cp_async16(dst + r * (W + 4) + 4 * j, ok ? s + r * ld + 4 * j : src, ok ? 16 : 0);
+        }
+    }
+}
+
+// column col of dZ buffer B (0 dzb, 1 dF, 2 d_sem, 3 dZ0, 4 dz1, 5 dz2) of the landed stage st, split into the hi / lo
+// B panels at pan and summed into dbs.  dz2 has 3 real columns; columns 3 .. 7 of its panel are written as zeros.
+template <int B, int KE, bool HEAD>
+__device__ __forceinline__ void split_col(const float* st, uint8_t* pan, int col, bool sem, float& dbs) {
+    using S = Stage<KE, HEAD>;
+    constexpr int soff = B == 0 ? S::DZB : B == 1 ? S::DF : B == 2 ? S::DSEM : B == 3 ? S::D1 : B == 4 ? S::DZ1 : S::DZ2;
+    constexpr int sld = B == 1 || B == 3 ? S::LD_D1 : (B == 5 ? 3 : S::LD64);
+    constexpr int rows = B == 5 ? 8 : 64;
+    constexpr int pb = B == 0 ? P_DZB : B == 1 ? P_DF : B == 2 ? P_DSEM : B == 3 ? P_DZ0 : B == 4 ? P_DZ1 : P_DZ2;
+    if constexpr (B >= 3 && !HEAD) return;
+    if ((B == 2 && !sem) || (B == 5 && col >= 8)) return;
+    const bool real = B != 5 || col < 3;
+    const float* z = st + soff + (real ? col : 0);
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            // rows 8ks + h + {0, 2, 4, 6} sit at kpos 8ks + 4h + {0, 1, 2, 3} (tc_common.cuh): one 16-byte store
+            float v[4], hi[4], lo[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                v[j] = real ? z[(8 * ks + 2 * j + h) * sld] : 0.0f;
+                split(v[j], hi[j], lo[j]);
+                dbs += v[j];
+            }
+            uint8_t* dst = pan + pb + (2 * ks + h) * rows * 16 + col * 16;
+            *reinterpret_cast<float4*>(dst) = make_float4(hi[0], hi[1], hi[2], hi[3]);
+            *reinterpret_cast<float4*>(dst + TR * rows * 4) = make_float4(lo[0], lo[1], lo[2], lo[3]);
+        }
     }
 }
 
@@ -104,149 +153,151 @@ __device__ __forceinline__ void flush(const float (&acc)[N / 2], float* dw, int6
     }
 }
 
+// Hand-offs of the CTA's i-th tile (ring slot i % STAGES, panel buffer i % 2), m = the CTA's tile count:
+//   producer: [i >= 1, i + 2 < m: wait RING(i - 1)]  copy i + 2  [i >= 2: wait EMPTY(i - 2)]  split i  -> FULL(i)
+//   consumer: wait FULL(i)  load A  [i + 3 < m: -> RING(i)]  MMAs  [i + 2 < m: -> EMPTY(i)]
+// Every arrival has exactly one matching wait, and no barrier is reused before its previous phase completed.
 template <int KE, bool HEAD>
 __global__ void __launch_bounds__(THREADS, 1) field_wgrad_kernel(const __grid_constant__ Params p) {
     using S = Stage<KE, HEAD>;
     extern __shared__ __align__(128) uint8_t smem[];
-    float* ring = reinterpret_cast<float*>(smem + P_BYTES);
-    const uint32_t pan = smem_u32(smem);
+    float* ring = reinterpret_cast<float*>(smem + 2 * P_BYTES);
     const int tid = threadIdx.x, lane = tid & 31, q = lane & 3;
     const int wgi = __shfl_sync(0xffffffffu, tid >> 7, 0);     // (visibly warp-uniform: the MMAs stay pipelined)
-    const int f0 = 16 * ((tid >> 5) & 3) + (lane >> 2);
     const bool sem = p.d_sem != nullptr;
     const int64_t n_tiles = (p.n + TR - 1) / TR;
     const int64_t my_tiles = (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;     // the CTA's tiles: blockIdx.x + i * gridDim.x
 
-    // copies of the CTA's i-th tile into stage i % STAGES; one commit group per tile, empty past the end
-    auto issue = [&](int64_t i) {
-        if (i < my_tiles) {
-            const int64_t row0 = (blockIdx.x + i * gridDim.x) * TR;
-            float* st = ring + (i % STAGES) * S::FLOATS;
-            copy_rows<KE>(st + S::ENC, p.enc, p.ld_enc, row0, p.n);
-            copy_rows<64>(st + S::HB, p.hb, 64, row0, p.n);
-            copy_rows<64>(st + S::DZB, p.dzb, 64, row0, p.n);
-            if (sem) copy_rows<64>(st + S::DSEM, p.d_sem, 64, row0, p.n);
-            copy_rows<HEAD ? 128 : 64>(st + S::D1, p.d1 + (HEAD ? 0 : 64), 128, row0, p.n);
-            if constexpr (HEAD) {
-                copy_rows<128>(st + S::HG, p.hg, 128, row0, p.n);
-                copy_rows<64>(st + S::H1, p.h1, 64, row0, p.n);
-                copy_rows<64>(st + S::DZ1, p.dz1, 64, row0, p.n);
-                // dz2 rows are 12 bytes: the tile is one run of TR * 3 / 4 chunks, the last one cut at row n
-                if (tid < TR * 3 / 4) {
-                    const int64_t left = (p.n - row0 < TR ? p.n - row0 : TR) * 12 - 16 * tid;
-                    const int b = left <= 0 ? 0 : (left < 16 ? (int)left : 16);
-                    cp_async16(st + S::DZ2 + 4 * tid, b ? p.dz2 + row0 * 3 + 4 * tid : p.dz2, b);
-                }
-            }
-        }
-        cp_async_commit();
-    };
-
-    // the dZ column this thread splits into the B panels and sums into its bias: 64 threads for each 64-column buffer
-    // dzb, dF, d_sem, dZ0, dz1, then 8 for dz2 (3 real columns, the rest of its panel stays zero)
-    const int col = tid & 63;
-    int soff = -1, sld = S::LD64, rows = 64;
-    uint32_t pb = 0;
-    float* db = nullptr;
-    bool real = true;
-    switch (tid >> 6) {
-        case 0: soff = S::DZB; pb = P_DZB; db = p.dbb0; break;
-        case 1: soff = S::DF; sld = S::LD_D1; pb = P_DF; db = p.dbb1; break;
-        case 2: if (sem) { soff = S::DSEM; pb = P_DSEM; db = p.dbb1 + 64; } break;
-        case 3: if (HEAD) { soff = S::D1; sld = S::LD_D1; pb = P_DZ0; } break;
-        case 4: if (HEAD) { soff = S::DZ1; pb = P_DZ1; } break;
-        default:
-            if (HEAD && col < 8) { soff = S::DZ2; sld = 3; rows = 8; pb = P_DZ2; db = p.db2; real = col < 3; }
-            break;
-    }
-
-    float a0[32], a1[32], a2[4], dbs = 0.0f;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) a0[i] = a1[i] = 0.0f;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) a2[i] = 0.0f;
-
-#pragma unroll
-    for (int s = 0; s < STAGES - 1; ++s) issue(s);
-    for (int64_t i = 0; i < my_tiles; ++i) {
-        cp_async_wait<STAGES - 2>();
-        __syncthreads();                  // tile i has landed for every thread; tile i-1's MMAs and reads are over
-        issue(i + STAGES - 1);            // into the stage tile i-1 used
-        const float* st = ring + (i % STAGES) * S::FLOATS;
-        if (soff >= 0) {
-            const float* z = st + soff + (real ? col : 0);
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    // rows 8ks + h + {0, 2, 4, 6} sit at kpos 8ks + 4h + {0, 1, 2, 3} (tc_common.cuh): one 16-byte store
-                    float v[4], hi[4], lo[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        v[j] = real ? z[(8 * ks + 2 * j + h) * sld] : 0.0f;
-                        split(v[j], hi[j], lo[j]);
-                        dbs += v[j];
-                    }
-                    uint8_t* dst = smem + pb + (2 * ks + h) * rows * 16 + col * 16;
-                    *reinterpret_cast<float4*>(dst) = make_float4(hi[0], hi[1], hi[2], hi[3]);
-                    *reinterpret_cast<float4*>(dst + TR * rows * 4) = make_float4(lo[0], lo[1], lo[2], lo[3]);
-                }
-            }
-        }
-        fence_async_proxy();
-        __syncthreads();                  // the panels are complete
-
-        uint32_t h0[2][4], l0[2][4], h1[2][4], l1[2][4];
-        if (wgi == 0) {
-            load_a<KE>(st + S::ENC, S::LD_ENC, f0, q, h0, l0);
-            load_a<64>(st + S::HB, S::LD64, f0, q, h1, l1);
-            wg_fence();
-            mma_tile<64>(a0, h0, l0, pan + P_DZB);
-            mma_tile<64>(a1, h1, l1, pan + P_DF);
-            wg_commit();
-            wg_wait0();
-        } else if (wgi == 1) {
-            if constexpr (HEAD) {
-                load_a<64>(st + S::HG + 64, S::LD128, f0, q, h0, l0);
-                load_a<64>(st + S::H1, S::LD64, f0, q, h1, l1);
-                wg_fence();
-                mma_tile<64>(a0, h0, l0, pan + P_DZ0);
-                mma_tile<64>(a1, h0, l0, pan + P_DZ1);
-                mma_tile<8>(a2, h1, l1, pan + P_DZ2);
-                wg_commit();
-                wg_wait0();
-            }
-        } else if (HEAD || sem) {
-            if (HEAD) load_a<64>(st + S::HG, S::LD128, f0, q, h0, l0);
-            if (sem) load_a<64>(st + S::HB, S::LD64, f0, q, h1, l1);
-            wg_fence();
-            if (HEAD) mma_tile<64>(a0, h0, l0, pan + P_DZ1);
-            if (sem) mma_tile<64>(a1, h1, l1, pan + P_DSEM);
-            wg_commit();
-            wg_wait0();
-        }
-    }
-    cp_async_wait<0>();
-
     if (wgi == 0) {
-        flush<64>(a0, p.dwb0, KE, KE, 64, f0, q);
-        flush<64>(a1, p.dwb1, 64, 64, 64, f0, q);
-    } else if (wgi == 1) {
-        if (HEAD) {
-            flush<64>(a0, p.dw0g, p.ld_w0, 64, 64, f0, q);
-            flush<64>(a1, p.dw1g, p.ld_w1, 64, 64, f0, q);
-            flush<8>(a2, p.dw2, 64, 64, 3, f0, q);
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(PROD_REGS));
+        // copies of the CTA's i-th tile into its ring slot; one commit group per tile, empty past the end
+        auto issue = [&](int64_t i, int slot) {
+            if (i < my_tiles) {
+                const int64_t row0 = (blockIdx.x + i * gridDim.x) * TR;
+                const int rows_left = p.n - row0 < TR ? (int)(p.n - row0) : TR;
+                float* st = ring + slot * S::FLOATS;
+                copy_rows<KE>(st + S::ENC, p.enc, p.ld_enc, row0, rows_left, tid);
+                copy_rows<64>(st + S::HB, p.hb, 64, row0, rows_left, tid);
+                copy_rows<64>(st + S::DZB, p.dzb, 64, row0, rows_left, tid);
+                if (sem) copy_rows<64>(st + S::DSEM, p.d_sem, 64, row0, rows_left, tid);
+                copy_rows<HEAD ? 128 : 64>(st + S::D1, p.d1 + (HEAD ? 0 : 64), 128, row0, rows_left, tid);
+                if constexpr (HEAD) {
+                    copy_rows<128>(st + S::HG, p.hg, 128, row0, rows_left, tid);
+                    copy_rows<64>(st + S::H1, p.h1, 64, row0, rows_left, tid);
+                    copy_rows<64>(st + S::DZ1, p.dz1, 64, row0, rows_left, tid);
+                    // dz2 rows are 12 bytes: the tile is one run of TR * 3 / 4 chunks, the last one cut at row n
+                    if (tid < TR * 3 / 4) {
+                        const int left = rows_left * 12 - 16 * tid;
+                        const int b = left <= 0 ? 0 : (left < 16 ? left : 16);
+                        cp_async16(st + S::DZ2 + 4 * tid, b ? p.dz2 + row0 * 3 + 4 * tid : p.dz2, b);
+                    }
+                }
+            }
+            cp_async_commit();
+        };
+        // thread tid splits column col of dZ buffers half, half + 2, half + 4 (split_col) and sums their biases
+        const int col = tid & 63, half = __shfl_sync(0xffffffffu, tid >> 6, 0);
+        float db0 = 0.0f, db1 = 0.0f, db2 = 0.0f;
+        issue(0, 0);
+        issue(1, 1);
+        int slot = 0;                         // tile i's ring slot; pb: its panel buffer
+        for (int64_t i = 0; i < my_tiles; ++i, slot = slot + 1 == STAGES ? 0 : slot + 1) {
+            const int pb = (int)(i & 1), prev = slot == 0 ? STAGES - 1 : slot - 1;     // prev: tile i-1's = i+2's slot
+            if (i >= 1 && i + 2 < my_tiles) bar_sync(BAR_RING + prev, THREADS);
+            issue(i + 2, prev);
+            if (i >= 2) bar_sync(BAR_EMPTY + pb, THREADS);
+            cp_async_wait<2>();
+            bar_sync(BAR_PROD, 128);          // tile i has landed for the whole producer warpgroup
+            const float* st = ring + slot * S::FLOATS;
+            uint8_t* pan = smem + pb * P_BYTES;
+            if (half == 0) {
+                split_col<0, KE, HEAD>(st, pan, col, sem, db0);
+                split_col<2, KE, HEAD>(st, pan, col, sem, db1);
+                split_col<4, KE, HEAD>(st, pan, col, sem, db2);
+            } else {
+                split_col<1, KE, HEAD>(st, pan, col, sem, db0);
+                split_col<3, KE, HEAD>(st, pan, col, sem, db1);
+                split_col<5, KE, HEAD>(st, pan, col, sem, db2);
+            }
+            fence_async_proxy();
+            bar_arrive(BAR_FULL + pb, THREADS);
+        }
+        cp_async_wait<0>();
+        if (half == 0) {
+            atomicAdd(p.dbb0 + col, db0);
+            if (sem) atomicAdd(p.dbb1 + 64 + col, db1);
+        } else {
+            atomicAdd(p.dbb1 + col, db0);
+            if (HEAD && col < 3) atomicAdd(p.db2 + col, db2);
         }
     } else {
-        if (HEAD) flush<64>(a0, p.dw1h, p.ld_w1, 64, 64, f0, q);
-        if (sem) flush<64>(a1, p.dwb1 + 64 * 64, 64, 64, 64, f0, q);
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(CONS_REGS));
+        const uint32_t pan0 = smem_u32(smem);
+        const int f0 = 16 * ((tid >> 5) & 3) + (lane >> 2);
+        float a0[32], a1[32], a2[32], a3[4];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) a0[i] = a1[i] = a2[i] = 0.0f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) a3[i] = 0.0f;
+
+        int slot = 0;
+        for (int64_t i = 0; i < my_tiles; ++i, slot = slot + 1 == STAGES ? 0 : slot + 1) {
+            const int pb = (int)(i & 1);
+            bar_sync(BAR_FULL + pb, THREADS);
+            const float* st = ring + slot * S::FLOATS;
+            const uint32_t pan = pan0 + (uint32_t)pb * P_BYTES;
+            uint32_t h0[2][4], l0[2][4], h1[2][4], l1[2][4], h2[2][4], l2[2][4];
+            if (wgi == 1) {
+                load_a<KE>(st + S::ENC, S::LD_ENC, f0, q, h0, l0);
+                if (HEAD) load_a<64>(st + S::HG + 64, S::LD128, f0, q, h1, l1);
+            } else {
+                load_a<64>(st + S::HB, S::LD64, f0, q, h0, l0);
+                if (HEAD) {
+                    load_a<64>(st + S::HG, S::LD128, f0, q, h1, l1);
+                    load_a<64>(st + S::H1, S::LD64, f0, q, h2, l2);
+                }
+            }
+            if (i + STAGES < my_tiles) bar_arrive(BAR_RING + slot, THREADS);
+            wg_fence();
+            if (wgi == 1) {
+                mma_tile<64>(a0, h0, l0, pan + P_DZB);
+                if (HEAD) {
+                    mma_tile<64>(a1, h1, l1, pan + P_DZ0);
+                    mma_tile<64>(a2, h1, l1, pan + P_DZ1);
+                }
+            } else {
+                mma_tile<64>(a0, h0, l0, pan + P_DF);
+                if (sem) mma_tile<64>(a2, h0, l0, pan + P_DSEM);
+                if (HEAD) {
+                    mma_tile<64>(a1, h1, l1, pan + P_DZ1);
+                    mma_tile<8>(a3, h2, l2, pan + P_DZ2);
+                }
+            }
+            wg_commit();
+            wg_wait0();
+            if (i + 2 < my_tiles) bar_arrive(BAR_EMPTY + pb, THREADS);
+        }
+
+        if (wgi == 1) {
+            flush<64>(a0, p.dwb0, KE, KE, 64, f0, q);
+            if (HEAD) {
+                flush<64>(a1, p.dw0g, p.ld_w0, 64, 64, f0, q);
+                flush<64>(a2, p.dw1g, p.ld_w1, 64, 64, f0, q);
+            }
+        } else {
+            flush<64>(a0, p.dwb1, 64, 64, 64, f0, q);
+            if (sem) flush<64>(a2, p.dwb1 + 64 * 64, 64, 64, 64, f0, q);
+            if (HEAD) {
+                flush<64>(a1, p.dw1h, p.ld_w1, 64, 64, f0, q);
+                flush<8>(a3, p.dw2, 64, 64, 3, f0, q);
+            }
+        }
     }
-    if (db && real) atomicAdd(db + col, dbs);
 }
 
 template <int KE, bool HEAD>
 static int launch_t(const Params& p, cudaStream_t st) {
-    constexpr int smem = P_BYTES + STAGES * Stage<KE, HEAD>::FLOATS * 4;
+    constexpr int smem = 2 * P_BYTES + STAGES * Stage<KE, HEAD>::FLOATS * 4;
     static_assert(smem <= 227 * 1024, "field_wgrad_kernel: shared memory");
     static bool configured[64] = {false};            // the attribute is per kernel and per device
     const int dev = current_device();
