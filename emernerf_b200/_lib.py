@@ -13,6 +13,31 @@ from .grid_desc import EmerGridDesc
 
 _LIB = None
 _P = c_void_p
+
+# host structs of emer_render_fwd / emer_render_bwd (include/emer_b200.h): field names and order as there
+RENDER_IN_PTRS = ("t0", "t1", "sigma", "sigma_s", "sigma_d", "rgb", "rgb_s", "rgb_d", "shadow", "rgb_sky", "dino",
+                  "dino_s", "dino_d", "dino_sky", "dino_pe", "fwd_flow", "bwd_flow")
+RENDER_OUT_PTRS = ("weights", "trans", "opacity", "depth", "median_depth", "rgb", "shadow_ratio", "dino", "dino_pe_free",
+                   "static_opacity", "dynamic_opacity", "static_depth", "dynamic_depth", "static_rgb", "dynamic_rgb",
+                   "shadow_reduced_static_rgb", "shadow_only_static_rgb", "shadow", "forward_flow", "backward_flow",
+                   "static_dino", "dynamic_dino")
+RENDER_GRAD_PTRS = ("g_weights", "g_trans", "g_opacity", "g_depth", "g_rgb", "g_shadow_ratio", "g_dino",
+                    "g_dino_pe_free", "d_sigma", "d_sigma_s", "d_sigma_d", "d_rgb", "d_rgb_s", "d_rgb_d", "d_shadow",
+                    "d_rgb_sky", "d_dino", "d_dino_s", "d_dino_d", "d_dino_sky", "d_dino_pe")
+
+
+class EmerRenderIn(ctypes.Structure):
+    _fields_ = [(k, _P) for k in RENDER_IN_PTRS] + [("ld_flow", c_int64), ("n_rays", c_int64),
+                                                     ("n_samples", c_int32), ("n_dino", c_int32)]
+
+
+class EmerRenderOut(ctypes.Structure):
+    _fields_ = [(k, _P) for k in RENDER_OUT_PTRS]
+
+
+class EmerRenderGrad(ctypes.Structure):
+    _fields_ = [(k, _P) for k in RENDER_GRAD_PTRS]
+
 # number of kernels this library launched through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = 0
 
@@ -61,6 +86,8 @@ _SIGNATURES = {
                           _P],
     "emer_cycle_loss_fwd": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, _P, _P, _P],
     "emer_cycle_loss_bwd": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, _P, _P, _P, _P, _P],
+    "emer_render_fwd": [POINTER(EmerRenderIn), POINTER(EmerRenderOut), _P],
+    "emer_render_bwd": [POINTER(EmerRenderIn), _P, _P, POINTER(EmerRenderGrad), _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])

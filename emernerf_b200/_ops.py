@@ -1128,6 +1128,166 @@ def accumulate(w: Tensor, v: Tensor) -> Tensor:
     return _Accumulate.apply(w, v)
 
 
+# ----------------------------------------------------------------------------- the body of `rendering` (csrc/render.cu)
+# differentiable inputs of emer_render_* (per sample: [R,S] or [R,S,3|C]; per ray: rgb_sky [R,3], dino_sky / dino_pe
+# [R,C]) and the outputs a training pass can differentiate; every other output is evaluation-only
+RENDER_INPUTS = ("sigma", "sigma_s", "sigma_d", "rgb", "rgb_s", "rgb_d", "shadow", "rgb_sky", "dino", "dino_s", "dino_d",
+                 "dino_sky", "dino_pe")
+RENDER_TRAIN_OUTPUTS = ("weights", "trans", "opacity", "depth", "median_depth", "rgb", "shadow_ratio", "dino",
+                        "dino_pe_free")
+RENDER_DECOMPOSITION = ("static_opacity", "dynamic_opacity", "static_depth", "dynamic_depth", "static_rgb",
+                        "dynamic_rgb", "shadow_reduced_static_rgb", "shadow_only_static_rgb", "shadow", "forward_flow",
+                        "backward_flow", "static_dino", "dynamic_dino")
+RENDER_MAX_CHANNELS = 256       # csrc/render.cu: 32 lanes x RENDER_MAX_PER_LANE
+
+
+def _render_in(t0: Tensor, t1: Tensor, ins: Dict[str, Tensor], flows) -> "_lib.EmerRenderIn":
+    r, s = ins["sigma"].shape
+    dino = ins.get("dino") if ins.get("dino") is not None else ins.get("dino_s")
+    c = _lib.EmerRenderIn(t0=t0.data_ptr(), t1=t1.data_ptr(), n_rays=r, n_samples=s,
+                          n_dino=0 if dino is None else dino.shape[-1], ld_flow=3)
+    for k in RENDER_INPUTS:
+        if ins.get(k) is not None:
+            setattr(c, k, ins[k].data_ptr())
+    if flows is not None:
+        (f, ld), (b, _) = flows
+        c.fwd_flow, c.bwd_flow, c.ld_flow = f.data_ptr(), b.data_ptr(), ld
+    return c
+
+
+def _render_fwd(t0: Tensor, t1: Tensor, ins: Dict[str, Tensor], flows, decomposition: bool) -> Dict[str, Tensor]:
+    """One emer_render_fwd launch; returns every output the inputs define (the decomposition when asked for)."""
+    r, s = ins["sigma"].shape
+    dev = ins["sigma"].device
+    new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)    # noqa: E731
+    two = ins.get("sigma_s") is not None
+    blend_rgb = ins.get("rgb") is None and ins.get("rgb_s") is not None
+    dino = ins.get("dino") if ins.get("dino") is not None else ins.get("dino_s")
+    out = {"weights": new(r, s), "trans": new(r, s), "opacity": new(r, 1), "depth": new(r, 1),
+           "median_depth": new(r, 1)}
+    if ins.get("rgb") is not None or blend_rgb:
+        out["rgb"] = new(r, 3)
+    if ins.get("shadow") is not None and blend_rgb:
+        out["shadow_ratio"] = new(r, 1)
+    if dino is not None:
+        c = dino.shape[-1]
+        out["dino"] = new(r, c)
+        if ins.get("dino_pe") is not None:
+            out["dino_pe_free"] = new(r, c)
+    if decomposition and two:
+        for k in ("static_opacity", "dynamic_opacity", "static_depth", "dynamic_depth"):
+            out[k] = new(r, 1)
+        if blend_rgb:
+            out["static_rgb"], out["dynamic_rgb"] = new(r, 3), new(r, 3)
+            if ins.get("shadow") is not None:
+                out["shadow_reduced_static_rgb"], out["shadow_only_static_rgb"] = new(r, 3), new(r, 3)
+                out["shadow"] = new(r, 1)
+            if flows is not None:
+                out["forward_flow"], out["backward_flow"] = new(r, 3), new(r, 3)
+        if ins.get("dino") is None and ins.get("dino_s") is not None:
+            out["static_dino"], out["dynamic_dino"] = new(r, dino.shape[-1]), new(r, dino.shape[-1])
+    cout = _lib.EmerRenderOut(**{k: v.data_ptr() for k, v in out.items()})
+    _lib.call("emer_render_fwd", ctypes.byref(_render_in(t0, t1, ins, flows)), ctypes.byref(cout), _stream())
+    return out
+
+
+class _Render(torch.autograd.Function):
+    """The training outputs of emer_render_fwd (RENDER_TRAIN_OUTPUTS, None where the inputs define none) and their
+    backward in one emer_render_bwd launch; t0 / t1 are constants, as in _Composite."""
+
+    @staticmethod
+    def forward(ctx, t0: Tensor, t1: Tensor, *ins):
+        ctx.set_materialize_grads(False)
+        named = dict(zip(RENDER_INPUTS, ins))
+        out = _render_fwd(t0, t1, named, None, False)
+        ctx.save_for_backward(t0, t1, out["weights"], out["trans"], *ins)
+        ctx.mark_non_differentiable(out["median_depth"])
+        return tuple(out.get(k) for k in RENDER_TRAIN_OUTPUTS)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        t0, t1, weights, trans, *ins = ctx.saved_tensors
+        named = dict(zip(RENDER_INPUTS, ins))
+        need = ctx.needs_input_grad[2:]
+        if all(g is None for g in grads) or not any(need):
+            return (None,) * (2 + len(RENDER_INPUTS))
+        g = _lib.EmerRenderGrad()
+        upstream = []           # holds the fp32 copies while the struct points at them
+        for k, gr in zip(RENDER_TRAIN_OUTPUTS, grads):
+            if gr is not None and k != "median_depth":
+                upstream.append(_f32c(gr))
+                setattr(g, "g_" + k, upstream[-1].data_ptr())
+        d = [torch.empty_like(x) if (x is not None and n) else None for x, n in zip(ins, need)]
+        for k, dk in zip(RENDER_INPUTS, d):
+            if dk is not None:
+                setattr(g, "d_" + k, dk.data_ptr())
+        _lib.call("emer_render_bwd", ctypes.byref(_render_in(t0, t1, named, None)), _ptr(weights), _ptr(trans),
+                  ctypes.byref(g), _stream())
+        return (None, None, *d)
+
+
+def render_usable(n_channels: int) -> bool:
+    return n_channels <= RENDER_MAX_CHANNELS
+
+
+def render(t0: Tensor, t1: Tensor, ins: Dict[str, Optional[Tensor]], flows=None,
+           decomposition: bool = False) -> Dict[str, Tensor]:
+    """The body of ``rendering`` in one emer_render_fwd launch (and one emer_render_bwd in the backward).
+
+    ``ins``: the RENDER_INPUTS present (the rest None or missing), sigma / sigma_s / sigma_d / shadow [R,S], rgb /
+    rgb_s / rgb_d [R,S,3], dino / dino_s / dino_d [R,S,C], rgb_sky [R,3], dino_sky / dino_pe [R,C].  ``flows``:
+    (forward, backward) [R,S,3] flows, read in place when they are column slices of wider rows; only the decomposition
+    uses them.  Returns the RENDER_TRAIN_OUTPUTS the inputs define (opacity, depth, median_depth, rgb, shadow_ratio
+    [R,1] or [R,3]; dino, dino_pe_free [R,C]) and, with ``decomposition``, the RENDER_DECOMPOSITION outputs, which
+    have no gradient: ask for them only where nothing needs one."""
+    sigma = ins["sigma"]
+    if sigma.dim() != 2:
+        raise ValueError(f"render: sigma must be [R, S], got {tuple(sigma.shape)}")
+    r, s = sigma.shape
+    _need_cuda(t0, t1, *[v for v in ins.values() if v is not None], *(flows or ()))
+    shapes = {"sigma_s": (r, s), "sigma_d": (r, s), "shadow": (r, s), "rgb": (r, s, 3), "rgb_s": (r, s, 3),
+              "rgb_d": (r, s, 3), "rgb_sky": (r, 3)}
+    cins = {}
+    for k in RENDER_INPUTS:
+        v = ins.get(k)
+        if v is None:
+            continue
+        if k in ("shadow", "sigma_s", "sigma_d") and v.dim() == 3:
+            v = v.squeeze(-1)
+        want = shapes.get(k)
+        if k in ("dino", "dino_s", "dino_d"):
+            want = (r, s, v.shape[-1])
+        elif k in ("dino_sky", "dino_pe"):
+            want = (r, v.shape[-1])
+        if want is not None and tuple(v.shape) != want:
+            raise ValueError(f"render: {k} must be {want}, got {tuple(v.shape)}")
+        cins[k] = _f32c(v)
+    for a, b in (("sigma_s", "sigma_d"), ("rgb_s", "rgb_d"), ("dino_s", "dino_d")):
+        if (a in cins) != (b in cins):
+            raise ValueError(f"render: {a} and {b} come together")
+    if ("rgb_s" in cins or "dino_s" in cins) and "sigma_s" not in cins:
+        raise ValueError("render: static / dynamic colours or features need static and dynamic densities")
+    dino = cins.get("dino", cins.get("dino_s"))
+    c = 0 if dino is None else dino.shape[-1]
+    for k in ("dino_s", "dino_d", "dino_sky", "dino_pe"):
+        if k in cins and cins[k].shape[-1] != c:
+            raise ValueError(f"render: {k} has {cins[k].shape[-1]} channels, the features {c}")
+    if not 0 <= c <= RENDER_MAX_CHANNELS:
+        raise ValueError(f"render: {c} feature channels (at most {RENDER_MAX_CHANNELS})")
+    t0, t1 = _f32c(t0), _f32c(t1)
+    if decomposition:
+        if torch.is_grad_enabled() and any(v.requires_grad for v in ins.values() if v is not None):
+            raise ValueError("render: the decomposition outputs have no gradient; ask for them without grad")
+        rows = None
+        if flows is not None:
+            rows = [_rows(f, 3) for f in flows]
+            if rows[0][1] != rows[1][1] or rows[0][0].shape[0] != r * s:
+                rows = [(_f32c(f).reshape(-1, 3), 3) for f in flows]
+        return _render_fwd(t0, t1, cins, rows, True)
+    outs = _Render.apply(t0, t1, *[cins.get(k) for k in RENDER_INPUTS])
+    return {k: v for k, v in zip(RENDER_TRAIN_OUTPUTS, outs) if v is not None}
+
+
 # ----------------------------------------------------------------------------- training losses (csrc/losses.cu)
 LOSS_KINDS = {"l1": 0, "l2": 1, "smooth_l1": 2, "depth_l1": 3, "depth_l2": 4, "depth_smooth_l1": 5, "sky_bce": 6,
               "sparsity": 7, "entropy": 8}

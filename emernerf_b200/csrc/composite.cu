@@ -9,6 +9,7 @@
 // (coalesced 128-byte rows), warp-shuffle scans carry the running sums between 32-sample
 // chunks.  HBM-bound: ~ (3 reads + 2..3 writes) * 4 B per sample.
 #include "common.cuh"
+#include "ray_scan.cuh"
 
 namespace emer {
 
@@ -23,12 +24,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32) composite_fwd_kernel(
     const int64_t ray = (int64_t)blockIdx.x * WARPS_PER_CTA + (threadIdx.x >> 5);
     if (ray >= n_rays) return;
     const int64_t base = ray * S;
-    float carry_e = 0.0f;     // sum of sigma*delta before this chunk
-    float carry_w = 0.0f;     // sum of weights before this chunk
-    float sum_w = 0.0f, sum_wm = 0.0f;
-    float med = 0.0f;
-    bool med_found = false;
-    float last_mid = 0.0f;
+    RayScan<true> scan;
     for (int s0 = 0; s0 < S; s0 += 32) {
         const int s = s0 + lane;
         const bool ok = s < S;
@@ -38,42 +34,20 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32) composite_fwd_kernel(
             b = __ldg(t1 + base + s);
             sg = __ldg(sigma + base + s);
         }
-        const float x = ok ? sg * (b - a) : 0.0f;
-        const float incl = warp_scan_incl(x, lane);
-        const float e_excl = carry_e + (incl - x);
-        const float T = expf(-e_excl);
-        const float alpha = 1.0f - expf(-x);
-        const float w = ok ? T * alpha : 0.0f;
-        const float mid = (a + b) / 2.0f;
+        float T;
+        const float w = scan.step(a, b, sg, ok, s0, S, lane, T);
         if (ok) {
             if (weights) weights[base + s] = w;
             if (trans) trans[base + s] = T;
             if (cdf) cdf[ray * (S + 1) + s] = 1.0f - T;
         }
-        const float w_incl = warp_scan_incl(w, lane);
-        const float cw = carry_w + w_incl;
-        // median: first sample with cumulative weight >= 0.5 (searchsorted side="left")
-        const unsigned hit = __ballot_sync(0xffffffffu, ok && (cw >= 0.5f));
-        if (!med_found && hit) {
-            const int first = __ffs(hit) - 1;
-            med = __shfl_sync(0xffffffffu, mid, first);
-            med_found = true;
-        }
-        // last valid midpoint (index clamp to S-1 when the ray never reaches 0.5)
-        const int last_lane = min(31, S - 1 - s0);
-        last_mid = __shfl_sync(0xffffffffu, mid, last_lane);
-        sum_w += w;
-        sum_wm = fmaf(w, mid, sum_wm);
-        carry_e += __shfl_sync(0xffffffffu, incl, 31);
-        carry_w += __shfl_sync(0xffffffffu, w_incl, 31);
     }
-    sum_w = warp_sum(sum_w);
-    sum_wm = warp_sum(sum_wm);
+    float op, dep, med;
+    scan.finish(op, dep, med);
     if (lane == 0) {
-        const float op = fminf(fmaxf(sum_w, 1e-6f), 1.0f);
         if (opacity) opacity[ray] = op;
-        if (depth) depth[ray] = sum_wm / op;
-        if (median) median[ray] = med_found ? med : last_mid;
+        if (depth) depth[ray] = dep;
+        if (median) median[ray] = med;
         if (cdf) cdf[ray * (S + 1) + S] = 1.0f;     // 1 - cat(trans, 0)[-1]
     }
 }

@@ -5,6 +5,9 @@
   every accumulate_along_rays                                      -> emer_accumulate_fwd/bwd
   proposal sampling                                                -> PropNetEstimator (emer_pdf_resample)
 
+With ``EMER_RENDERING=fused`` the whole body of ``rendering`` (blend, accumulations, sky / PE terms, decomposition) is
+one emer_render_fwd launch and one emer_render_bwd launch instead (csrc/render.cu); the default is ``torch``.
+
 Two behaviours of the reference are preserved on purpose:
   * the per-level proposal closures all bind the LAST proposal network (render_utils.py:357-359
     builds ``[lambda *args: prop_sigma_fn(*args, p) for p in proposal_networks]``; Python closes over
@@ -15,6 +18,7 @@ Two behaviours of the reference are preserved on purpose:
 """
 from __future__ import annotations
 
+import os
 from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
@@ -38,9 +42,78 @@ def render_weights_opacity_depth_from_density(t_starts: Tensor, t_ends: Tensor, 
 _FLOW_KEYS = ("forward_flow", "backward_flow", "forward_pred_backward_flow", "backward_pred_forward_flow")
 
 
+# "fused": the body of ``rendering`` as one emer_render_fwd launch (and one emer_render_bwd), csrc/render.cu;
+# "torch": emer_composite_* and one emer_accumulate_* per accumulated quantity, with the blend in torch ops
+RENDERING = os.environ.get("EMER_RENDERING", "torch")
+
+# results key -> emer_render input
+_RENDER_KEYS = {"density": "sigma", "static_density": "sigma_s", "dynamic_density": "sigma_d", "rgb": "rgb",
+                "static_rgb": "rgb_s", "dynamic_rgb": "rgb_d", "shadow_ratio": "shadow", "rgb_sky": "rgb_sky",
+                "dino_feat": "dino", "static_dino_feat": "dino_s", "dynamic_dino_feat": "dino_d",
+                "dino_sky_feat": "dino_sky", "dino_pe": "dino_pe"}
+
+
+def _fused_rendering(t_starts: Tensor, t_ends: Tensor, results: Dict[str, Tensor],
+                     return_decomposition: bool) -> Optional[Dict[str, Tensor]]:
+    """``rendering``'s outputs from ``_ops.render``, or None where the kernel does not cover the field's results (more
+    than 256 feature channels, the decomposition under grad, results with neither colours nor features): the caller
+    then takes the op-by-op path."""
+    decomposed = "static_density" in results and "dynamic_density" in results
+    has_rgb = "rgb" in results or (decomposed and "static_rgb" in results and "dynamic_rgb" in results)
+    plain_dino = "dino_feat" in results
+    has_dino = plain_dino or (decomposed and "static_dino_feat" in results and "dynamic_dino_feat" in results)
+    if not (has_rgb or has_dino):
+        return None
+    if has_dino and results["dino_feat" if plain_dino else "static_dino_feat"].shape[-1] > _ops.RENDER_MAX_CHANNELS:
+        return None
+    ins = {"sigma": results["density"].squeeze(-1)}
+    for k, name in _RENDER_KEYS.items():
+        if k == "density" or k not in results:
+            continue
+        if name in ("sigma_s", "sigma_d") and not decomposed:
+            continue
+        if name in ("rgb_s", "rgb_d", "shadow") and ("rgb" in results or not has_rgb):
+            continue                       # the reference blends (and reads the shadow) only without a plain rgb
+        if name in ("dino_s", "dino_d") and (plain_dino or not has_dino):
+            continue
+        if name in ("dino_sky", "dino_pe") and not has_dino:
+            continue
+        if name == "rgb_sky" and not has_rgb:
+            continue
+        ins[name] = results[k]
+    decomp = return_decomposition and decomposed
+    if decomp and torch.is_grad_enabled() and any(v.requires_grad for v in ins.values()):
+        return None
+    flows = None
+    if decomp and "forward_flow" in results and "rgb_s" in ins:
+        flows = (results["forward_flow"], results["backward_flow"])
+    r = _ops.render(t_starts, t_ends, ins, flows=flows, decomposition=decomp)
+    out = {"density": ins["sigma"], "depth": r["depth"], "opacity": r["opacity"], "median_depth": r["median_depth"]}
+    names = {"dino": "dino_feat"}
+    for k in ("rgb", "shadow_ratio", "dino", "dino_pe_free") + _ops.RENDER_DECOMPOSITION:
+        if k in r:
+            out[names.get(k, k)] = r[k]
+    if "dino_pe" in ins:
+        out["dino_pe"] = results["dino_pe"]
+    out["extras"] = {"weights": r["weights"], "trans": r["trans"]}
+    return out
+
+
 def rendering(t_starts: Tensor, t_ends: Tensor, query_fn: Optional[Callable] = None,
               return_decomposition: bool = False) -> Dict[str, Tensor]:
     results = query_fn(t_starts, t_ends)
+    if RENDERING == "fused":
+        out = _fused_rendering(t_starts, t_ends, results, return_decomposition)
+        if out is not None:
+            extras = out["extras"]
+            extras.update({"t_vals": (t_starts + t_ends) / 2.0, "t_dist": (t_ends - t_starts)})
+            for k in _FLOW_KEYS:
+                if k in results:
+                    extras[k] = results[k]
+            if "static_density" in results and "dynamic_density" in results:
+                extras["static_density"] = results["static_density"]
+                extras["dynamic_density"] = results["dynamic_density"]
+            return out
     density = results["density"].squeeze(-1)
     weights, trans, opacity, depth, median_depth, _ = _ops.composite(t_starts, t_ends, density)
     acc = _ops.accumulate

@@ -255,6 +255,104 @@ int emer_accumulate_fwd(const float* w, const float* v, float* out, int64_t n_ra
 int emer_accumulate_bwd(const float* w, const float* v, const float* g, float* dw, float* dv,
                         int64_t n_rays, int n_samples, int c, void* stream);
 
+/* ---- the whole body of `rendering` in one launch each way (replaces radiance_fields/render_utils.py:48-287: the
+ *      static / dynamic ratios, the shadow product, the blended colour and features, every accumulate_along_rays, the
+ *      sky and PE terms and the decomposition outputs), csrc/render.cu ---------------------------------------------
+ * Per ray, S samples, C feature channels (1 <= C <= 256).  Every input but t0, t1, sigma may be NULL (absent); every
+ * output may be NULL (not wanted).  Per-sample tensors are [R,S] or [R,S,3] / [R,S,C] rows, per-ray ones [R], [R,3] or
+ * [R,C], all dense, except the flows: R*S rows of 3 floats with row stride ld_flow (column slices of the flow MLP's
+ * 6-wide rows).  w = weights, r_s = sigma_s / (sigma + 1e-6), r_d = sigma_d / (sigma + 1e-6), w_s / w_d = the weights
+ * of sigma_s / sigma_d alone, op = opacity:
+ *   weights, trans, opacity, depth, median_depth      bit-identical to emer_composite_fwd's
+ *   rgb           = sum w*rgb  (rgb given)  or  sum w*(r_s*rgb_s*(1 - shadow) + r_d*rgb_d),  + rgb_sky*(1 - op)
+ *   shadow_ratio  = sum w*shadow^2
+ *   dino_pe_free  = sum w*dino  or  sum w*(r_s*dino_s + r_d*dino_d),  + dino_sky*(1 - op);   dino = dino_pe_free + dino_pe
+ * and, for evaluation (emer_render_bwd has no gradient for these):
+ *   static_ / dynamic_opacity, _depth                  as opacity / depth of sigma_s / sigma_d
+ *   static_rgb    = sum w_s*rgb_s + rgb_sky*(1 - static_opacity);   dynamic_rgb = sum w_d*rgb_d
+ *   shadow_reduced_static_rgb = sum w_s*rgb_s*(1 - shadow);  shadow_only_static_rgb = sum w_s*rgb_s*shadow + 1 - shadow
+ *   shadow        = sum w*shadow;   forward_flow / backward_flow = sum w_d*flow
+ *   static_dino   = sum w_s*dino_s + dino_sky*(1 - op)  (the TOTAL opacity, as the reference);  dynamic_dino = sum w_d*dino_d */
+typedef struct emer_render_in {
+    const float* t0;            /* [R,S] */
+    const float* t1;            /* [R,S] */
+    const float* sigma;         /* [R,S] */
+    const float* sigma_s;       /* [R,S]; sigma_s and sigma_d come together */
+    const float* sigma_d;
+    const float* rgb;           /* [R,S,3] */
+    const float* rgb_s;         /* [R,S,3]; rgb_s and rgb_d (and the sigmas) come together */
+    const float* rgb_d;
+    const float* shadow;        /* [R,S] */
+    const float* rgb_sky;       /* [R,3] */
+    const float* dino;          /* [R,S,C] */
+    const float* dino_s;        /* [R,S,C]; dino_s and dino_d (and the sigmas) come together */
+    const float* dino_d;
+    const float* dino_sky;      /* [R,C] */
+    const float* dino_pe;       /* [R,C] */
+    const float* fwd_flow;      /* R*S rows of 3, row stride ld_flow */
+    const float* bwd_flow;
+    int64_t ld_flow;
+    int64_t n_rays;
+    int32_t n_samples;
+    int32_t n_dino;             /* C */
+} emer_render_in;
+
+typedef struct emer_render_out {
+    float* weights;             /* [R,S] */
+    float* trans;               /* [R,S] */
+    float* opacity;             /* [R] */
+    float* depth;
+    float* median_depth;
+    float* rgb;                 /* [R,3] */
+    float* shadow_ratio;        /* [R] */
+    float* dino;                /* [R,C] */
+    float* dino_pe_free;        /* [R,C] */
+    float* static_opacity;      /* [R] */
+    float* dynamic_opacity;
+    float* static_depth;
+    float* dynamic_depth;
+    float* static_rgb;          /* [R,3] */
+    float* dynamic_rgb;
+    float* shadow_reduced_static_rgb;
+    float* shadow_only_static_rgb;
+    float* shadow;              /* [R] */
+    float* forward_flow;        /* [R,3] */
+    float* backward_flow;
+    float* static_dino;         /* [R,C] */
+    float* dynamic_dino;
+} emer_render_out;
+
+/* Gradients of emer_render_fwd's training outputs (NULL = zero) and of its inputs (WRITTEN, not accumulated; NULL =
+ * not wanted).  Deterministic: no float atomics. */
+typedef struct emer_render_grad {
+    const float* g_weights;     /* [R,S]: the line-of-sight and sky-weight losses differentiate the weights */
+    const float* g_trans;       /* [R,S] */
+    const float* g_opacity;     /* [R] */
+    const float* g_depth;
+    const float* g_rgb;         /* [R,3] */
+    const float* g_shadow_ratio;/* [R] */
+    const float* g_dino;        /* [R,C] */
+    const float* g_dino_pe_free;/* [R,C] */
+    float* d_sigma;             /* [R,S] */
+    float* d_sigma_s;
+    float* d_sigma_d;
+    float* d_rgb;               /* [R,S,3] */
+    float* d_rgb_s;
+    float* d_rgb_d;
+    float* d_shadow;            /* [R,S] */
+    float* d_rgb_sky;           /* [R,3] */
+    float* d_dino;              /* [R,S,C] */
+    float* d_dino_s;
+    float* d_dino_d;
+    float* d_dino_sky;          /* [R,C] */
+    float* d_dino_pe;
+} emer_render_grad;
+
+int emer_render_fwd(const emer_render_in* in, const emer_render_out* out, void* stream);
+/* weights, trans: emer_render_fwd's outputs for the same inputs. */
+int emer_render_bwd(const emer_render_in* in, const float* weights, const float* trans, const emer_render_grad* grad,
+                    void* stream);
+
 /* ---- ray generation (replaces datasets/base/pixel_source.py:39-76 get_rays and the per-ray gathers / coordinate
  *      assembly of get_train_rays, :699-719) ------------------------------------------------------------------ */
 /* Per ray i: m = img_idx[i] (or i when per_ray_mats, or 0), c2w[m] (4x4 row-major), intrinsics[m] (3x3):
