@@ -12,14 +12,15 @@
 //   L * 2^D * F * 4 (corner reads) + D*4 (position) + L*F*4 (output)
 //   = 1452 B (3-D 10x4), 2736 B (4-D 10x4), 300 B (3-D 8x1).
 //
-// Mapping (forward and table scatter): level-group-major, see level_group() below.  One thread per
-// (point, group of G levels); the launch is ordered so that the resident CTAs work on one group at
-// a time, and each hashed level's table (or its gradient slice) is read from HBM about once and
-// then served from L2.  The static 122 MB grid runs one level per group: 0.52 -> 0.35 ms (gather)
-// and 0.90 -> 0.49 ms (scatter) per 524 288 ray-coherent points against the point-major order
-// (H100 80GB HBM3, 400 W power limit).  All 2^D corner gathers of a level are issued back to back
-// (16-byte LDG for F=4) before the first use.  The input gradient (never needed in training) stays
-// one thread per point, all levels.
+// Mapping (forward and table scatter): level-group-major, see level_groups() below.  One thread per
+// (point, group of up to G levels); the launch is ordered so that the resident CTAs work on one group
+// at a time, and each hashed level's table (or its gradient slice) is read from HBM about once and
+// then served from L2.  The forward writes every 32-byte output sector whole, in one store
+// instruction: a row's sector holds a pair of F = 4 levels, and lane pairs swap halves.  Per 524 288
+// ray-coherent points of the static 122 MB grid (H100 80GB HBM3, 700 W): gather 0.34 -> 0.21 ms,
+// scatter 0.48 -> 0.43 ms against one level per group (DESIGN.md §4).  All 2^D corner gathers of a
+// level are issued back to back (16-byte LDG for F=4) before the first use.  The input gradient
+// (never needed in training) stays one thread per point, all levels.
 #include "common.cuh"
 
 namespace emer {
@@ -51,6 +52,12 @@ __device__ __forceinline__ uint32_t grid_index(const uint32_t (&c)[D], uint32_t 
     }
     return idx;
 }
+
+// Diagnostic build only (tools/microbench_grid_sectors.py): the forward writes and the table scatter reads a
+// level-major [L, N, F] buffer instead of [N, L*F], i.e. whole sectors at any schedule.  Never set in the library.
+#ifndef EMER_GRID_DIAG_LEVEL_MAJOR
+#define EMER_GRID_DIAG_LEVEL_MAJOR 0
+#endif
 
 // Positions are streamed (evict-first), so they do not push table lines out of L2.
 template <int D>
@@ -116,38 +123,55 @@ __device__ __forceinline__ void locate(const float (&p)[D], float scale, uint32_
     }
 }
 
-// Level-group schedule of the forward and the table scatter: a thread handles one point and G
-// consecutive levels, blockIdx.x is the point block and blockIdx.y the level group.  CTAs are
-// dispatched x-fastest, so the CTAs resident at any moment work on one group (two at a boundary),
-// and only those levels' tables compete for L2 instead of the whole grid.
-//
-// G: with F = 4 a hashed level of a 2^20-entry map is 16 MiB, and two such levels already thrash
-// H100's L2 (a pair of fine levels takes 1.2x the time of its two levels alone), so each level is
-// its own group, although a thread then writes half of a 32-byte output sector.  Narrower
-// features keep G*F = 8 floats, one whole sector per thread: the F = 1 proposal grids (8 levels,
-// 19-22 MB in all) fit L2 as a whole and run as a single group.
+// Level-group schedule of the forward and the table scatter: blockIdx.x is the point block and
+// blockIdx.y the level group.  CTAs are dispatched x-fastest, so the CTAs resident at any moment work
+// on one group (two at a boundary), and only those levels' tables compete for L2.
+// Group k = levels first(k) .. first(k) + count(k) - 1, packed 4 bits per group (a dynamically
+// indexed parameter array would be copied to the stack).
+struct LevelGroups {
+    uint64_t first, count;
+    __device__ int first_of(int k) const { return (int)((first >> (4 * k)) & 15u); }
+    __device__ int count_of(int k) const { return (int)((count >> (4 * k)) & 15u); }
+};
+
+// G: levels per step of a thread, one 32-byte sector of a row for F = 1 and 2.  A group is one step,
+// or for F = 4 one or two (a level pair).
 template <int F>
 constexpr int level_group() {
     return F == 4 ? 1 : 8 / F;
 }
 
+// output / upstream-gradient element (i, l) as float-F vector index
+__device__ __forceinline__ int64_t out_vec(int64_t i, int l, int L, int64_t n) {
+#if EMER_GRID_DIAG_LEVEL_MAJOR
+    return (int64_t)l * n + i;
+#else
+    return i * L + l;
+#endif
+}
+
 template <int D, int F, int G>
-__global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd,
+__global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd, const LevelGroups lg,
                                                        const float* __restrict__ x,
                                                        const float* __restrict__ table,
                                                        float* __restrict__ y, int64_t n) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    const bool active = i < n;                  // no early exit: lane pairs exchange outputs below
     const emer_grid_desc& g = gd.g;
     const int L = g.n_levels;
-    const int l0 = blockIdx.y * G;
+    const int l0 = lg.first_of(blockIdx.y);
+    const int cnt = lg.count_of(blockIdx.y);
     float p[D];
-    load_point<D>(x, i, p);
-    float* yo = y + i * (int64_t)(L * F);
 #pragma unroll
-    for (int j = 0; j < G; ++j) {
+    for (int d = 0; d < D; ++d) p[d] = 0.0f;
+    if (active) load_point<D>(x, i, p);
+    // F = 4 level pairs of an even L are the 32-byte sectors of the rows
+    const bool sector_pairs = !EMER_GRID_DIAG_LEVEL_MAJOR && F == 4 && cnt == 2 && !(L & 1);
+    float4 held = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+#pragma unroll
+    for (int j = 0; j < (F == 4 ? 2 * G : G); ++j) {
         const int l = l0 + j;
-        if (l >= L) break;
+        if (j >= cnt) break;
         const float scale = g.scale[l];
         const uint32_t res = g.resolution[l];
         const uint32_t off = g.offset[l];
@@ -185,12 +209,36 @@ __global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd,
             for (int f = 0; f < F; ++f) acc[f] = fmaf(wt[c], val[c].v[f], acc[f]);
         // outputs are streamed: evict-first, so they do not push table lines out of L2
         if constexpr (F == 4) {
-            __stcs(reinterpret_cast<float4*>(yo) + l, make_float4(acc[0], acc[1], acc[2], acc[3]));
-        } else if constexpr (F == 2) {
-            __stcs(reinterpret_cast<float2*>(yo) + l, make_float2(acc[0], acc[1]));
-        } else {
+            const float4 v = make_float4(acc[0], acc[1], acc[2], acc[3]);
+            if (!sector_pairs) {
+                if (active) __stcs(reinterpret_cast<float4*>(y) + out_vec(i, l, L, n), v);
+            } else if (j == 0) {
+                held = v;
+            } else {
+                // The sector of row r holds levels (l0, l0+1).  A lane pair (rows r0, r0+1) swaps halves so that
+                // each of its two stores writes one whole sector: the even lane level l0, the odd lane level
+                // l0+1, first of row r0, then of row r0+1.  Two 16-byte stores of one thread are two partial
+                // sector writes, which cost as much as writing the levels in separate passes.
+                const bool odd = threadIdx.x & 1;
+                const float4 send = odd ? held : v;
+                float4 recv;
+                recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
+                recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
+                recv.z = __shfl_xor_sync(0xffffffffu, send.z, 1);
+                recv.w = __shfl_xor_sync(0xffffffffu, send.w, 1);
+                const int64_t r0 = i & ~(int64_t)1;
+                float4* yl = reinterpret_cast<float4*>(y) + l0 + (odd ? 1 : 0);
+                if (r0 < n) __stcs(yl + r0 * L, odd ? recv : held);
+                if (r0 + 1 < n) __stcs(yl + (r0 + 1) * L, odd ? v : recv);
+            }
+        } else if (active) {
+            const int64_t q = out_vec(i, l, L, n);
+            if constexpr (F == 2) {
+                __stcs(reinterpret_cast<float2*>(y) + q, make_float2(acc[0], acc[1]));
+            } else {
 #pragma unroll
-            for (int f = 0; f < F; ++f) __stcs(yo + l * F + f, acc[f]);
+                for (int f = 0; f < F; ++f) __stcs(y + q * F + f, acc[f]);
+            }
         }
     }
 }
@@ -220,7 +268,7 @@ __global__ void grid_indices_kernel(const GridDescDev gd, const float* __restric
     }
 }
 
-// Table gradient, on the level-group schedule of the forward.  dtable is accumulated with vector
+// Table gradient, level-group-major like the forward (with its own pairs, level_groups()).  dtable is accumulated with vector
 // reductions (red.global.add.v4.f32 for F=4: one 16-byte L2 atomic per corner) into the caller's
 // buffer, which is added to and never overwritten; the resident CTAs' reductions then land in
 // one group's gradient slices, which stay in L2.
@@ -231,7 +279,7 @@ __global__ void grid_indices_kernel(const GridDescDev gd, const float* __restric
 // partial sums of a run are combined with a segmented shuffle reduction and only the run's first
 // lane issues the reductions.
 template <int D, int F, int G>
-__global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev gd,
+__global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev gd, const LevelGroups lg,
                                                              const float* __restrict__ x,
                                                              const float* __restrict__ dy,
                                                              float* __restrict__ dtable, int64_t n) {
@@ -240,29 +288,32 @@ __global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev g
     const int lane = threadIdx.x & 31;
     const emer_grid_desc& g = gd.g;
     const int L = g.n_levels;
-    const int l0 = blockIdx.y * G;
+    const int l0 = lg.first_of(blockIdx.y);
+    const int cnt = lg.count_of(blockIdx.y);
     float p[D];
 #pragma unroll
     for (int d = 0; d < D; ++d) p[d] = 0.0f;
     if (active) load_point<D>(x, i, p);
-    const float* dyo = dy + (active ? i : 0) * (int64_t)(L * F);
+    const int64_t ia = active ? i : 0;
 #pragma unroll
-    for (int j = 0; j < G; ++j) {
+    for (int j = 0; j < (F == 4 ? 2 * G : G); ++j) {
         const int l = l0 + j;
-        if (l >= L) break;                      // uniform over the grid
+        if (j >= cnt) break;                    // uniform over the grid
         float g_out[F];
 #pragma unroll
         for (int f = 0; f < F; ++f) g_out[f] = 0.0f;
+        const int64_t q = out_vec(ia, l, L, n);
         if (active) {                           // streamed: evict-first
             if constexpr (F == 4) {
-                float4 t = __ldcs(reinterpret_cast<const float4*>(dyo) + l);
+                const float4* dq = reinterpret_cast<const float4*>(dy) + q;
+                float4 t = __ldcs(dq);
                 g_out[0] = t.x; g_out[1] = t.y; g_out[2] = t.z; g_out[3] = t.w;
             } else if constexpr (F == 2) {
-                float2 t = __ldcs(reinterpret_cast<const float2*>(dyo) + l);
+                float2 t = __ldcs(reinterpret_cast<const float2*>(dy) + q);
                 g_out[0] = t.x; g_out[1] = t.y;
             } else {
 #pragma unroll
-                for (int f = 0; f < F; ++f) g_out[f] = __ldcs(dyo + l * F + f);
+                for (int f = 0; f < F; ++f) g_out[f] = __ldcs(dy + q * F + f);
             }
         }
         bool any = false;
@@ -448,12 +499,38 @@ static int validate(const emer_grid_desc* g) {
 
 using namespace emer;
 
+// The level groups of a launch, in launch order (blockIdx.y).  F = 1 / 2: G = 8 / F levels, one sector of a
+// row.  F = 4: levels (2k, 2k+1), one sector of a row when L is even, are paired in the forward whenever L is even;
+// the scatter pairs them only while both tables fit L2 with room to spare, since two hashed 16 MiB levels make
+// its reductions miss (see DESIGN.md §4).
+template <int F>
+static int level_groups(const emer_grid_desc& g, bool forward, LevelGroups& lg) {
+    constexpr uint64_t kScatterPairBytes = 24ull << 20;
+    const int L = g.n_levels;
+    int n = 0;
+    for (int l = 0; l < L; ++n) {
+        int c = level_group<F>();
+        if (F == 4) {
+            const bool pair = !(l & 1) && l + 1 < L &&
+                              (forward ? !(L & 1)
+                                       : (uint64_t)(g.offset[l + 2] - g.offset[l]) * F * 4 <= kScatterPairBytes);
+            c = pair ? 2 : 1;
+        }
+        c = c < L - l ? c : L - l;
+        lg.first |= (uint64_t)l << (4 * n);
+        lg.count |= (uint64_t)c << (4 * n);
+        l += c;
+    }
+    return n;
+}
+
 template <int D, int F>
 static void launch_fwd(const GridDescDev& gd, const float* x, const float* table, float* y, int64_t n,
                        cudaStream_t st) {
-    constexpr int G = level_group<F>();
-    const dim3 blocks((unsigned)ceil_div(n, 256), (unsigned)ceil_div(gd.g.n_levels, G));
-    grid_fwd_kernel<D, F, G><<<blocks, 256, 0, st>>>(gd, x, table, y, n);
+    LevelGroups lg{0, 0};
+    const int groups = level_groups<F>(gd.g, true, lg);
+    const dim3 blocks((unsigned)ceil_div(n, 256), (unsigned)groups);
+    grid_fwd_kernel<D, F, level_group<F>()><<<blocks, 256, 0, st>>>(gd, lg, x, table, y, n);
 }
 
 extern "C" int emer_grid_fwd(const emer_grid_desc* g, const float* x, const float* table, float* y,
@@ -492,9 +569,9 @@ static void launch_bwd(const GridDescDev& gd, const float* x, const float* table
                        float* dtable, float* dx, int64_t n, cudaStream_t st) {
     const unsigned blocks = (unsigned)ceil_div(n, 256);
     if (dtable) {
-        constexpr int G = level_group<F>();
-        const dim3 grid(blocks, (unsigned)ceil_div(gd.g.n_levels, G));
-        grid_bwd_table_kernel<D, F, G><<<grid, 256, 0, st>>>(gd, x, dy, dtable, n);
+        LevelGroups lg{0, 0};
+        const dim3 grid(blocks, (unsigned)level_groups<F>(gd.g, false, lg));
+        grid_bwd_table_kernel<D, F, level_group<F>()><<<grid, 256, 0, st>>>(gd, lg, x, dy, dtable, n);
     }
     if (dx) grid_bwd_dx_kernel<D, F><<<blocks, 256, 0, st>>>(gd, x, table, dy, dx, n);
 }
