@@ -88,6 +88,9 @@ _SIGNATURES = {
     "emer_cycle_loss_bwd": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, _P, _P, _P, _P, _P],
     "emer_render_fwd": [POINTER(EmerRenderIn), POINTER(EmerRenderOut), _P],
     "emer_render_bwd": [POINTER(EmerRenderIn), _P, _P, POINTER(EmerRenderGrad), _P],
+    "emer_image_metrics": [_P, _P, c_int64, c_int64, c_int, _P, _P, c_int64, _P, c_int64, c_int, _P, _P, _P],
+    "emer_depth_rmse": [_P, _P, c_int64, _P, _P, _P],
+    "emer_scene_flow_metrics": [_P, _P, c_int64, _P, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])
@@ -166,6 +169,10 @@ def tag_of(name: str, args) -> str:
             return f"kind{args[0]}_R{args[4]}_S{args[5]}"
         if name in ("emer_cycle_loss_fwd", "emer_cycle_loss_bwd"):
             return f"N{args[8]}"
+        if name == "emer_image_metrics":
+            return f"H{args[2]}_W{args[3]}_C{args[4]}_F{args[10]}"
+        if name in ("emer_depth_rmse", "emer_scene_flow_metrics"):
+            return f"N{args[2]}"
         if name == "emer_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("_save" if args[19].value else "")
     except Exception:

@@ -1,0 +1,178 @@
+"""The evaluation metrics of the reference on the device (csrc/metrics.cu): ``datasets/metrics.py``'s ``compute_psnr``,
+``compute_ssim``, ``compute_valid_depth_rmse`` and ``compute_scene_flow_metrics`` with the same signatures, return types
+and keys, plus the per-image metric block of ``radiance_fields/video_utils.py:render`` and its aggregation.
+
+    from emernerf_b200 import metrics
+    per_image.append(metrics.image_metrics(rgb, pixels, dynamic_mask, dino_feat, features))   # no host sync
+    results = metrics.summarize(per_image)                                                   # one sync
+
+Every function is one library launch.  ``image_metrics`` returns 0-d fp64 device tensors and can be captured in a CUDA
+graph; the functions that return Python floats sync once, for that float.
+
+Differences from the reference, all deliberate:
+  * SSIM's window moments and map are fp64 (skimage computes them in the images' dtype, float32 here); the results
+    agree with skimage's float32 path to its own rounding, about 1e-6.
+  * PSNRs, RMSE and the flow statistics accumulate in fp64, so they are the fp64 values of the reference's formulas.
+  * Inputs are cast to fp32 on the device; numpy arrays are moved to the current CUDA device first.  Any other
+    non-CUDA tensor is an error, as everywhere in this package.
+  * ``collect_centroids`` and ``eval_few_shot_occ`` (the kNN occupancy evaluation) are not here.
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Optional, Union
+
+import numpy as np
+import torch
+from torch import Tensor
+
+from . import _lib, _ops
+
+__all__ = ["compute_psnr", "compute_ssim", "compute_valid_depth_rmse", "compute_scene_flow_metrics", "image_metrics",
+           "summarize"]
+
+WORKSPACE_BYTES = 81920          # EMER_METRICS_WORKSPACE_BYTES
+MAX_CHANNELS = 4                 # image channels
+MAX_FEATURE_CHANNELS = 256
+WINDOW = 7                       # SSIM window: images need at least 7 x 7 pixels
+IMAGE_OUT = ("psnr", "ssim", "masked_psnr", "masked_ssim", "feat_psnr", "masked_feat_psnr", "mask_count",
+             "pred_min", "pred_max", "target_min", "target_max")         # EMER_METRIC_* order
+FLOW_KEYS = ("EPE3D", "acc3d_strict", "acc3d_relax", "outlier", "angle_error")
+SUMMARY_KEYS = ("psnr", "ssim", "feat_psnr", "masked_psnr", "masked_ssim", "masked_feat_psnr")
+_WS: Dict[object, Tensor] = {}
+
+
+def _workspace(dev: torch.device) -> Tensor:
+    """The device's metrics workspace: zeroed once and left zeroed by every call (the last CTA resets its ticket), so
+    it is shared by all calls on the device's stream and by graph replays.  Created outside graph capture."""
+    ws = _WS.get(dev)
+    if ws is None:
+        if dev.type == "cuda" and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("emernerf_b200.metrics: run image_metrics once before capturing it in a CUDA graph")
+        ws = torch.zeros(WORKSPACE_BYTES // 4, dtype=torch.int32, device=dev)
+        _WS[dev] = ws
+    return ws
+
+
+def _numpy_device() -> torch.device:
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _tensor(x: Union[Tensor, np.ndarray]) -> Tensor:
+    """numpy arrays go to the current CUDA device (the reference's compute_psnr / compute_ssim accept them)."""
+    if isinstance(x, Tensor):
+        return x
+    return torch.as_tensor(np.asarray(x)).to(_numpy_device())
+
+
+def _image_launch(pred: Tensor, target: Tensor, mask: Optional[Tensor] = None, feat_pred: Optional[Tensor] = None,
+                  feat_target: Optional[Tensor] = None) -> Tensor:
+    """One emer_image_metrics launch; returns its fp64 out[11] on the device."""
+    _ops._need_cuda(pred, target, mask, feat_pred, feat_target)
+    if pred.dim() != 3 or pred.shape != target.shape:
+        raise ValueError(f"image metrics: prediction {tuple(pred.shape)} and target {tuple(target.shape)} must be the "
+                         "same [H, W, C]")
+    h, w, c = pred.shape
+    if not 1 <= c <= MAX_CHANNELS:
+        raise ValueError(f"image metrics: {c} channels (1..{MAX_CHANNELS})")
+    if h < WINDOW or w < WINDOW:
+        raise ValueError(f"image metrics: a {h}x{w} image is smaller than the {WINDOW}x{WINDOW} SSIM window")
+    x, y = _ops._f32c(pred), _ops._f32c(target)
+    m = None
+    if mask is not None:
+        if mask.numel() != h * w:
+            raise ValueError(f"image metrics: mask {tuple(mask.shape)} for a {h}x{w} image")
+        m = _ops._f32c(mask.reshape(-1))
+    fx = fy = None
+    ld_x = ld_y = cf = 0
+    if feat_pred is not None and feat_target is not None:
+        if feat_pred.dim() != 3 or feat_pred.shape != feat_target.shape or tuple(feat_pred.shape[:2]) != (h, w):
+            raise ValueError(f"image metrics: features {tuple(feat_pred.shape)} and {tuple(feat_target.shape)} must "
+                             f"be the same [{h}, {w}, Cf]")
+        cf = feat_pred.shape[-1]
+        if not 1 <= cf <= MAX_FEATURE_CHANNELS:
+            raise ValueError(f"image metrics: {cf} feature channels (1..{MAX_FEATURE_CHANNELS})")
+        fx, ld_x = _ops._rows(feat_pred, cf)
+        fy, ld_y = _ops._rows(feat_target, cf)
+    out = torch.empty(len(IMAGE_OUT), dtype=torch.float64, device=x.device)
+    _lib.call("emer_image_metrics", _ops._ptr(x), _ops._ptr(y), h, w, c, _ops._ptr(m), _ops._ptr(fx), ld_x,
+              _ops._ptr(fy), ld_y, cf, _ops._ptr(out), _ops._ptr(_workspace(x.device)), _ops._stream())
+    return out
+
+
+def _pair_launch(name: str, pred: Tensor, target: Tensor, n_out: int) -> Tensor:
+    _ops._need_cuda(pred, target)
+    p, t = _ops._f32c(pred), _ops._f32c(target)
+    out = torch.empty(n_out, dtype=torch.float64, device=p.device)
+    n = p.numel() // 3 if name == "emer_scene_flow_metrics" else p.numel()
+    _lib.call(name, _ops._ptr(p), _ops._ptr(t), n, _ops._ptr(out), _ops._ptr(_workspace(p.device)), _ops._stream())
+    return out
+
+
+def compute_valid_depth_rmse(prediction: Tensor, target: Tensor) -> float:
+    """RMSE between predicted and target depths over the rays with target > 0 (NaN when there is none)."""
+    prediction, target = prediction.squeeze(), target.squeeze()
+    if prediction.shape != target.shape:
+        raise ValueError(f"depth RMSE: {tuple(prediction.shape)} vs {tuple(target.shape)}")
+    return _pair_launch("emer_depth_rmse", prediction, target, 3)[0].item()
+
+
+def compute_psnr(prediction: Union[Tensor, np.ndarray], target: Union[Tensor, np.ndarray]) -> float:
+    """-10 log10(mean squared error) over all elements of two tensors of one shape."""
+    prediction, target = _tensor(prediction), _tensor(target)
+    if prediction.shape != target.shape:
+        raise ValueError(f"PSNR: {tuple(prediction.shape)} vs {tuple(target.shape)}")
+    return _pair_launch("emer_depth_rmse", prediction, target, 3)[2].item()
+
+
+def compute_ssim(prediction: Union[Tensor, np.ndarray], target: Union[Tensor, np.ndarray]) -> float:
+    """skimage's structural_similarity(target, prediction, data_range=1.0, channel_axis=-1) of two [H, W, C] images,
+    after the reference's range assertions (target first), which read the extrema of the same launch."""
+    prediction, target = _tensor(prediction), _tensor(target)
+    out = _image_launch(prediction, target).tolist()
+    o = dict(zip(IMAGE_OUT, out))
+    assert o["target_max"] <= 1.0 and o["target_min"] >= 0.0, "target must be in range [0, 1]"
+    assert o["pred_max"] <= 1.0 and o["pred_min"] >= 0.0, "prediction must be in range [0, 1]"
+    return o["ssim"]
+
+
+def compute_scene_flow_metrics(pred: Tensor, labels: Tensor) -> Dict[str, float]:
+    """The NSFP statistics (EPE3D, acc3d_strict, acc3d_relax, outlier, angle_error) of [..., N, 3] flows."""
+    if pred.shape != labels.shape or pred.dim() != 3 or pred.shape[-1] != 3:
+        raise ValueError(f"scene flow metrics: pred {tuple(pred.shape)} and labels {tuple(labels.shape)} must be the "
+                         "same [B, N, 3]")
+    out = _pair_launch("emer_scene_flow_metrics", pred, labels, 7).tolist()
+    return dict(zip(FLOW_KEYS, out[:5]))
+
+
+def image_metrics(rgb: Tensor, pixels: Tensor, dynamic_mask: Optional[Tensor] = None,
+                  dino_feat: Optional[Tensor] = None, features: Optional[Tensor] = None) -> Dict[str, Tensor]:
+    """The metric block of ``video_utils.render`` for one image, as 0-d fp64 device tensors, in one launch and with no
+    host sync: ``psnr`` and ``ssim``; with a mask, ``masked_psnr``, ``masked_ssim`` and ``mask_count`` (the masked
+    metrics are NaN when the mask is empty); with both feature maps, ``feat_psnr`` and, with a mask,
+    ``masked_feat_psnr``.  ``summarize`` aggregates a list of these as the reference does."""
+    have_feat = dino_feat is not None and features is not None
+    out = _image_launch(rgb, pixels, dynamic_mask, dino_feat if have_feat else None, features if have_feat else None)
+    keys = ["psnr", "ssim"]
+    if dynamic_mask is not None:
+        keys += ["masked_psnr", "masked_ssim", "mask_count"]
+    if have_feat:
+        keys += ["feat_psnr"] + (["masked_feat_psnr"] if dynamic_mask is not None else [])
+    return {k: out[IMAGE_OUT.index(k)] for k in keys}
+
+
+def summarize(per_image: List[Dict[str, Tensor]]) -> Dict[str, float]:
+    """The reference's aggregation (``video_utils.py:45-47,421-428``): per metric, the mean over the images that
+    produced it, or -1 where none did.  The masked metrics count for an image whose mask is not empty, as the
+    reference's ``dynamic_mask.sum() > 0``.  One host sync for the whole list."""
+    flat = [v for d in per_image for v in d.values()]
+    values = torch.stack(flat).tolist() if flat else []
+    lists: Dict[str, List[float]] = {k: [] for k in SUMMARY_KEYS}
+    i = 0
+    for d in per_image:
+        got = dict(zip(d.keys(), values[i:i + len(d)]))
+        i += len(d)
+        for k in SUMMARY_KEYS:
+            if k not in got or (k.startswith("masked_") and not got.get("mask_count", 0.0) > 0):
+                continue
+            lists[k].append(got[k])
+    return {k: sum(v) / len(v) if len(v) > 0 else -1 for k, v in lists.items()}

@@ -435,6 +435,40 @@ int emer_cycle_loss_bwd(const float* f, int64_t ld_f, const float* b, int64_t ld
                         const float* bpf, int64_t ld_bpf, int64_t n, float coef, const float* fwd_out, const float* g,
                         float* d_fpb, float* d_bpf, void* stream);
 
+/* ---- evaluation metrics (csrc/metrics.cu).  Each call is ONE launch with no host sync; results are fp64 in a
+ *      caller-owned device array.  workspace: at least EMER_METRICS_WORKSPACE_BYTES of device memory, zeroed once by
+ *      its owner and left zeroed by every call (as the loss workspace above); sums are per CTA, then over CTAs in a
+ *      fixed order, so results are bit-identical on one device. --------------------------------------------------- */
+#define EMER_METRICS_WORKSPACE_BYTES 81920
+/* The metric block of one evaluation image (replaces radiance_fields/video_utils.py:205-247: compute_psnr, two
+ * skimage.metrics.structural_similarity calls on host copies, the masked PSNRs by boolean indexing, and the feature
+ * PSNRs).  pred, target: [H, W, C] dense, 1 <= C <= 4, H, W >= 7.  mask: [H, W] (nonzero = in the mask) or NULL.
+ * feat_pred, feat_target: H*W rows of feat_channels (<= 256) floats with row strides ld_feat_*, or both NULL.
+ * SSIM as skimage's (data_range 1, channel_axis -1): 7x7 uniform window with scipy's 'reflect' border, sample
+ * covariance 49/48, C1 = 0.01^2, C2 = 0.03^2, moments in fp64; ssim = mean over the interior [3, H-3) x [3, W-3) of
+ * every channel; masked_ssim = mean of the uncropped map over the masked pixels x C.  out[EMER_IMAGE_METRICS_OUT]:
+ * PSNR = -10 log10(mean squared error); a metric without its inputs (no mask, empty mask, no features) is NaN, and
+ * MASK_COUNT is NaN without a mask.  The extrema propagate NaN (as numpy's). */
+enum {
+    EMER_METRIC_PSNR = 0, EMER_METRIC_SSIM = 1, EMER_METRIC_MASKED_PSNR = 2, EMER_METRIC_MASKED_SSIM = 3,
+    EMER_METRIC_FEAT_PSNR = 4, EMER_METRIC_MASKED_FEAT_PSNR = 5, EMER_METRIC_MASK_COUNT = 6,
+    EMER_METRIC_PRED_MIN = 7, EMER_METRIC_PRED_MAX = 8, EMER_METRIC_TARGET_MIN = 9, EMER_METRIC_TARGET_MAX = 10,
+    EMER_IMAGE_METRICS_OUT = 11
+};
+int emer_image_metrics(const float* pred, const float* target, int64_t height, int64_t width, int channels,
+                       const float* mask, const float* feat_pred, int64_t ld_feat_pred, const float* feat_target,
+                       int64_t ld_feat_target, int feat_channels, double* out, void* workspace, void* stream);
+/* compute_valid_depth_rmse (datasets/metrics.py:12-28) without boolean indexing: over n values,
+ * out[0] = sqrt(mean((p - t)^2 over t > 0)) (NaN when no t > 0), out[1] = that count, and from the same pass
+ * out[2] = -10 log10(mean((p - t)^2) over all n), the PSNR of compute_psnr (datasets/metrics.py:31-47). */
+int emer_depth_rmse(const float* pred, const float* target, int64_t n, double* out, void* workspace, void* stream);
+/* compute_scene_flow_metrics (datasets/metrics.py:73-128) over n points of [n, 3] dense pred / labels:
+ * out[0] = EPE3D, out[1] = acc3d_strict, out[2] = acc3d_relax, out[3] = outlier, out[4] = angle_error (NaN when no
+ * |label| > 0.1), out[5] = the points in the angle mean, out[6] = n.  The fractions are counts / n; the dot products
+ * are clamped to the fp32 value of +-(1 - 1e-7), as torch rounds the reference's bounds. */
+int emer_scene_flow_metrics(const float* pred, const float* labels, int64_t n, double* out, void* workspace,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif
