@@ -91,6 +91,8 @@ _SIGNATURES = {
     "emer_image_metrics": [_P, _P, c_int64, c_int64, c_int, _P, _P, c_int64, _P, c_int64, c_int, _P, _P, _P],
     "emer_depth_rmse": [_P, _P, c_int64, _P, _P, _P],
     "emer_scene_flow_metrics": [_P, _P, c_int64, _P, _P, _P],
+    "emer_occ_accumulate": [_P, c_int64, c_int, _P, c_int64, _P, c_int64, c_int, c_float, _P, _P, _P, _P],
+    "emer_occ_classify": [_P, c_int64, c_int, _P, c_int64, _P, c_int64, _P, c_int, _P, c_float, _P, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])
@@ -173,6 +175,10 @@ def tag_of(name: str, args) -> str:
             return f"H{args[2]}_W{args[3]}_C{args[4]}_F{args[10]}"
         if name in ("emer_depth_rmse", "emer_scene_flow_metrics"):
             return f"N{args[2]}"
+        if name == "emer_occ_accumulate":
+            return f"C{args[2]}_K{args[7]}_N{args[6]}"
+        if name == "emer_occ_classify":
+            return f"C{args[2]}_K{args[8]}_N{args[6]}"
         if name == "emer_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("_save" if args[19].value else "")
     except Exception:

@@ -469,6 +469,32 @@ int emer_depth_rmse(const float* pred, const float* target, int64_t n, double* o
 int emer_scene_flow_metrics(const float* pred, const float* labels, int64_t n, double* out, void* workspace,
                             void* stream);
 
+/* ---- few-shot occupancy evaluation (csrc/occupancy.cu; replaces datasets/metrics.py:249-472, collect_centroids and
+ *      eval_few_shot_occ with knn_predict(knn_k=1, similarity="cosine"), and their boolean indexing, second field pass
+ *      and per-class .item() calls).  n voxels: feat rows of `channels` floats with row stride ld_feat (channels a
+ *      multiple of 4, at most EMER_OCC_MAX_CHANNELS; feat and ld_feat 16-byte aligned), density with stride
+ *      ld_density, labels int64.  A voxel is measured when density > threshold (strict; NaN fails).  Both calls ADD
+ *      into caller-owned buffers with one launch and no host sync, so frames and chunks accumulate.  workspace: at
+ *      least EMER_OCC_WORKSPACE_BYTES of device memory, zeroed once by its owner and left zeroed by every call (as
+ *      the metrics workspace above); per-CTA records are added in CTA order, so results are bit-identical on one
+ *      device. -------------------------------------------------------------------------------------------------- */
+#define EMER_OCC_MAX_CHANNELS 256
+#define EMER_OCC_MAX_CLASSES 32
+#define EMER_OCC_WORKSPACE_BYTES 16912640
+/* For the measured voxels with 0 <= label < n_classes (n_classes <= 32): sums[label, :] += feat row (fp64
+ * [n_classes, channels]) and counts[label] += 1 (int64 [n_classes]).  Other labels are skipped. */
+int emer_occ_accumulate(const float* feat, int64_t ld_feat, int channels, const float* density, int64_t ld_density,
+                        const int64_t* labels, int64_t n, int n_classes, float threshold, double* sums,
+                        int64_t* counts, void* workspace, void* stream);
+/* For the measured voxels: prediction = label_bank[argmax_j dot(q, c_j / (|c_j| + 1e-7))] in fp64 over the fp32
+ * centroids [n_classes, channels] (dense) and label_bank int64 [n_classes]; an exact tie goes to the lowest j.
+ * counts int64 [2 n_classes + 2] accumulates: [0, n_classes) voxels per label, [n_classes, 2 n_classes) correct
+ * predictions per label, [2 n_classes] measured voxels, [2 n_classes + 1] measured voxels whose label is outside
+ * [0, n_classes) (not classified). */
+int emer_occ_classify(const float* feat, int64_t ld_feat, int channels, const float* density, int64_t ld_density,
+                      const int64_t* labels, int64_t n, const float* centroids, int n_classes,
+                      const int64_t* label_bank, float threshold, int64_t* counts, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
