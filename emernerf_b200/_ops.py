@@ -1296,15 +1296,16 @@ LOSS_WORKSPACE_BYTES = 16384    # EMER_LOSS_WORKSPACE_BYTES
 _LOSS_WS: Dict[object, Tensor] = {}
 
 
-def _loss_workspace(dev: torch.device) -> Tensor:
-    """The device's loss workspace: zeroed once, left zeroed by every call (the last CTA resets its ticket), so it is
-    shared by all loss calls on the device's stream and by graph replays.  Created outside graph capture."""
-    ws = _LOSS_WS.get(dev)
+def _workspace(cache: Dict[object, Tensor], dev: torch.device, nbytes: int, what: str) -> Tensor:
+    """The device's entry of ``cache`` (one per kernel family: losses, metrics, occupancy): a workspace zeroed once and
+    left zeroed by every call (the last CTA resets its ticket), so it is shared by all of the family's calls on the
+    device's stream and by graph replays.  Created outside graph capture."""
+    ws = cache.get(dev)
     if ws is None:
         if dev.type == "cuda" and torch.cuda.is_current_stream_capturing():
-            raise RuntimeError("emernerf_b200 losses: run each loss once before capturing it in a CUDA graph")
-        ws = torch.zeros(LOSS_WORKSPACE_BYTES // 4, dtype=torch.int32, device=dev)
-        _LOSS_WS[dev] = ws
+            raise RuntimeError(f"emernerf_b200 {what}: run each call once before capturing it in a CUDA graph")
+        ws = torch.zeros(nbytes // 4, dtype=torch.int32, device=dev)
+        cache[dev] = ws
     return ws
 
 
@@ -1322,7 +1323,7 @@ class _PointwiseLoss(torch.autograd.Function):
             raise ValueError(f"pointwise loss: {tuple(a.shape)} vs {tuple(b.shape)}")
         out = torch.empty(2, dtype=torch.float32, device=ac.device)
         _lib.call("emer_pointwise_loss_fwd", kind, _ptr(ac), _ptr(bc), ac.numel(), p0, p1, pre, post, _ptr(out),
-                  _ptr(_loss_workspace(ac.device)), _stream())
+                  _ptr(_workspace(_LOSS_WS, ac.device, LOSS_WORKSPACE_BYTES, "losses")), _stream())
         ctx.save_for_backward(ac, bc, out)
         ctx.args = (kind, p0, p1, pre, post)
         ctx.shapes = (a.shape, None if b is None else b.shape)
@@ -1366,7 +1367,7 @@ class _RayLoss(torch.autograd.Function):
                              f"per-ray {tuple(gt.shape)}")
         out = torch.empty(2, dtype=torch.float32, device=wc.device)
         _lib.call("emer_ray_loss_fwd", kind, _ptr(wc), _ptr(tc), _ptr(gc), r, s, *consts, pre, post, _ptr(out),
-                  _ptr(_loss_workspace(wc.device)), _stream())
+                  _ptr(_workspace(_LOSS_WS, wc.device, LOSS_WORKSPACE_BYTES, "losses")), _stream())
         ctx.save_for_backward(wc, tc, gc, out)
         ctx.args = (kind, consts, pre, post)
         return out[0]
@@ -1427,7 +1428,8 @@ class _CycleLoss(torch.autograd.Function):
         args = [a for r in rows for a in (_ptr(r[0]), r[1])]
         n = rows[0][0].shape[0]
         out = torch.empty(6, dtype=torch.float32, device=rows[0][0].device)
-        _lib.call("emer_cycle_loss_fwd", *args, n, coef, _ptr(out), _ptr(_loss_workspace(out.device)), _stream())
+        _lib.call("emer_cycle_loss_fwd", *args, n, coef, _ptr(out),
+                  _ptr(_workspace(_LOSS_WS, out.device, LOSS_WORKSPACE_BYTES, "losses")), _stream())
         ctx.save_for_backward(*(r[0] for r in rows), out)
         ctx.lds = [r[1] for r in rows]
         ctx.coef, ctx.shape = coef, fpb.shape

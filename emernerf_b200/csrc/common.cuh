@@ -74,4 +74,22 @@ __device__ __forceinline__ float warp_scan_incl_rev(float v, int lane) {
     return v;
 }
 
+// Layer activations (EMER_ACT_*); the backward takes the stored OUTPUT y.
+__device__ __forceinline__ float act_fwd(float v, int act) {
+    if (act == EMER_ACT_RELU) return v > 0.0f ? v : 0.0f;
+    if (act == EMER_ACT_SIGMOID) return 1.0f / (1.0f + expf(-v));
+    return v;
+}
+
+__device__ __forceinline__ float act_bwd(float g, float y, int act) {
+    if (act == EMER_ACT_RELU) return y > 0.0f ? g : 0.0f;
+    if (act == EMER_ACT_SIGMOID) return g * (y * (1.0f - y));
+    return g;
+}
+
+// Density activation trunc_exp(raw - 1) of the reference (radiance_fields/radiance_field.py:828-835); its backward
+// clamps the exponent at 15.
+__device__ __forceinline__ float density_fwd(float raw) { return expf(raw - 1.0f); }
+__device__ __forceinline__ float density_bwd(float g, float raw) { return g * expf(fminf(raw - 1.0f, 15.0f)); }
+
 }  // namespace emer

@@ -3,52 +3,9 @@
 // 8 B/point (trunc_exp).  Reference: radiance_fields/nerf_utils.py:13-28,59-75;
 // radiance_fields/radiance_field.py:278-300,828-835.
 #include "common.cuh"
+#include "contract.cuh"
 
 namespace emer {
-
-struct Aabb {
-    float lo[3], hi[3];
-};
-
-// Forward arithmetic in exactly the reference's operation order (no FMA contraction):
-//   xn = (x - lo) / (hi - lo) * 2 - 1 ; mag = max_i |xn_i|
-//   y  = mag < 1 ? xn : (2 - 1/mag) * (xn / mag) ; out = y / 4 + 0.5 ; out *= all(0 < out < 1)
-__device__ __forceinline__ void contract_point(const float (&x)[3], const float* __restrict__ aabb,
-                                               int unbounded, int apply_selector, float (&out)[3],
-                                               float (&xn)[3], float& mag, int& amax, bool& sel) {
-    float m = -1.0f;
-    int am = 0;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        float lo = __ldg(aabb + d), hi = __ldg(aabb + 3 + d);
-        float t = (x[d] - lo) / (hi - lo);
-        if (unbounded) t = t * 2.0f - 1.0f;
-        xn[d] = t;
-        float a = fabsf(t);
-        if (a > m) { m = a; am = d; }
-    }
-    mag = m;
-    amax = am;
-    bool s = true;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        float y;
-        if (unbounded) {
-            y = (m < 1.0f) ? xn[d] : (2.0f - 1.0f / m) * (xn[d] / m);
-            y = y / 4.0f + 0.5f;
-        } else {
-            y = xn[d];
-        }
-        out[d] = y;
-        s = s && (y > 0.0f) && (y < 1.0f);
-    }
-    if (!apply_selector) s = true;
-    sel = s;
-    if (!s) {
-#pragma unroll
-        for (int d = 0; d < 3; ++d) out[d] = out[d] * 0.0f;   // keeps NaN propagation of `p * selector`
-    }
-}
 
 __global__ void contract_fwd_kernel(const float* __restrict__ pos, const float* __restrict__ aabb,
                                     const float* __restrict__ time, float* __restrict__ out,
@@ -56,10 +13,11 @@ __global__ void contract_fwd_kernel(const float* __restrict__ pos, const float* 
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     float x[3] = {__ldg(pos + i * 3), __ldg(pos + i * 3 + 1), __ldg(pos + i * 3 + 2)};
-    float o[3], xn[3], mag;
+    float lo[3], hi[3], o[3], xn[3], mag;
     int am;
     bool sel;
-    contract_point(x, aabb, unbounded, apply_selector, o, xn, mag, am, sel);
+    load_box(aabb, lo, hi);
+    contract_point(x, lo, hi, unbounded, apply_selector, o, xn, mag, am, sel);
     if (out_dim == 4) {
         reinterpret_cast<float4*>(out)[i] = make_float4(o[0], o[1], o[2], time ? __ldg(time + i) : 0.0f);
     } else {
@@ -76,10 +34,11 @@ __global__ void contract_bwd_kernel(const float* __restrict__ pos, const float* 
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     float x[3] = {__ldg(pos + i * 3), __ldg(pos + i * 3 + 1), __ldg(pos + i * 3 + 2)};
-    float o[3], xn[3], mag;
+    float lo[3], hi[3], o[3], xn[3], mag;
     int am;
     bool sel;
-    contract_point(x, aabb, unbounded, apply_selector, o, xn, mag, am, sel);
+    load_box(aabb, lo, hi);
+    contract_point(x, lo, hi, unbounded, apply_selector, o, xn, mag, am, sel);
     float g[3];
 #pragma unroll
     for (int d = 0; d < 3; ++d) g[d] = sel ? __ldg(dout + i * out_dim + d) : 0.0f;
@@ -113,8 +72,7 @@ __global__ void contract_bwd_kernel(const float* __restrict__ pos, const float* 
     }
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
-        float lo = __ldg(aabb + d), hi = __ldg(aabb + 3 + d);
-        float k = (unbounded ? 2.0f : 1.0f) / (hi - lo);
+        float k = (unbounded ? 2.0f : 1.0f) / (hi[d] - lo[d]);
         dpos[i * 3 + d] = gxn[d] * k;
     }
 }
@@ -122,13 +80,13 @@ __global__ void contract_bwd_kernel(const float* __restrict__ pos, const float* 
 __global__ void trunc_exp_fwd_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y,
                                      int64_t n) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) y[i] = expf(__ldg(x + i * ldx) - 1.0f);
+    if (i < n) y[i] = density_fwd(__ldg(x + i * ldx));
 }
 
 __global__ void trunc_exp_bwd_kernel(const float* __restrict__ x, int64_t ldx,
                                      const float* __restrict__ dy, float* __restrict__ dx, int64_t n) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dx[i] = __ldg(dy + i) * expf(fminf(__ldg(x + i * ldx) - 1.0f, 15.0f));
+    if (i < n) dx[i] = density_bwd(__ldg(dy + i), __ldg(x + i * ldx));
 }
 
 }  // namespace emer

@@ -223,8 +223,8 @@ __global__ void __launch_bounds__(THREADS, 1) field_fwd_kernel(const FwdParams p
             const float v0 = geo[4 * j] + bb1_s[c], v1 = geo[4 * j + 1] + bb1_s[c + 1];
             const float v2 = geo[4 * j + 2] + bb1_s[c], v3 = geo[4 * j + 3] + bb1_s[c + 1];
             if (j == 0 && q == 0) {
-                if (ok0) p.sigma[row0] = expf(v0 - 1.0f);
-                if (ok1) p.sigma[row1] = expf(v2 - 1.0f);
+                if (ok0) p.sigma[row0] = density_fwd(v0);
+                if (ok1) p.sigma[row1] = density_fwd(v2);
             }
             if (p.save_hg) {
                 st2(p.save_hg + row0 * 128 + H + c, v0, v1, ok0);

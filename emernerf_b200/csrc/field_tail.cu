@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(256) field_tail_fwd_kernel(const float* __rest
             const float* src = feats + pt * ld_feats + q * 4;
             if (vec_in) v = __ldg(reinterpret_cast<const float4*>(src));
             else v = make_float4(__ldg(src), __ldg(src + 1), __ldg(src + 2), __ldg(src + 3));
-            if (q == 0 && sigma) sigma[pt] = expf(v.x - 1.0f);
+            if (q == 0 && sigma) sigma[pt] = density_fwd(v.x);
         } else {
             v = *reinterpret_cast<const float4*>(tail + (q - gq) * 4);
         }
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(256) field_tail_bwd_kernel(const float* __rest
         for (int s = lane; s < S; s += 32) {
             const int64_t pt = ray * S + s;
             const float g = __ldg(d_sigma + pt);
-            if (g != 0.0f) d_out[pt * ld_out] += g * expf(fminf(__ldg(feats + pt * ld_feats) - 1.0f, 15.0f));
+            if (g != 0.0f) d_out[pt * ld_out] += density_bwd(g, __ldg(feats + pt * ld_feats));
         }
     }
     if (d_emb) {

@@ -22,36 +22,13 @@
 // level are issued back to back (16-byte LDG for F=4) before the first use.  The input gradient
 // (never needed in training) stays one thread per point, all levels.
 #include "common.cuh"
+#include "grid_common.cuh"
 
 namespace emer {
 
 struct GridDescDev {
     emer_grid_desc g;
 };
-
-template <int D>
-__device__ __forceinline__ uint32_t grid_index(const uint32_t (&c)[D], uint32_t res, uint32_t size,
-                                               bool hashed) {
-    uint32_t idx = 0;
-    if (hashed) {
-        // coherent prime hash; level size is 2^log2_hashmap_size whenever a level is hashed
-        constexpr uint32_t P[4] = {1u, 2654435761u, 805459861u, 3674653429u};
-#pragma unroll
-        for (int d = 0; d < D; ++d) idx ^= c[d] * P[d];
-        idx &= (size - 1u);
-    } else {
-        uint32_t stride = 1;
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-            if (stride <= size) {
-                idx += c[d] * stride;
-                stride *= res;
-            }
-        }
-        if (idx >= size) idx %= size;   // only the +1 corner on the far faces wraps
-    }
-    return idx;
-}
 
 // Diagnostic build only (tools/microbench_grid_sectors.py): the forward writes and the table scatter reads a
 // level-major [L, N, F] buffer instead of [N, L*F], i.e. whole sectors at any schedule.  Never set in the library.
@@ -107,19 +84,6 @@ __device__ __forceinline__ void red_add_entry(float* lt, uint32_t idx, const flo
     } else {
 #pragma unroll
         for (int f = 0; f < F; ++f) atomicAdd(lt + (size_t)idx * F + f, v[f]);
-    }
-}
-
-// pos = fmaf(scale, x, 0.5); cell = (uint32)(int)floor(pos); frac = pos - floor(pos)
-template <int D>
-__device__ __forceinline__ void locate(const float (&p)[D], float scale, uint32_t (&c0)[D],
-                                       float (&w)[D]) {
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-        float pos = fmaf(scale, p[d], 0.5f);
-        float fl = floorf(pos);
-        c0[d] = (uint32_t)(int)fl;
-        w[d] = pos - fl;
     }
 }
 
@@ -186,18 +150,8 @@ __global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd, con
 #pragma unroll
         for (int c = 0; c < (1 << D); ++c) {
             uint32_t cc[D];
-            float t = 1.0f;
-#pragma unroll
-            for (int d = 0; d < D; ++d) {
-                if ((c >> d) & 1) {
-                    t = t * w[d];
-                    cc[d] = c0[d] + 1u;
-                } else {
-                    t = t * (1.0f - w[d]);
-                    cc[d] = c0[d];
-                }
-            }
-            wt[c] = t;
+            corner_cell<D>(c, c0, cc);
+            wt[c] = corner_weight<D>(c, w);
             val[c] = load_entry<F>(lt, grid_index<D>(cc, res, size, hashed));
         }
         float acc[F];
@@ -260,8 +214,7 @@ __global__ void grid_indices_kernel(const GridDescDev gd, const float* __restric
 #pragma unroll
         for (int c = 0; c < (1 << D); ++c) {
             uint32_t cc[D];
-#pragma unroll
-            for (int d = 0; d < D; ++d) cc[d] = c0[d] + ((c >> d) & 1);
+            corner_cell<D>(c, c0, cc);
             out[(i * g.n_levels + l) * (1 << D) + c] =
                 (int32_t)(off + grid_index<D>(cc, g.resolution[l], size, g.hashed[l] != 0));
         }
@@ -331,8 +284,7 @@ __global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev g
 #pragma unroll
         for (int c = 0; c < (1 << D); ++c) {
             uint32_t cc[D];
-#pragma unroll
-            for (int d = 0; d < D; ++d) cc[d] = c0[d] + ((c >> d) & 1);
+            corner_cell<D>(c, c0, cc);
             idx[c] = grid_index<D>(cc, res, size, hashed);
         }
         float* lt = dtable + (size_t)off * F;
@@ -357,9 +309,7 @@ __global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev g
             const int run_end = later ? (lane + __ffs(later) - 1) : 31;
 #pragma unroll
             for (int c = 0; c < (1 << D); ++c) {
-                float t = 1.0f;
-#pragma unroll
-                for (int d = 0; d < D; ++d) t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
+                const float t = corner_weight<D>(c, w);
                 float v[F];
 #pragma unroll
                 for (int f = 0; f < F; ++f) v[f] = t * g_out[f];
@@ -379,9 +329,7 @@ __global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev g
         } else if (any) {
 #pragma unroll
             for (int c = 0; c < (1 << D); ++c) {
-                float t = 1.0f;
-#pragma unroll
-                for (int d = 0; d < D; ++d) t = t * (((c >> d) & 1) ? w[d] : (1.0f - w[d]));
+                const float t = corner_weight<D>(c, w);
                 float v[F];
 #pragma unroll
                 for (int f = 0; f < F; ++f) v[f] = t * g_out[f];
@@ -439,8 +387,7 @@ __global__ void __launch_bounds__(256) grid_bwd_dx_kernel(const GridDescDev gd,
 #pragma unroll
         for (int c = 0; c < (1 << D); ++c) {
             uint32_t cc[D];
-#pragma unroll
-            for (int d = 0; d < D; ++d) cc[d] = c0[d] + ((c >> d) & 1);
+            corner_cell<D>(c, c0, cc);
             Vec<F> v = load_entry<F>(lt, grid_index<D>(cc, res, size, hashed));
             float t = 0.0f;
 #pragma unroll

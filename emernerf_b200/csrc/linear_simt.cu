@@ -23,19 +23,6 @@ constexpr int BK = 16;    // k slice
 constexpr int TM = 8;     // rows per thread
 constexpr int TN = 4;     // cols per thread
 
-__device__ __forceinline__ float act_fwd(float v, int act) {
-    if (act == EMER_ACT_RELU) return v > 0.0f ? v : 0.0f;
-    if (act == EMER_ACT_SIGMOID) return 1.0f / (1.0f + expf(-v));
-    return v;
-}
-
-// derivative expressed through the stored OUTPUT y
-__device__ __forceinline__ float act_bwd(float g, float y, int act) {
-    if (act == EMER_ACT_RELU) return y > 0.0f ? g : 0.0f;
-    if (act == EMER_ACT_SIGMOID) return g * (y * (1.0f - y));
-    return g;
-}
-
 // C[M, ncols] = A[M, kred] * B[kred, ncols] (+ epilogue).
 //   A(m, r): MODE_FWD  -> X[m*lda + r]
 //            MODE_BWD  -> dZ = dY[m*lda + r] * act'(Y[m*ldy + r])

@@ -20,17 +20,6 @@ constexpr int WGS = 2;                       // warpgroups per CTA
 constexpr int THREADS = WGS * 128;
 constexpr int KB = 4;                        // k steps per wgmma batch; the B panels are padded to a multiple of 8 KB
 
-__device__ __forceinline__ float act_fwd(float v, int act) {
-    if (act == EMER_ACT_RELU) return v > 0.0f ? v : 0.0f;
-    if (act == EMER_ACT_SIGMOID) return 1.0f / (1.0f + expf(-v));
-    return v;
-}
-__device__ __forceinline__ float act_bwd(float g, float y, int act) {
-    if (act == EMER_ACT_RELU) return y > 0.0f ? g : 0.0f;
-    if (act == EMER_ACT_SIGMOID) return g * (y * (1.0f - y));
-    return g;
-}
-
 struct Params {
     const float* a;       // fwd: X [n, lda]      bwd: dY [n, lda]
     int64_t lda;

@@ -13,6 +13,7 @@
 // Arithmetic is fp32 in the reference's op order; the Python-float constants arrive rounded once from double by the
 // caller (as torch rounds Python scalars).
 #include "common.cuh"
+#include "cta_reduce.cuh"
 
 namespace emer {
 
@@ -104,72 +105,30 @@ __device__ __forceinline__ float pointwise_term(const LossParams& p, int64_t i, 
 }
 
 // ---------------------------------------------------------------------------------------------- reduction
-// Sums of one CTA in a fixed order (warp tree, then warps in index order); valid in thread 0.
-template <typename T>
-__device__ __forceinline__ T block_sum(T v, T* sh) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) sh[wid] = v;
-    __syncthreads();
-    T t = 0;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < LOSS_WARPS; ++w) t += sh[w];
-    return t;
-}
-
-// Maximum of one CTA; valid in thread 0.
-__device__ __forceinline__ unsigned int block_max(unsigned int v, unsigned int* sh) {
-    v = __reduce_max_sync(0xffffffffu, v);
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) sh[wid] = v;
-    __syncthreads();
-    unsigned int t = 0u;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < LOSS_WARPS; ++w) t = max(t, sh[w]);
-    return t;
-}
-
-// Called by every thread after thread 0 has stored its CTA's partials: true in every thread of the CTA that takes the
-// last ticket, which then sees all partials.
-__device__ bool last_cta(LossWorkspace* ws) {
-    __shared__ bool last;
-    if (threadIdx.x == 0) {
-        __threadfence();
-        last = atomicAdd(&ws->ticket, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!last) return false;
-    __threadfence();
-    return true;
-}
-
 // Every CTA publishes its partials; the one that takes the last ticket adds them up in CTA order.  Returns true in
 // thread 0 of that CTA, with the totals in a / b / c.
 __device__ bool reduce_across_ctas(LossWorkspace* ws, float& a, float& b, long long& c) {
     __shared__ float shf[LOSS_WARPS];
     __shared__ long long shc[LOSS_WARPS];
-    a = block_sum(a, shf);
-    b = block_sum(b, shf);
-    c = block_sum(c, shc);
+    a = block_sum<LOSS_WARPS>(a, shf);
+    b = block_sum<LOSS_WARPS>(b, shf);
+    c = block_sum<LOSS_WARPS>(c, shc);
     if (threadIdx.x == 0) {
         ws->sum_a[blockIdx.x] = a;
         ws->sum_b[blockIdx.x] = b;
         ws->count[blockIdx.x] = c;
     }
-    if (!last_cta(ws)) return false;
+    if (!take_last_ticket(&ws->ticket)) return false;
     a = 0.0f; b = 0.0f; c = 0;
     for (int i = threadIdx.x; i < (int)gridDim.x; i += LOSS_THREADS) {
         a += __ldcg(ws->sum_a + i);
         b += __ldcg(ws->sum_b + i);
         c += __ldcg(ws->count + i);
     }
-    a = block_sum(a, shf);
-    b = block_sum(b, shf);
-    c = block_sum(c, shc);
-    if (threadIdx.x == 0) ws->ticket = 0u;        // ready for the next call (and the next graph replay)
+    a = block_sum<LOSS_WARPS>(a, shf);
+    b = block_sum<LOSS_WARPS>(b, shf);
+    c = block_sum<LOSS_WARPS>(c, shc);
+    release_ticket(&ws->ticket);
     return threadIdx.x == 0;
 }
 
@@ -370,15 +329,15 @@ __global__ void __launch_bounds__(LOSS_THREADS) cycle_loss_fwd_kernel(const Cycl
         mx[CYC_FPB] = max(mx[CYC_FPB], norm_key(fp));
         mx[CYC_BPF] = max(mx[CYC_BPF], norm_key(bp));
     }
-    sum = block_sum(sum, shf);
+    sum = block_sum<LOSS_WARPS>(sum, shf);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) mx[k] = block_max(mx[k], shu);
+    for (int k = 0; k < 4; ++k) mx[k] = block_max<LOSS_WARPS>(mx[k], shu);
     if (threadIdx.x == 0) {
         p.ws->sum_a[blockIdx.x] = sum;
 #pragma unroll
         for (int k = 0; k < 4; ++k) p.ws->norm_max[k][blockIdx.x] = mx[k];
     }
-    if (!last_cta(p.ws)) return;
+    if (!take_last_ticket(&p.ws->ticket)) return;
     sum = 0.0f;
 #pragma unroll
     for (int k = 0; k < 4; ++k) mx[k] = 0u;
@@ -387,11 +346,11 @@ __global__ void __launch_bounds__(LOSS_THREADS) cycle_loss_fwd_kernel(const Cycl
 #pragma unroll
         for (int k = 0; k < 4; ++k) mx[k] = max(mx[k], __ldcg(p.ws->norm_max[k] + c));
     }
-    sum = block_sum(sum, shf);
+    sum = block_sum<LOSS_WARPS>(sum, shf);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) mx[k] = block_max(mx[k], shu);
+    for (int k = 0; k < 4; ++k) mx[k] = block_max<LOSS_WARPS>(mx[k], shu);
+    release_ticket(&p.ws->ticket);
     if (threadIdx.x == 0) {
-        p.ws->ticket = 0u;
         const float count = (float)(p.n * 3);
         p.out[0] = 0.5f * (sum / count) * p.coef;
         p.out[1] = count;

@@ -15,6 +15,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "cta_reduce.cuh"
 
 namespace emer {
 
@@ -97,19 +98,14 @@ __device__ void block_reduce(Partials& p) {
 // Every CTA publishes its partials; the one that takes the last ticket adds them up in CTA order.  Returns true in
 // thread 0 of that CTA, with the totals in p.
 __device__ bool reduce_across_ctas(Partials& p, MetricsWorkspace* ws) {
-    __shared__ bool last;
     block_reduce(p);
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int k = 0; k < P_N; ++k) ws->sum[k][blockIdx.x] = p.s[k];
 #pragma unroll
         for (int k = 0; k < E_N; ++k) ws->ext[k][blockIdx.x] = p.e[k];
-        __threadfence();
-        last = atomicAdd(&ws->ticket, 1u) == gridDim.x - 1;
     }
-    __syncthreads();
-    if (!last) return false;
-    __threadfence();
+    if (!take_last_ticket(&ws->ticket)) return false;
     init(p);
     for (int i = threadIdx.x; i < (int)gridDim.x; i += MET_THREADS) {
         double s[P_N];
@@ -121,7 +117,7 @@ __device__ bool reduce_across_ctas(Partials& p, MetricsWorkspace* ws) {
         combine(p, s, e);
     }
     block_reduce(p);
-    if (threadIdx.x == 0) ws->ticket = 0u;        // ready for the next call (and the next graph replay)
+    release_ticket(&ws->ticket);
     return threadIdx.x == 0;
 }
 

@@ -17,6 +17,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "cta_reduce.cuh"
 
 namespace emer {
 
@@ -54,18 +55,12 @@ struct OccParams {
 // the records of all CTAs, in CTA order, into out_d / out_i and resets the ticket.
 __device__ void occ_finish(const double* sd, int nd, const unsigned long long* si, int ni, double* out_d,
                            int64_t* out_i, unsigned char* ws) {
-    __shared__ bool last;
     unsigned int* ticket = (unsigned int*)ws;
     double* pd = (double*)(ws + OCC_WS_HEADER);
     long long* pi = (long long*)(pd + (size_t)gridDim.x * nd);
     for (int i = threadIdx.x; i < nd; i += blockDim.x) pd[(size_t)blockIdx.x * nd + i] = sd[i];
     for (int i = threadIdx.x; i < ni; i += blockDim.x) pi[(size_t)blockIdx.x * ni + i] = (long long)si[i];
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
+    if (!take_last_ticket(ticket)) return;
     for (int i = threadIdx.x; i < nd; i += blockDim.x) {
         double s = 0.0;
         for (int b = 0; b < (int)gridDim.x; ++b) s += __ldcg(pd + (size_t)b * nd + i);
@@ -76,7 +71,7 @@ __device__ void occ_finish(const double* sd, int nd, const unsigned long long* s
         for (int b = 0; b < (int)gridDim.x; ++b) s += __ldcg(pi + (size_t)b * ni + i);
         out_i[i] += s;
     }
-    if (threadIdx.x == 0) *ticket = 0u;              // ready for the next call
+    release_ticket(ticket);
 }
 
 // class of row r if it passes the filter (density > threshold, NaN fails; 0 <= label < k), else -1

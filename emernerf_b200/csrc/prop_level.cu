@@ -5,11 +5,16 @@
 // Replaces, per level, ~15 launches of the modular path (third_party/nerfacc_prop_net.py:147-170 with
 // render_utils.py:314-324 and radiance_field.py:825-841 of the reference) and every intermediate
 // [R,S,*] tensor: the only HBM traffic is the table gathers (L2-resident: 18-22 MB tables) and the
-// [R, n+1] edges / CDF rows.  The resampling arithmetic is the same code as emer_pdf_resample
-// (bit-exact s/t edges); the MLP runs on the FP32 FMA pipe with weights broadcast from shared memory.
+// [R, n+1] edges / CDF rows.  Resampling, contraction and grid lookup are the device functions of emer_pdf_resample,
+// emer_contract_fwd and emer_grid_fwd (sampling.cuh, contract.cuh, grid_common.cuh), so s/t edges, positions and table
+// indices are bit-identical to the modular path's; the MLP runs on the FP32 FMA pipe with weights broadcast from
+// shared memory.
 //
 // One warp per ray; lane l owns edges / samples l, l+32, ... (n <= 256).
 #include "common.cuh"
+#include "contract.cuh"
+#include "grid_common.cuh"
+#include "sampling.cuh"
 
 namespace emer {
 
@@ -40,18 +45,6 @@ constexpr int PL_MAX_EDGES = 257;
 constexpr int PL_HID = 64;
 constexpr int PL_MAX_IN = 16;
 
-__device__ __forceinline__ float pl_s_to_t(float s, float s_min, float s_max, int kind) {
-    const float v = s * s_max + (1.0f - s) * s_min;
-    switch (kind) {
-        case EMER_STOT_UNIFORM: return v;
-        case EMER_STOT_LINDISP: return 1.0f / v;
-        case EMER_STOT_SQRT: return v * v;
-        case EMER_STOT_LOG: return expf(v);
-        case EMER_STOT_UNIFORM_LINDISP: return v < 0.5f ? v * 400.0f : (1.0f / (2.0f - 2.0f * v)) * 200.0f;
-        default: return v < 0.5f ? 2.0f * v : 1.0f / (2.0f - 2.0f * v);
-    }
-}
-
 // what a warp needs of its ray
 struct PlRay {
     float ox, oy, oz, dx, dy, dz, lo3[3], hi3[3];
@@ -61,8 +54,7 @@ __device__ __forceinline__ PlRay pl_load_ray(const float* origins, const float* 
     PlRay rc;
     rc.ox = __ldg(origins + ray * 3); rc.oy = __ldg(origins + ray * 3 + 1); rc.oz = __ldg(origins + ray * 3 + 2);
     rc.dx = __ldg(dirs + ray * 3); rc.dy = __ldg(dirs + ray * 3 + 1); rc.dz = __ldg(dirs + ray * 3 + 2);
-#pragma unroll
-    for (int d = 0; d < 3; ++d) { rc.lo3[d] = __ldg(aabb + d); rc.hi3[d] = __ldg(aabb + 3 + d); }
+    load_box(aabb, rc.lo3, rc.hi3);
     return rc;
 }
 
@@ -76,66 +68,24 @@ __device__ __forceinline__ void pl_encode(const emer_grid_desc& g, const float* 
     const float tt = t0 + t1;
     // positions = origins + dirs * (t0 + t1) / 2   (render_utils.py:318)
     float pos[3] = {rc.ox + rc.dx * tt / 2.0f, rc.oy + rc.dy * tt / 2.0f, rc.oz + rc.dz * tt / 2.0f};
-    // contraction + selector (same operation order as contract_point in elementwise.cu)
-    float xn[3], m = -1.0f;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        float q = (pos[d] - rc.lo3[d]) / (rc.hi3[d] - rc.lo3[d]);
-        if (unbounded) q = q * 2.0f - 1.0f;
-        xn[d] = q;
-        m = fmaxf(m, fabsf(q));
-    }
-    bool sel = true;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        float y;
-        if (unbounded) {
-            y = (m < 1.0f) ? xn[d] : (2.0f - 1.0f / m) * (xn[d] / m);
-            y = y / 4.0f + 0.5f;
-        } else {
-            y = xn[d];
-        }
-        xc[d] = y;
-        sel = sel && (y > 0.0f) && (y < 1.0f);
-    }
-    if (!sel) { xc[0] = xc[0] * 0.0f; xc[1] = xc[1] * 0.0f; xc[2] = xc[2] * 0.0f; }
-    // hash grid (3-D), same corner order / fma chain as grid_fwd_kernel
+    float xn[3], mag;
+    int amax;
+    bool sel;
+    contract_point(pos, rc.lo3, rc.hi3, unbounded, 1, xc, xn, mag, amax, sel);
 #pragma unroll
     for (int l = 0; l < L; ++l) {
-        const float scale = g.scale[l];
         const uint32_t res = g.resolution[l], off = g.offset[l], size = g.offset[l + 1] - off;
         const bool hashed = g.hashed[l] != 0;
         uint32_t c0[3];
         float w[3];
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-            const float ps = fmaf(scale, xc[d], 0.5f);
-            const float fl = floorf(ps);
-            c0[d] = (uint32_t)(int)fl;
-            w[d] = ps - fl;
-        }
+        locate<3>(xc, g.scale[l], c0, w);
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int cc = 0; cc < 8; ++cc) {
-            float wt = 1.0f;
+            const float wt = corner_weight<3>(cc, w);
             uint32_t ci[3];
-#pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                if ((cc >> d) & 1) { wt = wt * w[d]; ci[d] = c0[d] + 1u; }
-                else { wt = wt * (1.0f - w[d]); ci[d] = c0[d]; }
-            }
-            uint32_t idx = 0;
-            if (hashed) {
-                idx = (ci[0] * 1u) ^ (ci[1] * 2654435761u) ^ (ci[2] * 805459861u);
-                idx &= (size - 1u);
-            } else {
-                uint32_t stride = 1;
-#pragma unroll
-                for (int d = 0; d < 3; ++d)
-                    if (stride <= size) { idx += ci[d] * stride; stride *= res; }
-                if (idx >= size) idx %= size;
-            }
-            const float* e = table + ((size_t)off + idx) * F;
+            corner_cell<3>(cc, c0, ci);
+            const float* e = table + ((size_t)off + grid_index<3>(ci, res, size, hashed)) * F;
             if (LF_T > 0) acc[0] = fmaf(wt, __ldg(e), acc[0]);
             else for (int f = 0; f < F; ++f) acc[f] = fmaf(wt, __ldg(e + f), acc[f]);
         }
@@ -170,27 +120,12 @@ __global__ void __launch_bounds__(PL_WARPS * 32) prop_level_kernel(const PropPar
     if (ray >= p.n_rays) return;
     const int n = p.n, m1 = p.m1;
 
-    // ---- 1. inverse-CDF resampling (same arithmetic, same order as pdf_resample_kernel)
-    const float* c = p.prev_cdf + ray * m1;
-    const float* v = p.prev_s + ray * m1;
-    const float u_floor = __ldg(c), u_ceil = __ldg(c + m1 - 1);
-    const float u_step = (u_ceil - u_floor) / (float)n;
+    // ---- 1. inverse-CDF resampling
     const float bb = p.bias ? __ldg(p.bias + ray) : 0.5f;
     for (int k = lane; k <= n; k += 32) {
-        const float u = u_floor + ((float)k + (bb - 0.5f)) * u_step;
-        int lo = 0, hi = m1;
-        while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (__ldg(c + mid) > u) hi = mid;
-            else lo = mid + 1;
-        }
-        const int p0 = min(max(lo - 1, 0), m1 - 1), p1 = min(max(lo, 0), m1 - 1);
-        const float u_lo = __ldg(c + p0), u_hi = __ldg(c + p1), t_lo = __ldg(v + p0), t_hi = __ldg(v + p1);
-        const float du = u_hi - u_lo;
-        float s;
-        if (du < 1e-10f) s = (t_lo + t_hi) * 0.5f;
-        else s = (u - u_lo) * ((t_hi - t_lo) / du) + t_lo;
-        const float t = pl_s_to_t(s, p.s_min, p.s_max, p.stot_kind);
+        int bin;
+        const float s = resample_edge(p.prev_cdf + ray * m1, p.prev_s + ray * m1, m1, n, k, bb, bin);
+        const float t = s_to_t(s, p.s_min, p.s_max, p.stot_kind);
         p.out_s[ray * (n + 1) + k] = s;
         p.out_t[ray * (n + 1) + k] = t;
         t_edges[wid][k] = t;
@@ -219,7 +154,7 @@ __global__ void __launch_bounds__(PL_WARPS * 32) prop_level_kernel(const PropPar
                 h = h > 0.0f ? h : 0.0f;
                 raw = fmaf(w1s[j], h, raw);
             }
-            const float sigma = expf(raw - 1.0f);
+            const float sigma = density_fwd(raw);
             xdelta = sigma * (t1 - t0);
             if (p.out_sigma) p.out_sigma[ray * n + k] = sigma;
         }

@@ -3,29 +3,16 @@
 // Replaces nerfacc.pdf.importance_sampling (the one nerfacc CUDA kernel the reference hits by
 // default, third_party/nerfacc_prop_net.py:153,172) and _transform_stot (:317-339).
 // Integer work (upper-bound bin per output edge) is bit-exact against the oracle; the fp32
-// arithmetic is written operation by operation in the oracle's order (library built with
-// -fmad=false), so the produced s/t edges are bit-identical for identical CDFs.
+// arithmetic (sampling.cuh, which the fused proposal level includes too) is written operation by
+// operation in the oracle's order (library built with -fmad=false), so the produced s/t edges are
+// bit-identical for identical CDFs.
 //
 // Layout: vals, cdfs [R, m1] row-major; outputs [R, n+1].  One thread per output edge;
 // a ray's CDF row (<= 129 floats) is read through L1.  HBM-bound and tiny:
 // (2*m1 + 2*(n+1)) * 4 bytes per ray.
-#include "common.cuh"
+#include "sampling.cuh"
 
 namespace emer {
-
-__device__ __forceinline__ float s_to_t(float s, float s_min, float s_max, int kind) {
-    // icontract(s * s_max + (1 - s) * s_min)
-    const float v = s * s_max + (1.0f - s) * s_min;
-    switch (kind) {
-        case EMER_STOT_UNIFORM: return v;
-        case EMER_STOT_LINDISP: return 1.0f / v;
-        case EMER_STOT_SQRT: return v * v;
-        case EMER_STOT_LOG: return expf(v);
-        // torch evaluates `200 / x` as reciprocal(x) * 200 (Tensor.__rtruediv__): two roundings
-        case EMER_STOT_UNIFORM_LINDISP: return v < 0.5f ? v * 400.0f : (1.0f / (2.0f - 2.0f * v)) * 200.0f;
-        default: return v < 0.5f ? 2.0f * v : 1.0f / (2.0f - 2.0f * v);
-    }
-}
 
 __global__ void pdf_resample_kernel(const float* __restrict__ vals, const float* __restrict__ cdfs,
                                     int m1, int n, const float* __restrict__ bias, float s_min,
@@ -36,29 +23,8 @@ __global__ void pdf_resample_kernel(const float* __restrict__ vals, const float*
     if (tid >= total) return;
     const int64_t ray = tid / (n + 1);
     const int k = (int)(tid - ray * (n + 1));
-    const float* c = cdfs + ray * m1;
-    const float* v = vals + ray * m1;
-    const float u_floor = __ldg(c);
-    const float u_ceil = __ldg(c + m1 - 1);
-    const float u_step = (u_ceil - u_floor) / (float)n;
-    const float b = bias ? __ldg(bias + ray) : 0.5f;
-    const float u = u_floor + ((float)k + (b - 0.5f)) * u_step;
-    // upper bound: first p in [0, m1] with c[p] > u
-    int lo = 0, hi = m1;
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(c + mid) > u) hi = mid;
-        else lo = mid + 1;
-    }
-    const int p = lo;
-    const int p0 = min(max(p - 1, 0), m1 - 1);
-    const int p1 = min(max(p, 0), m1 - 1);
-    const float u_lo = __ldg(c + p0), u_hi = __ldg(c + p1);
-    const float t_lo = __ldg(v + p0), t_hi = __ldg(v + p1);
-    const float du = u_hi - u_lo;
-    float s;
-    if (du < 1e-10f) s = (t_lo + t_hi) * 0.5f;
-    else s = (u - u_lo) * ((t_hi - t_lo) / du) + t_lo;
+    int p;
+    const float s = resample_edge(cdfs + ray * m1, vals + ray * m1, m1, n, k, bias ? __ldg(bias + ray) : 0.5f, p);
     out_s[tid] = s;
     if (out_t) out_t[tid] = s_to_t(s, s_min, s_max, kind);
     if (out_bins) out_bins[tid] = p;

@@ -64,18 +64,6 @@ OCC_FEATURE_DIM = 64             # the reference's width of a centroid when no f
 _OCC_WS: Dict[object, Tensor] = {}
 
 
-def _workspace(dev: torch.device) -> Tensor:
-    """The device's metrics workspace: zeroed once and left zeroed by every call (the last CTA resets its ticket), so
-    it is shared by all calls on the device's stream and by graph replays.  Created outside graph capture."""
-    ws = _WS.get(dev)
-    if ws is None:
-        if dev.type == "cuda" and torch.cuda.is_current_stream_capturing():
-            raise RuntimeError("emernerf_b200.metrics: run image_metrics once before capturing it in a CUDA graph")
-        ws = torch.zeros(WORKSPACE_BYTES // 4, dtype=torch.int32, device=dev)
-        _WS[dev] = ws
-    return ws
-
-
 def _numpy_device() -> torch.device:
     return torch.device("cuda", torch.cuda.current_device())
 
@@ -117,8 +105,9 @@ def _image_launch(pred: Tensor, target: Tensor, mask: Optional[Tensor] = None, f
         fx, ld_x = _ops._rows(feat_pred, cf)
         fy, ld_y = _ops._rows(feat_target, cf)
     out = torch.empty(len(IMAGE_OUT), dtype=torch.float64, device=x.device)
+    ws = _ops._workspace(_WS, x.device, WORKSPACE_BYTES, "metrics")
     _lib.call("emer_image_metrics", _ops._ptr(x), _ops._ptr(y), h, w, c, _ops._ptr(m), _ops._ptr(fx), ld_x,
-              _ops._ptr(fy), ld_y, cf, _ops._ptr(out), _ops._ptr(_workspace(x.device)), _ops._stream())
+              _ops._ptr(fy), ld_y, cf, _ops._ptr(out), _ops._ptr(ws), _ops._stream())
     return out
 
 
@@ -127,7 +116,8 @@ def _pair_launch(name: str, pred: Tensor, target: Tensor, n_out: int) -> Tensor:
     p, t = _ops._f32c(pred), _ops._f32c(target)
     out = torch.empty(n_out, dtype=torch.float64, device=p.device)
     n = p.numel() // 3 if name == "emer_scene_flow_metrics" else p.numel()
-    _lib.call(name, _ops._ptr(p), _ops._ptr(t), n, _ops._ptr(out), _ops._ptr(_workspace(p.device)), _ops._stream())
+    ws = _ops._workspace(_WS, p.device, WORKSPACE_BYTES, "metrics")
+    _lib.call(name, _ops._ptr(p), _ops._ptr(t), n, _ops._ptr(out), _ops._ptr(ws), _ops._stream())
     return out
 
 
@@ -203,12 +193,7 @@ def summarize(per_image: List[Dict[str, Tensor]]) -> Dict[str, float]:
 
 # ---------------------------------------------------------------------------------------------- few-shot occupancy
 def _occ_workspace(dev: torch.device) -> Tensor:
-    """The device's occupancy workspace, zeroed once and left zeroed by every call (as ``_workspace``)."""
-    ws = _OCC_WS.get(dev)
-    if ws is None:
-        ws = torch.zeros(OCC_WORKSPACE_BYTES // 4, dtype=torch.int32, device=dev)
-        _OCC_WS[dev] = ws
-    return ws
+    return _ops._workspace(_OCC_WS, dev, OCC_WORKSPACE_BYTES, "occupancy")
 
 
 def _occ_limits(n_classes: int, channels: int) -> None:
@@ -263,9 +248,10 @@ def collect_centroids(train_indices, dataset, model, device) -> Tuple[Tensor, Te
             if tuple(sums.shape) != (k, c):
                 raise ValueError(f"occupancy evaluation: {k} classes x {c} channels after {tuple(sums.shape)}")
             _ops._need_cuda(feat, density, labels, sums)
+            ws = _occ_workspace(feat.device)
             _lib.call("emer_occ_accumulate", _ops._ptr(feat), ld, c, _ops._ptr(density), 1, _ops._ptr(labels),
-                      feat.shape[0], k, OCC_DENSITY_THRESHOLD, _ops._ptr(sums), _ops._ptr(counts),
-                      _ops._ptr(_occ_workspace(feat.device)), _ops._stream())
+                      feat.shape[0], k, OCC_DENSITY_THRESHOLD, _ops._ptr(sums), _ops._ptr(counts), _ops._ptr(ws),
+                      _ops._stream())
     k = len(dataset.label_mapping)
     if sums is None:
         return torch.zeros(k, OCC_FEATURE_DIM, device=device), torch.arange(k, device=device)
@@ -300,9 +286,10 @@ def eval_few_shot_occ(test_indices, dataset, model, device, centroids_bank: Tens
             if feat.shape[1] != c:
                 raise ValueError(f"occupancy evaluation: {feat.shape[1]}-channel features for {c}-channel centroids")
             _ops._need_cuda(feat, density, labels, centroids, bank, counts)
+            ws = _occ_workspace(feat.device)
             _lib.call("emer_occ_classify", _ops._ptr(feat), ld, c, _ops._ptr(density), 1, _ops._ptr(labels),
                       feat.shape[0], _ops._ptr(centroids), k, _ops._ptr(bank), OCC_DENSITY_THRESHOLD,
-                      _ops._ptr(counts), _ops._ptr(_occ_workspace(feat.device)), _ops._stream())
+                      _ops._ptr(counts), _ops._ptr(ws), _ops._stream())
     got = counts.tolist()                           # the one host sync
     total, correct, measured, outside = got[:k], got[k:2 * k], got[2 * k], got[2 * k + 1]
     if outside:

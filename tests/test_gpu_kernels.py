@@ -252,6 +252,14 @@ def test_pdf_resample_bit_exact(m1, n, stratified):
     assert torch.equal(s_got.cpu(), iv.vals)
     assert torch.equal(t_got.cpu(), t_want)
     assert (s_got[:, 1:] >= s_got[:, :-1]).all()
+    # the fused proposal level draws the same edges from the same CDF rows (whatever its grid and MLP hold)
+    _, desc, geom = _grid("3d_f1")
+    zeros = lambda *shape: torch.zeros(*shape, device=DEV)
+    box = torch.tensor([-1.0, -1.0, -1.0, 1.0, 1.0, 1.0], device=DEV)
+    s_pl, t_pl, _ = _ops.prop_level(vals.to(DEV), cdfs.to(DEV), n, None if jit is None else jit.to(DEV), s_min, s_max,
+                                    "uniform_lindisp", zeros(R, 3), zeros(R, 3), box, True, desc,
+                                    zeros(geom.n_params), zeros(64, 4), zeros(64), zeros(1, 64), zeros(1))
+    assert torch.equal(s_pl, s_got) and torch.equal(t_pl, t_got)
 
 
 @pytest.mark.parametrize("kind", ["uniform", "lindisp", "sqrt", "uniform_lindisp_0"])
