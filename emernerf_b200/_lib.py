@@ -38,6 +38,24 @@ class EmerRenderOut(ctypes.Structure):
 class EmerRenderGrad(ctypes.Structure):
     _fields_ = [(k, _P) for k in RENDER_GRAD_PTRS]
 
+
+# host structs of emer_pixel_batch (include/emer_b200.h): field names and order as there
+PIXEL_BATCH_IN_PTRS = ("cand", "u_pick", "u_x", "u_y", "i_sel", "i_dy", "i_dx", "images", "sky_masks", "dynamic_masks",
+                       "features", "timestamps", "cam_ids", "c2w", "intrinsics")
+PIXEL_BATCH_OUT_PTRS = ("img_idx", "cam_idx", "pixels", "sky_masks", "dynamic_masks", "features", "timestamps",
+                        "origins", "viewdirs", "norms", "pixel_coords")
+
+
+class EmerPixelBatchIn(ctypes.Structure):
+    _fields_ = [(k, _P) for k in PIXEL_BATCH_IN_PTRS] + [
+        ("n_uniform", c_int64), ("n_importance", c_int64), ("height", c_int32), ("width", c_int32),
+        ("map_h", c_int32), ("map_w", c_int32), ("map_downscale", c_int32), ("feat_h", c_int32), ("feat_w", c_int32),
+        ("feat_c", c_int32), ("feat_scale_y", c_float), ("feat_scale_x", c_float)]
+
+
+class EmerPixelBatchOut(ctypes.Structure):
+    _fields_ = [(k, _P) for k in PIXEL_BATCH_OUT_PTRS]
+
 # number of kernels this library launched through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = 0
 
@@ -74,6 +92,8 @@ _SIGNATURES = {
     "emer_field_wgrad": [_P, c_int64, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, _P, c_int64, _P, _P,
                          c_int64, _P, _P, c_int64, _P],
     "emer_gen_rays": [_P, _P, _P, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P, c_int64, _P],
+    "emer_topk_ratio": [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P],
+    "emer_pixel_batch": [POINTER(EmerPixelBatchIn), POINTER(EmerPixelBatchOut), _P],
     "emer_adam_step": [_P, _P, c_int, c_int64, _P, c_float, c_float, c_float, c_float, c_int, _P],
     "emer_composite_fwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, _P],
     "emer_composite_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, _P],

@@ -3,12 +3,10 @@
 // Replaces datasets/base/pixel_source.py:39-76 (get_rays) together with the per-ray gathers in front of it
 // (:716-719: c2w = cam_to_worlds[img_idx], intrinsics = intrinsics[img_idx]) and the pixel-coordinate / timestamp
 // assembly of get_train_rays (:699, :711-712): one launch instead of ~15 small torch kernels and two [R,4,4] / [R,3,3]
-// gathered copies.  Arithmetic in the reference's order (-fmad=false: every product and sum rounds separately):
-//     cam = ((x - cx + 0.5) / fx, (y - cy + 0.5) / fy, 1)
-//     dir_i = cam_0 R[i][0] + cam_1 R[i][1] + cam_2 R[i][2];  norm = sqrt(sum dir_i^2);  viewdir = dir / (norm + 1e-8)
-//     origin = c2w[:3, 3]
+// gathered copies.  The per-ray arithmetic is pixel_ray (rays.cuh), shared with the training-batch kernel of
+// raybatch.cu.
 // HBM-bound, 9 floats out per ray: trivial next to the render, it exists to keep the batch on the device.
-#include "common.cuh"
+#include "rays.cuh"
 
 namespace emer {
 
@@ -24,22 +22,12 @@ __global__ void gen_rays_kernel(const int64_t* __restrict__ img_idx, const float
     const float* C = c2w + m * 16;
     const float* K = intr + m * 9;
     const float px = __ldg(x + i), py = __ldg(y + i);
-    const float cam[3] = {(px - __ldg(K + 2) + 0.5f) / __ldg(K + 0), (py - __ldg(K + 5) + 0.5f) / __ldg(K + 4), 1.0f};
-    float d[3], sq = 0.0f;
+    float o[3], v[3], nrm;
+    pixel_ray(C, K, px, py, o, v, nrm);
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
-        float s = cam[0] * __ldg(C + r * 4 + 0);
-        s = s + cam[1] * __ldg(C + r * 4 + 1);
-        s = s + cam[2] * __ldg(C + r * 4 + 2);
-        d[r] = s;
-        sq = sq + s * s;
-    }
-    const float nrm = sqrtf(sq);
-    const float inv = nrm + 1e-8f;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-        origins[i * 3 + r] = __ldg(C + r * 4 + 3);
-        viewdirs[i * 3 + r] = d[r] / inv;
+        origins[i * 3 + r] = o[r];
+        viewdirs[i * 3 + r] = v[r];
     }
     if (norms) norms[i] = nrm;
     if (pixel_coords) {

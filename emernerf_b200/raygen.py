@@ -6,6 +6,10 @@ the batch -- origins, unit view directions, direction norms, pixel coordinates (
 the image index -- in ONE launch (``emer_gen_rays``, csrc/raygen.cu) straight from the per-image camera tables, without
 the gathered [R, 4, 4] / [R, 3, 3] copies.  A training batch then needs 3 integers per ray from the host instead of
 15 floats.
+
+``PixelRaySampler`` and ``LidarRaySampler`` replace the sources' ``get_train_rays`` whole: the reference's random
+draws, made on the device's generator in the reference's order, and the batch assembled from them without a host sync
+(``emer_topk_ratio`` and ``emer_pixel_batch``, csrc/raybatch.cu; INTEGRATION.md section 11).
 """
 from __future__ import annotations
 
@@ -62,3 +66,222 @@ def train_rays(img_idx: Tensor, y: Tensor, x: Tensor, cam_to_worlds: Tensor, int
     if times is not None:
         out["normed_timestamps"] = times
     return out
+
+
+# ----------------------------------------------------------------------------- training batches
+RAYBATCH_WORKSPACE_BYTES = 141376    # EMER_RAYBATCH_WORKSPACE_BYTES
+TOPK_MAX_K = 16384                   # EMER_TOPK_MAX_K
+PIXEL_BATCH_MAX_FEATURES = 256       # EMER_PIXEL_BATCH_MAX_FEATURES
+_MAX_CATEGORIES = 1 << 24            # torch.multinomial's limit on the number of weights
+_WS: Dict[object, Tensor] = {}
+
+
+def _workspace(dev: torch.device) -> Tensor:
+    return _ops._workspace(_WS, dev, RAYBATCH_WORKSPACE_BYTES, "PixelRaySampler")
+
+
+def _dense(t: Optional[Tensor], name: str, dtype=torch.float32) -> Optional[Tensor]:
+    if t is None:
+        return None
+    if t.dtype != dtype or not t.is_contiguous():
+        raise TypeError(f"PixelRaySampler: source.{name} must be a contiguous {dtype} tensor, got {t.dtype}"
+                        f"{'' if t.is_contiguous() else ' (not contiguous)'}")
+    return t
+
+
+def _candidate_key(candidate_indices):
+    """What identifies a candidate set without device work: a list's contents, a tensor's identity and version."""
+    if candidate_indices is None:
+        return ("all",)
+    if isinstance(candidate_indices, Tensor):
+        return ("tensor", id(candidate_indices), candidate_indices._version)
+    return ("list", tuple(int(i) for i in candidate_indices))
+
+
+class _Candidates:
+    """The device copy of the candidate image indices, rebuilt only when ``_candidate_key`` changes.  None means
+    every image, as in the reference."""
+
+    def __init__(self):
+        self.key, self.tensor, self._held = None, None, None
+
+    def get(self, candidate_indices, n_images: int, dev: torch.device) -> Tuple[Tensor, tuple]:
+        key = _candidate_key(candidate_indices) + (n_images,)
+        if key == self.key:
+            return self.tensor, key
+        if key[0] == "all":
+            t = torch.arange(n_images, device=dev)
+        elif key[0] == "list":
+            if key[1] and not (min(key[1]) >= 0 and max(key[1]) < n_images):
+                raise IndexError(f"candidate indices out of range for {n_images} images")
+            t = torch.tensor(key[1], dtype=torch.int64).to(dev)
+        else:
+            t = candidate_indices
+            if t.device != dev or t.dim() != 1:
+                raise ValueError(f"candidate indices must be a 1-D tensor on {dev}")
+            t = t.to(torch.int64)
+            if t.numel() and not bool(((t >= 0) & (t < n_images)).all()):     # one sync per candidate tensor
+                raise IndexError(f"candidate indices out of range for {n_images} images")
+        # a tensor's key holds its id: keep the tensor alive, so the id cannot be reused by another one
+        self.key, self.tensor, self._held = key, t, candidate_indices
+        return t, key
+
+
+class PixelRaySampler:
+    """``ScenePixelSource.get_train_rays`` (datasets/base/pixel_source.py:666-731) on the device, bound to a source:
+    ``source.get_train_rays = PixelRaySampler(source).get_train_rays``.
+
+    It makes the reference's random draws on the same generator, in the same order and with the same shapes:
+    ``randint`` for the uniform rays' image, column and row, then, when the error map is live
+    (``buffer_ratio > 0 and pixel_error_buffered``), the ``Exp(1)`` draw of ``torch.multinomial`` over the candidate
+    images' weights and ``randint`` for the importance rays' row and column offsets.  So the batch is the reference's:
+    the same pixels, the same gathered values, the same keys, uniform rays first.  The one permitted difference is the
+    order of equal top-k keys, which the kernel breaks by ascending index.  Selection and batch assembly are
+    ``emer_topk_ratio`` and ``emer_pixel_batch`` (csrc/raybatch.cu).
+
+    No host sync in steady state: the error map is validated as torch.multinomial validates it (finite, non-negative,
+    positive sum over the candidate images) once per map state -- a different tensor, a moved ``_version`` or another
+    candidate set -- with one sync, and a candidate list is copied to the device once per distinct list.  Every table
+    of the source must live on one CUDA device (the reference's ``to()`` puts them there).
+    """
+
+    def __init__(self, source):
+        self.source = source
+        self._cand = _Candidates()
+        self._valid = None                   # (error maps, their _version, candidate key) last validated
+
+    def _validate(self, maps: Tensor, cand: Tensor, cand_key) -> None:
+        v = self._valid
+        if v is not None and v[0] is maps and v[1] == maps._version and v[2] == cand_key:
+            return
+        if maps.is_cuda and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("PixelRaySampler: the error map changed since the last call; run one call outside "
+                               "graph capture first, so it is validated before capture")
+        w = maps[cand]
+        finite_nonneg, zero_sum = torch.stack([(w.max() < float("inf")) & (w.min() >= 0), w.sum() == 0]).tolist()
+        if not finite_nonneg:
+            raise RuntimeError("probability tensor contains either `inf`, `nan` or element < 0")
+        if zero_sum:
+            raise RuntimeError("invalid multinomial distribution (sum of probabilities <= 0)")
+        self._valid = (maps, maps._version, cand_key)
+
+    def get_train_rays(self, num_rays: int, candidate_indices=None) -> Dict[str, Tensor]:
+        s = self.source
+        H, W = int(s.HEIGHT), int(s.WIDTH)
+        c2w, intr = _dense(s.cam_to_worlds, "cam_to_worlds"), _dense(s.intrinsics, "intrinsics")
+        images = _dense(s.images, "images")
+        sky, dyn = _dense(s.sky_masks, "sky_masks"), _dense(s.dynamic_masks, "dynamic_masks")
+        feats = _dense(s.features, "features")
+        times = _dense(s.normalized_timestamps, "normalized_timestamps")
+        cam_ids = _dense(s.cam_ids, "cam_ids", torch.int64)
+        if cam_ids is None:
+            raise ValueError("PixelRaySampler: the batch's cam_idx needs source.cam_ids")
+        n_images = len(images) if images is not None else len(c2w)
+        dev = c2w.device
+        _ops._need_cuda(c2w, intr, images, sky, dyn, feats, times, cam_ids)
+        cand, cand_key = self._cand.get(candidate_indices, n_images, dev)
+
+        importance = s.buffer_ratio > 0 and s.pixel_error_buffered
+        n_i = int(num_rays * s.buffer_ratio) if importance else 0
+        n_u = num_rays - n_i
+        # the reference's draws, in its order (sample_uniform_rays, then sample_important_rays)
+        u_pick = torch.randint(0, len(cand), size=(n_u,), device=dev)
+        u_x = torch.randint(0, W, size=(n_u,), device=dev)
+        u_y = torch.randint(0, H, size=(n_u,), device=dev)
+        sel = i_dy = i_dx = maps = None
+        map_h = map_w = ds = 0
+        if importance:
+            maps = _dense(s.pixel_error_maps, "pixel_error_maps")
+            _ops._need_cuda(maps)
+            _, map_h, map_w = maps.shape
+            ds = int(s.buffer_downscale)
+            m = len(cand) * map_h * map_w
+            # torch.multinomial's argument checks, in its order and with its messages
+            if n_i <= 0:
+                raise RuntimeError("cannot sample n_sample <= 0 samples")
+            if n_i > m:
+                raise RuntimeError("cannot sample n_sample > prob_dist.size(-1) samples without replacement")
+            if m > _MAX_CATEGORIES:
+                raise RuntimeError("number of categories cannot exceed 2^24")
+            if n_i > TOPK_MAX_K:
+                raise ValueError(f"PixelRaySampler: {n_i} importance rays; the selection kernel takes at most "
+                                 f"{TOPK_MAX_K}")
+            self._validate(maps, cand, cand_key)
+            q = torch.empty(m, dtype=torch.float32, device=dev).exponential_(1)
+            sel = torch.empty(n_i, dtype=torch.int64, device=dev)
+            p = _ops._ptr
+            _lib.call("emer_topk_ratio", p(maps), map_h * map_w, p(cand), len(cand), p(q), n_i, p(sel),
+                      p(_workspace(dev)), _ops._stream())
+            i_dy = torch.randint(0, ds, (n_i,), device=dev)
+            i_dx = torch.randint(0, ds, (n_i,), device=dev)
+        return self._assemble(n_u, n_i, cand, u_pick, u_x, u_y, sel, i_dy, i_dx, map_h, map_w, ds, H, W, images, sky,
+                              dyn, feats, times, cam_ids, c2w, intr)
+
+    def _assemble(self, n_u, n_i, cand, u_pick, u_x, u_y, sel, i_dy, i_dx, map_h, map_w, ds, H, W, images, sky, dyn,
+                  feats, times, cam_ids, c2w, intr) -> Dict[str, Tensor]:
+        n, dev = n_u + n_i, c2w.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        out = {"origins": torch.empty((n, 3), **f32), "viewdirs": torch.empty((n, 3), **f32),
+               "direction_norms": torch.empty((n, 1), **f32), "pixel_coords": torch.empty((n, 2), **f32)}
+        if times is not None:
+            out["normed_timestamps"] = torch.empty(n, **f32)
+        out["img_idx"] = torch.empty(n, dtype=torch.int64, device=dev)
+        out["cam_idx"] = torch.empty(n, dtype=torch.int64, device=dev)
+        if images is not None:
+            out["pixels"] = torch.empty((n, 3), **f32)
+        if sky is not None:
+            out["sky_masks"] = torch.empty(n, **f32)
+        if dyn is not None:
+            out["dynamic_masks"] = torch.empty(n, **f32)
+        fh = fw = fc = 0
+        fsy = fsx = 0.0
+        if feats is not None:
+            _, fh, fw, fc = feats.shape
+            if fc > PIXEL_BATCH_MAX_FEATURES:
+                raise ValueError(f"PixelRaySampler: {fc} feature channels; at most {PIXEL_BATCH_MAX_FEATURES}")
+            scale = self.source.featmap_downscale_factor
+            fsy, fsx = (scale, scale) if isinstance(scale, (int, float)) else scale
+            out["features"] = torch.empty((n, fc), **f32)
+        p = _ops._ptr
+        src = dict(cand=cand, u_pick=u_pick, u_x=u_x, u_y=u_y, i_sel=sel, i_dy=i_dy, i_dx=i_dx, images=images,
+                   sky_masks=sky, dynamic_masks=dyn, features=feats, timestamps=times, cam_ids=cam_ids, c2w=c2w,
+                   intrinsics=intr)
+        args_in = _lib.EmerPixelBatchIn(
+            *(p(src[k]) for k in _lib.PIXEL_BATCH_IN_PTRS), n_u, n_i, H, W, map_h, map_w, ds, fh, fw, fc,
+            float(fsy), float(fsx))
+        names = dict(pixels="pixels", sky_masks="sky_masks", dynamic_masks="dynamic_masks", features="features",
+                     timestamps="normed_timestamps", origins="origins", viewdirs="viewdirs", norms="direction_norms",
+                     pixel_coords="pixel_coords", img_idx="img_idx", cam_idx="cam_idx")
+        args_out = _lib.EmerPixelBatchOut(*(p(out.get(names[k])) for k in _lib.PIXEL_BATCH_OUT_PTRS))
+        _lib.call("emer_pixel_batch", ctypes.byref(args_in), ctypes.byref(args_out), _ops._stream())
+        return out
+
+
+class LidarRaySampler:
+    """``SceneLidarSource.get_train_rays`` (datasets/base/lidar_source.py:223-308) without its per-step
+    ``torch.tensor`` and ``torch.equal``: the points of the candidate scans are gathered once per candidate set (a
+    host compare of the list; a tensor by identity and version), then each step is the reference's one ``randint`` and
+    four gathers.  ``torch.isin`` gives the reference's mask, in point order.  ``candidate_indices=None`` samples every
+    point (the reference then indexes whatever it cached last)."""
+
+    def __init__(self, source):
+        self.source = source
+        self._key, self._cached, self._held = None, None, None
+
+    def get_train_rays(self, num_rays: int, candidate_indices=None) -> Dict[str, Tensor]:
+        s = self.source
+        key = _candidate_key(candidate_indices)
+        if key != self._key:
+            arrays = (s.origins, s.directions, s.ranges, s.normalized_timestamps)
+            if candidate_indices is None:
+                self._cached = arrays
+            else:
+                ts = s.timesteps
+                cand = candidate_indices if key[0] == "tensor" else torch.tensor(key[1], dtype=ts.dtype)
+                mask = torch.isin(ts, cand.to(ts.device))
+                self._cached = tuple(a[mask] for a in arrays)
+            self._key, self._held = key, candidate_indices
+        origins, directions, ranges, times = self._cached
+        idx = torch.randint(0, len(origins), size=(num_rays,), device=s.device)
+        return {"lidar_origins": origins[idx], "lidar_viewdirs": directions[idx], "lidar_ranges": ranges[idx],
+                "lidar_normed_timestamps": times[idx]}

@@ -363,6 +363,68 @@ int emer_gen_rays(const int64_t* img_idx, const float* x, const float* y, const 
                   int per_ray_mats, const float* timestamps, int height, int width, float* origins, float* viewdirs,
                   float* norms, float* pixel_coords, float* out_times, int64_t n, void* stream);
 
+/* ---- training batches of pixel rays (replaces ScenePixelSource.get_train_rays with its samplers,
+ *      datasets/base/pixel_source.py:564-731) ------------------------------------------------------------------ */
+/* workspace: at least EMER_RAYBATCH_WORKSPACE_BYTES of device memory, zeroed once by its owner and left zeroed by
+ * every call (as the loss workspace below), so it is reused by every call and graph replay on one stream. */
+#define EMER_TOPK_MAX_K 16384
+#define EMER_RAYBATCH_WORKSPACE_BYTES 141376
+/* The selection of torch.multinomial(p[cand].reshape(-1), k, replacement=False) = topk(p[cand] / q, k) for a caller-
+ * drawn q ~ Exp(1): out_idx (int64 [k]) gets the j in [0, M = n_cand * plane) of the k largest
+ * p[cand[j / plane] * plane + j % plane] / q[j] (IEEE division), by descending key, then ascending j.  p: the error
+ * maps [N, plane] (fp32, dense), cand: int64 [n_cand] image indices, q: fp32 [M].  The keys must be finite or +inf and
+ * non-negative (the caller validates p as torch.multinomial does).  1 <= k <= min(EMER_TOPK_MAX_K, M), M < 2^31.
+ * Five launches: three radix-select passes and a collection over the keys, and a one-CTA sort of the k survivors. */
+int emer_topk_ratio(const float* p, int64_t plane, const int64_t* cand, int64_t n_cand, const float* q, int64_t k,
+                    int64_t* out_idx, void* workspace, void* stream);
+
+#define EMER_PIXEL_BATCH_MAX_FEATURES 256
+/* Inputs of a training batch: n_uniform rays from the uniform draws, then n_importance rays from the selected indices.
+ * Images are [n_images, height, width] (rgb with 3 channels), features [n_images, feat_h, feat_w, feat_c]; every
+ * table is dense and on the device; images, masks, features, timestamps and cam_ids may be NULL. */
+typedef struct EmerPixelBatchIn {
+    const int64_t* cand;                      /* [n_cand] image indices the draws refer to                           */
+    const int64_t* u_pick;                    /* [n_uniform] positions in cand                                      */
+    const int64_t* u_x;                       /* [n_uniform] pixel columns                                          */
+    const int64_t* u_y;                       /* [n_uniform] pixel rows                                             */
+    const int64_t* i_sel;                     /* [n_importance] j of emer_topk_ratio over the maps [cand, map_h, map_w] */
+    const int64_t* i_dy;                      /* [n_importance] row offsets in [0, map_downscale)                   */
+    const int64_t* i_dx;                      /* [n_importance] column offsets                                      */
+    const float* images;                      /* [N, H, W, 3]                                                       */
+    const float* sky_masks;                   /* [N, H, W]                                                          */
+    const float* dynamic_masks;               /* [N, H, W]                                                          */
+    const float* features;                    /* [N, feat_h, feat_w, feat_c]                                        */
+    const float* timestamps;                  /* [N]                                                                */
+    const int64_t* cam_ids;                   /* [N]                                                                */
+    const float* c2w;                         /* [N, 4, 4]                                                          */
+    const float* intrinsics;                  /* [N, 3, 3]                                                          */
+    int64_t n_uniform, n_importance;
+    int32_t height, width;
+    int32_t map_h, map_w, map_downscale;
+    int32_t feat_h, feat_w, feat_c;
+    float feat_scale_y, feat_scale_x;         /* feature row = (int)((float)y * feat_scale_y), likewise the column  */
+} EmerPixelBatchIn;
+
+/* Outputs, [R = n_uniform + n_importance] rows; an output whose input is NULL must be NULL. */
+typedef struct EmerPixelBatchOut {
+    int64_t* img_idx;                         /* [R]                                                                */
+    int64_t* cam_idx;                         /* [R] cam_ids[img]                                                   */
+    float* pixels;                            /* [R, 3]                                                             */
+    float* sky_masks;                         /* [R]                                                                */
+    float* dynamic_masks;                     /* [R]                                                                */
+    float* features;                          /* [R, feat_c]                                                        */
+    float* timestamps;                        /* [R] timestamps[img]                                                */
+    float* origins;                           /* [R, 3]                                                             */
+    float* viewdirs;                          /* [R, 3]                                                             */
+    float* norms;                             /* [R, 1]                                                             */
+    float* pixel_coords;                      /* [R, 2] (y * (1/height), x * (1/width)), as torch computes y / H on CUDA */
+} EmerPixelBatchOut;
+
+/* One launch: for uniform ray i, img = cand[u_pick[i]], (y, x) = (u_y[i], u_x[i]); for importance ray t,
+ * (c, row, col) = idx_to_3d(i_sel[t]), img = cand[c], y = clamp(row * map_downscale + i_dy[t], 0, height - 1), x
+ * likewise; then the gathers and the ray of emer_gen_rays at (x, y) with img's camera. */
+int emer_pixel_batch(const EmerPixelBatchIn* in, const EmerPixelBatchOut* out, void* stream);
+
 /* ---- optimizer (replaces torch.optim.Adam's step + optimizer.zero_grad() + tiny-cuda-nn's gradient memset,
  *      builders.py:50-61,114-120; train_emernerf.py:742-745,823-826) --------------------------------------------- */
 /* One parameter block: n fp32 values of a parameter, its gradient and Adam moments (16-byte aligned, device). */
