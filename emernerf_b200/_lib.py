@@ -56,6 +56,24 @@ class EmerPixelBatchIn(ctypes.Structure):
 class EmerPixelBatchOut(ctypes.Structure):
     _fields_ = [(k, _P) for k in PIXEL_BATCH_OUT_PTRS]
 
+
+# host structs of emer_image_rays (include/emer_b200.h): field names and order as there
+IMAGE_RAYS_IN_PTRS = ("sky_masks", "dynamic_masks", "features", "timestamps", "cam_ids", "c2w", "intrinsics")
+IMAGE_RAYS_OUT_PTRS = ("origins", "viewdirs", "norms", "pixel_coords", "timestamps", "img_idx", "cam_idx", "sky_masks",
+                       "dynamic_masks", "features")
+
+
+class EmerImageRaysIn(ctypes.Structure):
+    _fields_ = [(k, _P) for k in IMAGE_RAYS_IN_PTRS] + [
+        ("first_image", c_int64), ("n_images", c_int64), ("height", c_int32), ("width", c_int32), ("h", c_int32),
+        ("w", c_int32), ("downscale", c_float), ("mask_scale_y", c_float), ("mask_scale_x", c_float),
+        ("feat_h", c_int32), ("feat_w", c_int32), ("feat_c", c_int32), ("feat_scale_y", c_float),
+        ("feat_scale_x", c_float)]
+
+
+class EmerImageRaysOut(ctypes.Structure):
+    _fields_ = [(k, _P) for k in IMAGE_RAYS_OUT_PTRS]
+
 # number of kernels this library launched through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = 0
 
@@ -94,6 +112,9 @@ _SIGNATURES = {
     "emer_gen_rays": [_P, _P, _P, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P, c_int64, _P],
     "emer_topk_ratio": [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P],
     "emer_pixel_batch": [POINTER(EmerPixelBatchIn), POINTER(EmerPixelBatchOut), _P],
+    "emer_image_rays": [POINTER(EmerImageRaysIn), POINTER(EmerImageRaysOut), _P],
+    "emer_error_map": [_P, _P, _P, c_int64, _P, _P, _P],
+    "emer_error_map_normalize": [_P, c_int64, _P, _P],
     "emer_adam_step": [_P, _P, c_int, c_int64, _P, c_float, c_float, c_float, c_float, c_int, _P],
     "emer_composite_fwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, _P],
     "emer_composite_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, _P],

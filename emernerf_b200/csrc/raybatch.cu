@@ -240,27 +240,18 @@ __global__ void __launch_bounds__(BATCH_THREADS) pixel_batch_kernel(const EmerPi
             o.viewdirs[i * 3 + r] = dir[r];
         }
         o.norms[i] = nrm;
-        // torch on CUDA divides a tensor by a host scalar as a * (1 / b) (div_true_kernel_cuda), so y / HEIGHT here is
-        // the product with the rounded reciprocal, not emer_gen_rays' quotient
-        o.pixel_coords[i * 2 + 0] = fy * __frcp_rn((float)a.height);
-        o.pixel_coords[i * 2 + 1] = fx * __frcp_rn((float)a.width);
+        o.pixel_coords[i * 2 + 0] = pixel_coord(fy, a.height);
+        o.pixel_coords[i * 2 + 1] = pixel_coord(fx, a.width);
         if (o.features) {
-            // (y * downscale).long(): an fp32 product truncated toward zero (pixel_source.py:464-465); clamped so a
-            // scale that rounds up cannot read past the map (torch would raise an index error there)
-            const int64_t fr = min((int64_t)(fy * a.feat_scale_y), (int64_t)a.feat_h - 1);
-            const int64_t fc = min((int64_t)(fx * a.feat_scale_x), (int64_t)a.feat_w - 1);
+            const int64_t fr = feature_cell(fy, a.feat_scale_y, a.feat_h);
+            const int64_t fc = feature_cell(fx, a.feat_scale_x, a.feat_w);
             feat_row[threadIdx.x] = ((img * a.feat_h + fr) * a.feat_w + fc) * a.feat_c;
         }
     }
     if (!o.features) return;
     __syncthreads();
-    // the feature rows of the CTA's rays, copied cooperatively: consecutive threads write consecutive floats
-    const int nr = (int)min((int64_t)BATCH_THREADS, n - i0);
-    const int c = a.feat_c;
-    for (int e = threadIdx.x; e < nr * c; e += BATCH_THREADS) {
-        const int r = e / c;
-        o.features[(i0 + r) * c + (e - r * c)] = __ldg(a.features + feat_row[r] + (e - r * c));
-    }
+    copy_feature_rows(a.features, feat_row, (int)min((int64_t)BATCH_THREADS, n - i0), a.feat_c,
+                      o.features + i0 * a.feat_c, BATCH_THREADS);
 }
 
 }  // namespace emer

@@ -9,13 +9,17 @@ the gathered [R, 4, 4] / [R, 3, 3] copies.  A training batch then needs 3 intege
 
 ``PixelRaySampler`` and ``LidarRaySampler`` replace the sources' ``get_train_rays`` whole: the reference's random
 draws, made on the device's generator in the reference's order, and the batch assembled from them without a host sync
-(``emer_topk_ratio`` and ``emer_pixel_batch``, csrc/raybatch.cu; INTEGRATION.md section 11).
+(``emer_topk_ratio`` and ``emer_pixel_batch``, csrc/raybatch.cu; INTEGRATION.md section 11).  ``PixelRaySampler`` also
+replaces ``get_render_rays`` and ``update_pixel_error_maps``, and with ``refresh_pixel_error_maps`` the whole error-map
+refresh of the training loop (``emer_image_rays``, ``emer_error_map`` and ``emer_error_map_normalize``,
+csrc/errormap.cu; INTEGRATION.md section 12).
 """
 from __future__ import annotations
 
 import ctypes
 from typing import Dict, Optional, Tuple
 
+import numpy as np
 import torch
 from torch import Tensor
 
@@ -78,6 +82,16 @@ _WS: Dict[object, Tensor] = {}
 
 def _workspace(dev: torch.device) -> Tensor:
     return _ops._workspace(_WS, dev, RAYBATCH_WORKSPACE_BYTES, "PixelRaySampler")
+
+
+ERRORMAP_WORKSPACE_BYTES = 16        # EMER_ERRORMAP_WORKSPACE_BYTES
+_MAP_WS: Dict[object, Tensor] = {}
+# get_render_rays' entries with a trailing dimension ([h, w, k]); the others are [h, w]
+_TRAILING = ("origins", "viewdirs", "direction_norm", "pixel_coords", "pixels", "features")
+
+
+def _map_workspace(dev: torch.device) -> Tensor:
+    return _ops._workspace(_MAP_WS, dev, ERRORMAP_WORKSPACE_BYTES, "PixelRaySampler error map")
 
 
 def _dense(t: Optional[Tensor], name: str, dtype=torch.float32) -> Optional[Tensor]:
@@ -149,6 +163,7 @@ class PixelRaySampler:
         self.source = source
         self._cand = _Candidates()
         self._valid = None                   # (error maps, their _version, candidate key) last validated
+        self._resized = None                 # (images, their _version, d, the images resized by d)
 
     def _validate(self, maps: Tensor, cand: Tensor, cand_key) -> None:
         v = self._valid
@@ -255,6 +270,158 @@ class PixelRaySampler:
         args_out = _lib.EmerPixelBatchOut(*(p(out.get(names[k])) for k in _lib.PIXEL_BATCH_OUT_PTRS))
         _lib.call("emer_pixel_batch", ctypes.byref(args_in), ctypes.byref(args_out), _ops._stream())
         return out
+
+    # ------------------------------------------------------------------------- render rays and the error map
+    def _images_at(self, images: Tensor, d: float) -> Tensor:
+        """Every image resized by d, [N, h, w, 3], as get_render_rays resizes one: torch's bicubic antialiased
+        ``interpolate`` with ``scale_factor=d``, run once over all images (each image is its own batch entry) and kept
+        while the images tensor and its ``_version`` stay the same."""
+        if d == 1.0:
+            return images
+        r = self._resized
+        if r is not None and r[0] is images and r[1] == images._version and r[2] == d:
+            return r[3]
+        out = torch.nn.functional.interpolate(images.permute(0, 3, 1, 2), scale_factor=d, mode="bicubic",
+                                              antialias=True).permute(0, 2, 3, 1).contiguous()
+        self._resized = (images, images._version, d, out)
+        return out
+
+    def _image_rays(self, first: int, count: int, d: float) -> Tuple[Dict[str, Tensor], int, int]:
+        """get_render_rays' entries for the images [first, first + count) at downscale d, flat ([count * h * w, ...]),
+        in the reference's key order; and (h, w)."""
+        s = self.source
+        H, W = int(s.HEIGHT), int(s.WIDTH)
+        c2w, intr = _dense(s.cam_to_worlds, "cam_to_worlds"), _dense(s.intrinsics, "intrinsics")
+        images = _dense(s.images, "images")
+        sky, dyn = _dense(s.sky_masks, "sky_masks"), _dense(s.dynamic_masks, "dynamic_masks")
+        feats = _dense(s.features, "features")
+        times = _dense(s.normalized_timestamps, "normalized_timestamps")
+        cam_ids = _dense(s.cam_ids, "cam_ids", torch.int64)
+        if images is None or cam_ids is None:
+            raise ValueError("PixelRaySampler: render rays need source.images and source.cam_ids")
+        _ops._need_cuda(c2w, intr, images, sky, dyn, feats, times, cam_ids)
+        if first < 0 or first + count > len(images):
+            raise IndexError(f"images [{first}, {first + count}) out of range for {len(images)} images")
+        resized = self._images_at(images, d)
+        h, w = resized.shape[1:3]
+        n, dev = count * h * w, c2w.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        out = {"origins": torch.empty((n, 3), **f32), "viewdirs": torch.empty((n, 3), **f32),
+               "direction_norm": torch.empty((n, 1), **f32), "pixel_coords": torch.empty((n, 2), **f32)}
+        if times is not None:
+            out["normed_timestamps"] = torch.empty(n, **f32)
+        out["img_idx"] = torch.empty(n, dtype=torch.int64, device=dev)
+        out["cam_idx"] = torch.empty(n, dtype=torch.int64, device=dev)
+        out["pixels"] = resized[first:first + count].reshape(n, 3)
+        if sky is not None:
+            out["sky_masks"] = torch.empty(n, **f32)
+        if dyn is not None:
+            out["dynamic_masks"] = torch.empty(n, **f32)
+        fh = fw = fc = 0
+        fsy = fsx = 0.0
+        if feats is not None:
+            _, fh, fw, fc = feats.shape
+            if fc > PIXEL_BATCH_MAX_FEATURES:
+                raise ValueError(f"PixelRaySampler: {fc} feature channels; at most {PIXEL_BATCH_MAX_FEATURES}")
+            # get_features(downscale=(featmap_downscale_factor[0] / d, featmap_downscale_factor[1] / d))
+            fsy, fsx = (v / d for v in self.source.featmap_downscale_factor)
+            out["features"] = torch.empty((n, fc), **f32)
+        p = _ops._ptr
+        src = dict(sky_masks=sky, dynamic_masks=dyn, features=feats, timestamps=times, cam_ids=cam_ids, c2w=c2w,
+                   intrinsics=intr)
+        # interpolate(scale_factor=d, mode="nearest") reads source row floor(y * (float)(1 / d))
+        args_in = _lib.EmerImageRaysIn(*(p(src[k]) for k in _lib.IMAGE_RAYS_IN_PTRS), first, count, H, W, h, w,
+                                       float(d), 1.0 / d, 1.0 / d, fh, fw, fc, float(fsy), float(fsx))
+        names = dict(origins="origins", viewdirs="viewdirs", norms="direction_norm", pixel_coords="pixel_coords",
+                     timestamps="normed_timestamps", img_idx="img_idx", cam_idx="cam_idx", sky_masks="sky_masks",
+                     dynamic_masks="dynamic_masks", features="features")
+        args_out = _lib.EmerImageRaysOut(*(p(out.get(names[k])) for k in _lib.IMAGE_RAYS_OUT_PTRS))
+        _lib.call("emer_image_rays", ctypes.byref(args_in), ctypes.byref(args_out), _ops._stream())
+        return out, h, w
+
+    @torch.no_grad()
+    def get_render_rays(self, img_idx: int) -> Dict[str, Tensor]:
+        """``ScenePixelSource.get_render_rays`` (pixel_source.py:733-846) at ``source.downscale_factor``: the
+        reference's keys, in its order, with its ``[h, w, ...]`` shapes and dtypes, every entry on the device.  The
+        image is resized by torch's own bicubic ``interpolate``; the rest is one ``emer_image_rays`` launch."""
+        return self._render_rays_at(int(img_idx), float(self.source.downscale_factor))
+
+    def _render_rays_at(self, img_idx: int, d: float) -> Dict[str, Tensor]:
+        out, h, w = self._image_rays(img_idx, 1, d)
+        return {k: v.reshape(h, w, *v.shape[1:]) if k in _TRAILING else v.reshape(h, w) for k, v in out.items()}
+
+    def _fold_error(self, gt: Tensor, rgb: Tensor, opacity: Optional[Tensor], rows: Tensor) -> None:
+        n = rows.numel()
+        if gt.numel() != 3 * n or rgb.numel() != 3 * n or (opacity is not None and opacity.numel() != n):
+            raise ValueError(f"PixelRaySampler: {n} error-map pixels, got gt {tuple(gt.shape)}, rgb "
+                             f"{tuple(rgb.shape)}" + ("" if opacity is None else f", opacity {tuple(opacity.shape)}"))
+        gt, rgb = _ops._f32c(gt), _ops._f32c(rgb)
+        opacity = None if opacity is None else _ops._f32c(opacity)
+        _ops._need_cuda(gt, rgb, opacity, rows)
+        p = _ops._ptr
+        _lib.call("emer_error_map", p(gt), p(rgb), p(opacity), n, p(rows), p(_map_workspace(rows.device)),
+                  _ops._stream())
+
+    def _publish(self, maps: Tensor) -> None:
+        p = _ops._ptr
+        _ops._need_cuda(maps)
+        _lib.call("emer_error_map_normalize", p(maps), maps.numel(), p(_map_workspace(maps.device)), _ops._stream())
+        self.source.pixel_error_maps = maps
+        self.source.pixel_error_buffered = True
+
+    @torch.no_grad()
+    def update_pixel_error_maps(self, render_results) -> None:
+        """``ScenePixelSource.update_pixel_error_maps`` (pixel_source.py:491-517): ``render_results`` holds lists,
+        one entry per image, of numpy arrays (what ``render_pixels`` returns) or of device tensors under "gt_rgbs",
+        "rgbs" and optionally "dynamic_opacities".  The new map is a new tensor, computed and normalised in two
+        launches with the reference's arithmetic; the next ``get_train_rays`` validates it."""
+        s = self.source
+        if s.pixel_error_maps is None:
+            return
+        dev = s.pixel_error_maps.device
+
+        def stacked(items):
+            if isinstance(items[0], np.ndarray):
+                return torch.from_numpy(np.stack(items, axis=0)).to(dev)
+            return torch.stack(list(items)).to(dev)
+
+        gt, rgb = stacked(render_results["gt_rgbs"]), stacked(render_results["rgbs"])
+        assert gt.shape[:-1] == s.pixel_error_maps.shape
+        dyn = render_results.get("dynamic_opacities")
+        opacity = stacked(dyn) if dyn is not None and len(dyn) > 0 else None
+        maps = torch.empty(s.pixel_error_maps.shape, dtype=torch.float32, device=dev)
+        self._fold_error(gt, rgb, opacity, maps)
+        self._publish(maps)
+
+    @torch.no_grad()
+    def refresh_pixel_error_maps(self, model, proposal_estimator, proposal_networks, cfg) -> None:
+        """The error-map refresh of the training loop (train_emernerf.py:889-904 of the reference): every image of
+        the source rendered at ``1 / buffer_downscale`` through ``render_rays``, one call per image, and its error
+        written straight into a new map, which is then normalised and set on the source.  No numpy and no host sync
+        of its own; the source's ``downscale_factor`` is not touched.  The decomposition is asked for only when the
+        field has a dynamic branch, the one case where the reference's map uses it."""
+        from .radiance_fields.render_utils import render_rays
+
+        s = self.source
+        if s.pixel_error_maps is None:
+            return
+        model.eval()
+        if proposal_estimator is not None:
+            proposal_estimator.eval()
+        for p in proposal_networks or ():
+            p.eval()
+        decomposition = getattr(model, "dynamic_xyz_encoder", None) is not None
+        d = 1 / s.buffer_downscale
+        maps = torch.empty(s.pixel_error_maps.shape, dtype=torch.float32, device=s.pixel_error_maps.device)
+        for i in range(len(maps)):
+            data = self._render_rays_at(i, d)
+            assert data["pixels"].shape[:2] == maps.shape[1:]
+            out = render_rays(radiance_field=model, proposal_estimator=proposal_estimator,
+                              proposal_networks=proposal_networks, data_dict=data, cfg=cfg,
+                              return_decomposition=decomposition)
+            self._fold_error(data["pixels"], out["rgb"], out.get("dynamic_opacity") if decomposition else None,
+                             maps[i])
+        self._publish(maps)
 
 
 class LidarRaySampler:

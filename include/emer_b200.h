@@ -425,6 +425,65 @@ typedef struct EmerPixelBatchOut {
  * likewise; then the gathers and the ray of emer_gen_rays at (x, y) with img's camera. */
 int emer_pixel_batch(const EmerPixelBatchIn* in, const EmerPixelBatchOut* out, void* stream);
 
+/* ---- whole-image render rays and the pixel error map (csrc/errormap.cu; replaces ScenePixelSource.get_render_rays,
+ *      datasets/base/pixel_source.py:733-846, without the resize of the image, and update_pixel_error_maps, :491-517,
+ *      with the host copies of radiance_fields/video_utils.py:104-468 that feed it) ---------------------------------- */
+/* Inputs of emer_image_rays: the source's tables at full size [N, height, width], as EmerPixelBatchIn; masks,
+ * features, timestamps and cam_ids may be NULL. */
+typedef struct EmerImageRaysIn {
+    const float* sky_masks;                   /* [N, height, width]                                                 */
+    const float* dynamic_masks;               /* [N, height, width]                                                 */
+    const float* features;                    /* [N, feat_h, feat_w, feat_c]                                        */
+    const float* timestamps;                  /* [N]                                                                */
+    const int64_t* cam_ids;                   /* [N]                                                                */
+    const float* c2w;                         /* [N, 4, 4]                                                          */
+    const float* intrinsics;                  /* [N, 3, 3]                                                          */
+    int64_t first_image, n_images;            /* the images [first_image, first_image + n_images)                   */
+    int32_t height, width;                    /* full size                                                          */
+    int32_t h, w;                             /* rendered size, the resized image's                                 */
+    float downscale;                          /* the source's downscale_factor d, as fp32: K * d                    */
+    float mask_scale_y, mask_scale_x;         /* nearest source row = min(floor(y * mask_scale_y), height - 1);     */
+                                              /* (float)(1.0 / d), torch's scale for interpolate(scale_factor=d)    */
+    int32_t feat_h, feat_w, feat_c;
+    float feat_scale_y, feat_scale_x;         /* feature row = (int)((float)y * feat_scale_y): featmap_downscale / d */
+} EmerImageRaysIn;
+
+/* Outputs, [R = n_images * h * w] rows in (image, y, x) order; an output whose input is NULL must be NULL. */
+typedef struct EmerImageRaysOut {
+    float* origins;                           /* [R, 3]                                                             */
+    float* viewdirs;                          /* [R, 3]                                                             */
+    float* norms;                             /* [R, 1]                                                             */
+    float* pixel_coords;                      /* [R, 2] (y * (1/h), x * (1/w)), as torch computes y / h on CUDA     */
+    float* timestamps;                        /* [R] timestamps[img]                                                */
+    int64_t* img_idx;                         /* [R]                                                                */
+    int64_t* cam_idx;                         /* [R] cam_ids[img]                                                   */
+    float* sky_masks;                         /* [R] the nearest source pixel                                       */
+    float* dynamic_masks;                     /* [R]                                                                */
+    float* features;                          /* [R, feat_c]                                                        */
+} EmerImageRaysOut;
+
+/* One launch: for every pixel (y, x) of the h x w grid of every image, the ray of emer_gen_rays with the intrinsics
+ * scaled by d in fp32, the pixel coordinates, and the gathers of get_render_rays at the nearest-mode source pixel and
+ * at get_features' cell. */
+int emer_image_rays(const EmerImageRaysIn* in, const EmerImageRaysOut* out, void* stream);
+
+/* workspace: at least EMER_ERRORMAP_WORKSPACE_BYTES of device memory, zeroed once by its owner and left zeroed by
+ * emer_error_map_normalize (as the raybatch workspace above).  Between the two calls it holds the running minimum and
+ * maximum of the map. */
+#define EMER_ERRORMAP_WORKSPACE_BYTES 16
+/* For n pixels (one or more whole images): map[i] = mean_c |gt[i, c] - rgb[i, c]| as torch computes it on the CPU
+ * (((e0 + e1) + e2) / 3 in fp32), times 5 (fp32) where opacity[i] > 0.1f when opacity is not NULL.  gt and rgb are
+ * [n, 3], opacity [n], map [n] (the images' rows of the map).  Folds the minimum and maximum into the workspace with
+ * integer atomics on the fp32 bit patterns (the errors are >= 0, or NaN, which orders above them), so the result does
+ * not depend on the order of the CTAs. */
+int emer_error_map(const float* gt, const float* rgb, const float* opacity, int64_t n, float* map, void* workspace,
+                   void* stream);
+/* map[i] = (map[i] - min) / (max - min) over the n entries of the whole map, with the minimum and maximum every
+ * emer_error_map call since the last normalisation folded in: fp32 subtractions and an IEEE division, as torch
+ * computes them on CUDA with 0-d tensor operands.  A NaN error or a constant map gives NaN (0 / 0), as there.  Zeroes
+ * the workspace. */
+int emer_error_map_normalize(float* map, int64_t n, void* workspace, void* stream);
+
 /* ---- optimizer (replaces torch.optim.Adam's step + optimizer.zero_grad() + tiny-cuda-nn's gradient memset,
  *      builders.py:50-61,114-120; train_emernerf.py:742-745,823-826) --------------------------------------------- */
 /* One parameter block: n fp32 values of a parameter, its gradient and Adam moments (16-byte aligned, device). */
