@@ -132,6 +132,7 @@ _SIGNATURES = {
     "emer_image_metrics": [_P, _P, c_int64, c_int64, c_int, _P, _P, c_int64, _P, c_int64, c_int, _P, _P, _P],
     "emer_depth_rmse": [_P, _P, c_int64, _P, _P, _P],
     "emer_scene_flow_metrics": [_P, _P, c_int64, _P, _P, _P],
+    "emer_lidar_flow_accumulate": [_P, c_int64, _P, _P, _P, _P, c_int64, c_float, _P, _P, _P],
     "emer_occ_accumulate": [_P, c_int64, c_int, _P, c_int64, _P, c_int64, c_int, c_float, _P, _P, _P, _P],
     "emer_occ_classify": [_P, c_int64, c_int, _P, c_int64, _P, c_int64, _P, c_int, _P, c_float, _P, _P, _P],
 }
@@ -216,6 +217,8 @@ def tag_of(name: str, args) -> str:
             return f"H{args[2]}_W{args[3]}_C{args[4]}_F{args[10]}"
         if name in ("emer_depth_rmse", "emer_scene_flow_metrics"):
             return f"N{args[2]}"
+        if name == "emer_lidar_flow_accumulate":
+            return f"N{args[6]}" + ("_G" if args[5].value else "")
         if name == "emer_occ_accumulate":
             return f"C{args[2]}_K{args[7]}_N{args[6]}"
         if name == "emer_occ_classify":

@@ -284,6 +284,29 @@ __global__ void __launch_bounds__(MET_THREADS) depth_rmse_kernel(const float* pr
 // torch clamps with the bounds rounded to the tensor's dtype: +-(1 - 1e-7) in fp32
 constexpr double FLOW_DOT_MAX = (double)(float)(1.0 - 1e-7);
 
+// compute_scene_flow_metrics' terms of one point, added into s: s[0] += the end-point error |p - l|, s[1..3] += 1 when
+// the point is strictly accurate, relaxed accurate, an outlier, and when |l| > 0.1, s[4] += the angle and s[5] += 1.
+// The one statement of the formula: scene_flow_kernel and lidar_flow_kernel call it.
+__device__ __forceinline__ void flow_point(double px, double py, double pz, double lx, double ly, double lz,
+                                           double* s) {
+    const double dx = px - lx, dy = py - ly, dz = pz - lz;
+    const double l2 = sqrt(dx * dx + dy * dy + dz * dz);
+    const double ln = sqrt(lx * lx + ly * ly + lz * lz);
+    const double rel = l2 / (ln + 1e-20);
+    s[0] += l2;
+    s[1] += (l2 < 0.05 || rel < 0.05) ? 1.0 : 0.0;
+    s[2] += (l2 < 0.1 || rel < 0.1) ? 1.0 : 0.0;
+    s[3] += (l2 > 0.3 || rel > 0.1) ? 1.0 : 0.0;
+    if (ln > 0.1) {
+        const double pn = sqrt(px * px + py * py + pz * pz);
+        const double dl = ln + 1e-7, dp = pn + 1e-7;         // unit vectors as the reference forms them
+        double dot = (lx / dl) * (px / dp) + (ly / dl) * (py / dp) + (lz / dl) * (pz / dp);
+        dot = dot != dot ? 0.0 : fmin(fmax(dot, -FLOW_DOT_MAX), FLOW_DOT_MAX);
+        s[4] += acos(dot);
+        s[5] += 1.0;
+    }
+}
+
 __global__ void __launch_bounds__(MET_THREADS) scene_flow_kernel(const float* pred, const float* labels, int64_t n,
                                                                double* out, MetricsWorkspace* ws) {
     Partials acc;
@@ -291,22 +314,7 @@ __global__ void __launch_bounds__(MET_THREADS) scene_flow_kernel(const float* pr
     for (int64_t i = (int64_t)blockIdx.x * MET_THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * MET_THREADS) {
         const double px = __ldg(pred + 3 * i), py = __ldg(pred + 3 * i + 1), pz = __ldg(pred + 3 * i + 2);
         const double lx = __ldg(labels + 3 * i), ly = __ldg(labels + 3 * i + 1), lz = __ldg(labels + 3 * i + 2);
-        const double dx = px - lx, dy = py - ly, dz = pz - lz;
-        const double l2 = sqrt(dx * dx + dy * dy + dz * dz);
-        const double ln = sqrt(lx * lx + ly * ly + lz * lz);
-        const double rel = l2 / (ln + 1e-20);
-        acc.s[0] += l2;
-        acc.s[1] += (l2 < 0.05 || rel < 0.05) ? 1.0 : 0.0;
-        acc.s[2] += (l2 < 0.1 || rel < 0.1) ? 1.0 : 0.0;
-        acc.s[3] += (l2 > 0.3 || rel > 0.1) ? 1.0 : 0.0;
-        if (ln > 0.1) {
-            const double pn = sqrt(px * px + py * py + pz * pz);
-            const double dl = ln + 1e-7, dp = pn + 1e-7;         // unit vectors as the reference forms them
-            double dot = (lx / dl) * (px / dp) + (ly / dl) * (py / dp) + (lz / dl) * (pz / dp);
-            dot = dot != dot ? 0.0 : fmin(fmax(dot, -FLOW_DOT_MAX), FLOW_DOT_MAX);
-            acc.s[4] += acos(dot);
-            acc.s[5] += 1.0;
-        }
+        flow_point(px, py, pz, lx, ly, lz, acc.s);
     }
     if (!reduce_across_ctas(acc, ws)) return;
     const double m = (double)n;
@@ -317,6 +325,63 @@ __global__ void __launch_bounds__(MET_THREADS) scene_flow_kernel(const float* pr
     out[4] = acc.s[4] / acc.s[5];                // NaN when no label norm exceeds 0.1
     out[5] = acc.s[5];
     out[6] = m;
+}
+
+// ---------------------------------------------------------------------------------------------- lidar scene flow
+// The NSFP terms of one chunk of a lidar frame, added into the frame's row.  The metrics workspace has 7 sums per CTA;
+// this kernel needs 8, so it lays the same bytes out for at most MET_MAX_CTAS / 2 CTAs (metrics_grid's cap).  The
+// ticket sits at offset 0 in both layouts and is zero between calls.
+constexpr int LF_MAX_CTAS = MET_MAX_CTAS / 2;
+
+struct LidarFlowWorkspace {
+    unsigned int ticket;
+    unsigned int pad[15];
+    double sum[EMER_LIDAR_FLOW_SUMS][LF_MAX_CTAS];
+};
+static_assert(sizeof(LidarFlowWorkspace) <= EMER_METRICS_WORKSPACE_BYTES, "workspace layout exceeds the ABI size");
+static_assert(EMER_LIDAR_FLOW_COUNTED == 6 && EMER_LIDAR_FLOW_VALID == 7, "flow_point fills slots 0..5");
+
+__global__ void __launch_bounds__(MET_THREADS) lidar_flow_kernel(const float* pred, int64_t ld_pred,
+                                                               const float* density, const float* labels,
+                                                               const int64_t* flow_class, const uint8_t* ground,
+                                                               int64_t n, float threshold, double* sums,
+                                                               LidarFlowWorkspace* ws) {
+    __shared__ double sh[MET_WARPS];
+    double s[EMER_LIDAR_FLOW_SUMS];
+#pragma unroll
+    for (int k = 0; k < EMER_LIDAR_FLOW_SUMS; ++k) s[k] = 0.0;
+    for (int64_t i = (int64_t)blockIdx.x * MET_THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * MET_THREADS) {
+        if (__ldg(flow_class + i) == -1) continue;                   // no flow label
+        s[EMER_LIDAR_FLOW_VALID] += 1.0;
+        if (ground && __ldg(ground + i)) continue;
+        s[EMER_LIDAR_FLOW_COUNTED] += 1.0;
+        float px = __ldg(pred + i * ld_pred), py = __ldg(pred + i * ld_pred + 1), pz = __ldg(pred + i * ld_pred + 2);
+        if (__ldg(density + i) < threshold) {                       // pred[density < 0.2] *= 0: NaN stays, -x gives -0
+            px *= 0.0f; py *= 0.0f; pz *= 0.0f;
+        }
+        flow_point(px, py, pz, __ldg(labels + 3 * i), __ldg(labels + 3 * i + 1), __ldg(labels + 3 * i + 2), s);
+    }
+    double t[EMER_LIDAR_FLOW_SUMS];
+#pragma unroll
+    for (int k = 0; k < EMER_LIDAR_FLOW_SUMS; ++k) t[k] = block_sum<MET_WARPS>(s[k], sh);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < EMER_LIDAR_FLOW_SUMS; ++k) ws->sum[k][blockIdx.x] = t[k];
+    }
+    if (!take_last_ticket(&ws->ticket)) return;
+#pragma unroll
+    for (int k = 0; k < EMER_LIDAR_FLOW_SUMS; ++k) s[k] = 0.0;
+    for (int c = threadIdx.x; c < (int)gridDim.x; c += MET_THREADS) {
+#pragma unroll
+        for (int k = 0; k < EMER_LIDAR_FLOW_SUMS; ++k) s[k] += __ldcg(ws->sum[k] + c);
+    }
+#pragma unroll
+    for (int k = 0; k < EMER_LIDAR_FLOW_SUMS; ++k) t[k] = block_sum<MET_WARPS>(s[k], sh);
+    release_ticket(&ws->ticket);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < EMER_LIDAR_FLOW_SUMS; ++k) sums[k] += t[k];
+    }
 }
 
 static int metrics_grid(int64_t work_items, int per_cta, int per_sm) {
@@ -379,4 +444,19 @@ extern "C" int emer_scene_flow_metrics(const float* pred, const float* labels, i
     scene_flow_kernel<<<metrics_grid(n, MET_THREADS, 2), MET_THREADS, 0, (cudaStream_t)stream>>>(
         pred, labels, n, out, (MetricsWorkspace*)workspace);
     return check_launch("emer_scene_flow_metrics");
+}
+
+extern "C" int emer_lidar_flow_accumulate(const float* pred, int64_t ld_pred, const float* dynamic_density,
+                                          const float* labels, const int64_t* flow_class, const uint8_t* ground,
+                                          int64_t n, float threshold, double* sums, void* workspace, void* stream) {
+    EMER_REQUIRE(sums && workspace && (n == 0 || (pred && dynamic_density && labels && flow_class)),
+                 "emer_lidar_flow_accumulate: NULL pointer");
+    EMER_REQUIRE(n >= 0, "emer_lidar_flow_accumulate: negative size");
+    EMER_REQUIRE(ld_pred >= 3, "emer_lidar_flow_accumulate: prediction row stride %lld below 3", (long long)ld_pred);
+    const int grid = metrics_grid(n, MET_THREADS, 2);
+    EMER_REQUIRE(grid <= LF_MAX_CTAS, "emer_lidar_flow_accumulate: %d CTAs exceed the workspace", grid);
+    lidar_flow_kernel<<<grid, MET_THREADS, 0, (cudaStream_t)stream>>>(pred, ld_pred, dynamic_density, labels,
+                                                                      flow_class, ground, n, threshold, sums,
+                                                                      (LidarFlowWorkspace*)workspace);
+    return check_launch("emer_lidar_flow_accumulate");
 }

@@ -32,9 +32,25 @@ Deliberate differences from the reference:
   * Cosine similarities are fp64, and an exact tie goes to the lowest class index (the reference's ``topk`` leaves
     the order of ties unspecified).
   * Neither function switches the model to eval mode; the reference's driver does that before it calls them.
+
+The lidar scene-flow evaluation (``emer_lidar_flow_accumulate``, csrc/metrics.cu) replaces the flow block of the
+reference's driver (train_emernerf.py:237-281) with one call:
+
+    avg_flow_metrics = metrics.eval_lidar_flow(dataset.full_lidar_set, model, remove_ground=True)   # one sync
+
+Per frame it runs ``model.query_flow`` over every point of the frame, in chunks of ``FLOW_CHUNK_POINTS``, and launches
+one kernel per chunk, which applies the flow-class filter, the ground filter and the dynamic-density gate itself.
+Deliberate differences from the reference:
+  * The field runs on every point of the frame, where the reference first compacts the frame by boolean indexing.
+    The field is row-independent, so the counted points get the same flows, up to the layer kernels' choice by row
+    count.
+  * The per-frame statistics are fp64 sums, where the reference's are fp32 means; a point whose error lies within
+    fp32 rounding of a threshold may count differently.
 """
 from __future__ import annotations
 
+import logging
+import weakref
 from typing import Dict, List, Optional, Tuple, Union
 
 import numpy as np
@@ -44,7 +60,8 @@ from torch import Tensor
 from . import _lib, _ops
 
 __all__ = ["compute_psnr", "compute_ssim", "compute_valid_depth_rmse", "compute_scene_flow_metrics", "image_metrics",
-           "summarize", "collect_centroids", "eval_few_shot_occ"]
+           "summarize", "collect_centroids", "eval_few_shot_occ", "eval_lidar_flow"]
+logger = logging.getLogger()
 
 WORKSPACE_BYTES = 81920          # EMER_METRICS_WORKSPACE_BYTES
 MAX_CHANNELS = 4                 # image channels
@@ -62,6 +79,10 @@ OCC_CHUNK_POINTS = 1 << 20       # voxels per field pass: bounds the memory of a
 OCC_DENSITY_THRESHOLD = 0.2      # the reference's filter of the voxels the cameras see
 OCC_FEATURE_DIM = 64             # the reference's width of a centroid when no frame produced a feature
 _OCC_WS: Dict[object, Tensor] = {}
+FLOW_CHUNK_POINTS = 1 << 20      # lidar points per query_flow call: bounds the memory of a frame of any size
+FLOW_DENSITY_THRESHOLD = 0.2     # the reference's gate: flows count only on dynamic points
+FLOW_SUMS = 8                    # EMER_LIDAR_FLOW_SUMS
+FLOW_EVAL_KEYS = ("EPE3D", "acc3d_strict", "acc3d_relax", "angle_error", "outlier")   # the driver's key order
 
 
 def _numpy_device() -> torch.device:
@@ -308,3 +329,97 @@ def eval_few_shot_occ(test_indices, dataset, model, device, centroids_bank: Tens
         "num_measured_points": measured,
         "num_total_points": num_total_points,
     }
+
+
+# ---------------------------------------------------------------------------------------------- lidar scene flow
+_SAMPLERS: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
+
+
+def _lidar_sampler(source):
+    """The LidarRaySampler whose frame table serves ``source``: the one bound as ``source.get_render_rays`` if there
+    is one, else one kept per source (it holds the source by a weak proxy, so the cache does not keep it alive)."""
+    from .raygen import LidarRaySampler
+
+    bound = getattr(getattr(source, "get_render_rays", None), "__self__", None)
+    if isinstance(bound, LidarRaySampler) and bound.source is source:
+        return bound
+    try:
+        sampler = _SAMPLERS.get(source)
+        if sampler is None:
+            sampler = _SAMPLERS[source] = LidarRaySampler(weakref.proxy(source))
+        return sampler
+    except TypeError:                               # not weakly referenceable: a table per call
+        return LidarRaySampler(source)
+
+
+def eval_lidar_flow(lidar_set, model, remove_ground: bool = True) -> Dict[str, np.float64]:
+    """The lidar scene-flow evaluation of the reference's driver (train_emernerf.py:237-281) over
+    ``dataset.full_lidar_set`` (anything with ``datasource`` and ``split_indices``): per frame, the points with a
+    flow label (``lidar_flow_class != -1``), without the ground points when ``remove_ground``, the model's forward
+    flow zeroed where its dynamic density is below 0.2, and the NSFP statistics against ``lidar_flow``; then the mean
+    of each statistic over the frames, as ``np.float64`` under the driver's keys and in its order.
+
+    As there, a frame without a labelled point is skipped (and logged), the check comes before the ground removal, a
+    frame without a label norm above 0.1 gives a NaN angle error, and no frame at all gives NaN.  A frame whose
+    labelled points are all ground gives NaN for every statistic, what the reference's statistics give for an empty
+    frame (the reference's ``query_flow`` itself fails on zero points).  Runs under ``no_grad``; one host sync, at the
+    end, and the frame table's two when the source's timesteps are new."""
+    rows = _lidar_flow_sums(lidar_set, model, remove_ground).cpu().tolist()     # the one host sync
+    per_frame: Dict[str, List[np.float64]] = {k: [] for k in FLOW_EVAL_KEYS}
+    for r in rows:
+        if r[7] == 0:                                   # EMER_LIDAR_FLOW_VALID
+            logger.info("no valid points, skipping...")
+            continue
+        counted = np.float64(r[6])
+        with np.errstate(divide="ignore", invalid="ignore"):
+            got = {"EPE3D": r[0] / counted, "acc3d_strict": r[1] / counted, "acc3d_relax": r[2] / counted,
+                   "angle_error": np.float64(r[4]) / np.float64(r[5]), "outlier": r[3] / counted}
+        for k in FLOW_EVAL_KEYS:
+            per_frame[k].append(got[k])
+    return {k: np.mean(v) for k, v in per_frame.items()}
+
+
+def _lidar_flow_sums(lidar_set, model, remove_ground: bool) -> Tensor:
+    """The fp64 [frames, EMER_LIDAR_FLOW_SUMS] rows of ``eval_lidar_flow``, on the device; no host sync once the frame table
+    exists."""
+    source = getattr(lidar_set, "datasource", None)
+    indices = getattr(lidar_set, "split_indices", None)
+    if source is None or indices is None:
+        raise ValueError("lidar flow evaluation: the set needs `datasource` and `split_indices` (a SplitWrapper)")
+    if getattr(model, "flow_xyz_encoder", None) is None:
+        raise ValueError("lidar flow evaluation: the model has no flow branch")
+    indices = list(indices)
+    dev = source.origins.device
+    sums = torch.zeros(len(indices), FLOW_SUMS, dtype=torch.float64, device=dev)
+    _ops._need_cuda(sums)
+    ws = _ops._workspace(_WS, dev, WORKSPACE_BYTES, "metrics")
+    sampler = _lidar_sampler(source)
+    p = _ops._ptr
+    with torch.no_grad():
+        for f, t in enumerate(indices):
+            d = sampler.get_render_rays(t)
+            if "lidar_flow" not in d:
+                raise ValueError("lidar flow evaluation: the source has no flows, flow_classes and grounds")
+            points = d["lidar_origins"] + d["lidar_ranges"] * d["lidar_viewdirs"]
+            times, labels, classes = d["lidar_normed_timestamps"], d["lidar_flow"], d["lidar_flow_class"]
+            ground = d["lidar_ground"] if remove_ground else None
+            n = points.shape[0]
+            for s in range(0, n, FLOW_CHUNK_POINTS):
+                e = min(s + FLOW_CHUNK_POINTS, n)
+                out = model.query_flow(positions=points[s:e], normed_timestamps=times[s:e])
+                pred, ld = _ops._rows(out["forward_flow"], 3)      # in place in the [n, 6] flow output
+                density = _ops._f32c(out["dynamic_density"].reshape(-1))
+                lab = _ops._f32c(labels[s:e])
+                cls = classes[s:e].to(torch.int64).contiguous()
+                g = None
+                if ground is not None:
+                    g = ground[s:e]
+                    g = (g if g.dtype == torch.bool else g != 0).contiguous().view(torch.uint8)
+                if pred.shape[0] != e - s or density.numel() != e - s:
+                    raise ValueError(f"lidar flow evaluation: the field returned {pred.shape[0]} flows and "
+                                     f"{density.numel()} densities for {e - s} points")
+                _ops._need_cuda(pred, density, lab, cls, g, sums)
+                _lib.call("emer_lidar_flow_accumulate", p(pred), ld, p(density), p(lab), p(cls), p(g), e - s,
+                          FLOW_DENSITY_THRESHOLD, p(sums[f]), p(ws), _ops._stream())
+                out = pred = density = None             # free this chunk before the next query
+    return sums

@@ -12,7 +12,8 @@ draws, made on the device's generator in the reference's order, and the batch as
 (``emer_topk_ratio`` and ``emer_pixel_batch``, csrc/raybatch.cu; INTEGRATION.md section 11).  ``PixelRaySampler`` also
 replaces ``get_render_rays`` and ``update_pixel_error_maps``, and with ``refresh_pixel_error_maps`` the whole error-map
 refresh of the training loop (``emer_image_rays``, ``emer_error_map`` and ``emer_error_map_normalize``,
-csrc/errormap.cu; INTEGRATION.md section 12).
+csrc/errormap.cu; INTEGRATION.md section 12).  ``LidarRaySampler`` also replaces the lidar sources' ``get_render_rays``
+with a frame table (INTEGRATION.md section 10).
 """
 from __future__ import annotations
 
@@ -429,11 +430,17 @@ class LidarRaySampler:
     ``torch.tensor`` and ``torch.equal``: the points of the candidate scans are gathered once per candidate set (a
     host compare of the list; a tensor by identity and version), then each step is the reference's one ``randint`` and
     four gathers.  ``torch.isin`` gives the reference's mask, in point order.  ``candidate_indices=None`` samples every
-    point (the reference then indexes whatever it cached last)."""
+    point (the reference then indexes whatever it cached last).
+
+    ``get_render_rays(time_idx)`` replaces the sources' ``get_render_rays`` (lidar_source.py:310-327 and the Waymo
+    override, datasets/waymo.py:341-356) without their seven boolean indexes, each a scan of every point of the drive
+    and a host sync.  A frame table is built once per state of ``source.timesteps`` (its identity and ``_version``)
+    with two host syncs; after that a frame costs no sync."""
 
     def __init__(self, source):
         self.source = source
         self._key, self._cached, self._held = None, None, None
+        self._frames = None                  # (timesteps, its _version, {time index: (start, count)}, order or None)
 
     def get_train_rays(self, num_rays: int, candidate_indices=None) -> Dict[str, Tensor]:
         s = self.source
@@ -452,3 +459,48 @@ class LidarRaySampler:
         idx = torch.randint(0, len(origins), size=(num_rays,), device=s.device)
         return {"lidar_origins": origins[idx], "lidar_viewdirs": directions[idx], "lidar_ranges": ranges[idx],
                 "lidar_normed_timestamps": times[idx]}
+
+    def _frame_table(self):
+        """(table {time index: (start, count)}, order): the points of frame t are ``order[start:start + count]``, or
+        the rows ``[start, start + count)`` when order is None.  When every timestep is one contiguous run (the Waymo
+        loader concatenates the scans in order) each frame is a slice; otherwise a stable argsort keeps the points of
+        a frame in their order, as the reference's boolean index does."""
+        ts = self.source.timesteps
+        f = self._frames
+        if f is not None and f[0] is ts and f[1] == ts._version:
+            return f[2], f[3]
+        values, counts = torch.unique_consecutive(ts, return_counts=True)     # sizes its output: one sync
+        values, counts = torch.stack([values.to(torch.int64), counts]).tolist()   # the second
+        order = None
+        if len(set(values)) == len(values):
+            starts = np.cumsum([0] + counts[:-1]).tolist()
+            table = {v: (s, c) for v, s, c in zip(values, starts, counts)}
+        else:
+            totals: Dict[int, int] = {}
+            for v, c in zip(values, counts):
+                totals[v] = totals.get(v, 0) + c
+            keys = sorted(totals)
+            starts = np.cumsum([0] + [totals[k] for k in keys[:-1]]).tolist()
+            table = {k: (s, totals[k]) for k, s in zip(keys, starts)}
+            order = torch.argsort(ts, stable=True)
+        self._frames = (ts, ts._version, table, order)
+        return table, order
+
+    @torch.no_grad()
+    def get_render_rays(self, time_idx: int) -> Dict[str, Tensor]:
+        """Every point of the scan at ``time_idx``, in the source's point order: the reference's four keys, plus
+        ``lidar_flow``, ``lidar_flow_class`` and ``lidar_ground`` when the source has ``flows``, ``flow_classes`` and
+        ``grounds`` (the Waymo source).  Each value is ``torch.equal`` to the reference's; an absent index gives empty
+        tensors, as there.  Slices of the source's tensors when its timesteps are contiguous runs, gathers
+        otherwise."""
+        s = self.source
+        table, order = self._frame_table()
+        start, count = table.get(int(time_idx), (0, 0))
+        arrays = {"lidar_origins": s.origins, "lidar_viewdirs": s.directions, "lidar_ranges": s.ranges,
+                  "lidar_normed_timestamps": s.normalized_timestamps}
+        if all(getattr(s, k, None) is not None for k in ("flows", "flow_classes", "grounds")):
+            arrays.update(lidar_flow=s.flows, lidar_flow_class=s.flow_classes, lidar_ground=s.grounds)
+        if order is None:
+            return {k: v[start:start + count] for k, v in arrays.items()}
+        rows = order[start:start + count]
+        return {k: v[rows] for k, v in arrays.items()}

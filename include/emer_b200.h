@@ -589,6 +589,26 @@ int emer_depth_rmse(const float* pred, const float* target, int64_t n, double* o
  * are clamped to the fp32 value of +-(1 - 1e-7), as torch rounds the reference's bounds. */
 int emer_scene_flow_metrics(const float* pred, const float* labels, int64_t n, double* out, void* workspace,
                             void* stream);
+/* The lidar scene-flow evaluation of one chunk of a frame (replaces the per-frame body of the reference's flow
+ * evaluation, train_emernerf.py:248-281: the boolean indexes on lidar_flow_class != -1 and on the ground, the
+ * dynamic-density gate and compute_scene_flow_metrics with its host copies).  n points: pred rows of 3 floats with
+ * row stride ld_pred (>= 3; the forward flow read in place from the field's [n, 6] flow output), dynamic_density [n],
+ * labels [n, 3] dense, flow_class int64 [n], ground [n] (nonzero = ground) or NULL to keep the ground.  A point is
+ * valid when flow_class != -1 and counted when it is valid and not ground.  Over the counted points, with
+ * pred *= 0 where dynamic_density < threshold (NaN stays NaN, a negative value gives -0, a NaN density is not gated),
+ * the terms of emer_scene_flow_metrics are ADDED into sums[EMER_LIDAR_FLOW_SUMS] (fp64): the EPE sum, the strict,
+ * relaxed and outlier counts, the angle sum and the angle count (|label| > 0.1), then the counted and the valid points.
+ * One launch, no host sync, so the chunks of a frame add into one row; the last CTA adds the per-CTA sums in CTA order,
+ * so the row is bit-identical on one device.  With n = 0 the inputs may be NULL (an empty tensor's data).  workspace:
+ * the metrics workspace above. */
+enum {
+    EMER_LIDAR_FLOW_EPE = 0, EMER_LIDAR_FLOW_STRICT = 1, EMER_LIDAR_FLOW_RELAX = 2, EMER_LIDAR_FLOW_OUTLIER = 3,
+    EMER_LIDAR_FLOW_ANGLE = 4, EMER_LIDAR_FLOW_ANGLE_COUNT = 5, EMER_LIDAR_FLOW_COUNTED = 6, EMER_LIDAR_FLOW_VALID = 7,
+    EMER_LIDAR_FLOW_SUMS = 8
+};
+int emer_lidar_flow_accumulate(const float* pred, int64_t ld_pred, const float* dynamic_density, const float* labels,
+                               const int64_t* flow_class, const uint8_t* ground, int64_t n, float threshold,
+                               double* sums, void* workspace, void* stream);
 
 /* ---- few-shot occupancy evaluation (csrc/occupancy.cu; replaces datasets/metrics.py:249-472, collect_centroids and
  *      eval_few_shot_occ with knn_predict(knn_k=1, similarity="cosine"), and their boolean indexing, second field pass
