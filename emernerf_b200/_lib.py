@@ -109,6 +109,12 @@ _SIGNATURES = {
                        _P, _P, c_int64, _P, c_int, c_int64, _P],
     "emer_field_wgrad": [_P, c_int64, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, _P, c_int64, _P, _P,
                          c_int64, _P, _P, c_int64, _P],
+    "emer_flow_field_fwd": [_P, c_int64, c_int, _P, _P, _P, _P, c_int, _P, c_int64, _P, _P, c_int64, _P, _P, _P, c_int, _P, _P,
+                            _P, _P, _P, _P, c_int64, _P],
+    "emer_flow_field_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, c_int, _P, c_int64, _P, _P, c_int64, _P, _P, _P,
+                            _P, _P, _P, c_int64, _P, _P, c_int, c_int64, _P],
+    "emer_flow_warp_fwd": [_P, _P, _P, c_int64, _P, _P, _P, c_int, _P, c_int64, _P],
+    "emer_flow_warp_bwd": [_P, _P, _P, c_int64, _P, c_int, _P, _P, c_int64, _P],
     "emer_gen_rays": [_P, _P, _P, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P, c_int64, _P],
     "emer_topk_ratio": [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P],
     "emer_pixel_batch": [POINTER(EmerPixelBatchIn), POINTER(EmerPixelBatchOut), _P],
@@ -223,6 +229,12 @@ def tag_of(name: str, args) -> str:
             return f"C{args[2]}_K{args[7]}_N{args[6]}"
         if name == "emer_occ_classify":
             return f"C{args[2]}_K{args[8]}_N{args[6]}"
+        if name == "emer_flow_field_fwd":
+            return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("" if args[18].value else "_density")
+        if name == "emer_flow_field_bwd":
+            return f"k{args[10]}_f{args[12]}_N{args[29]}"
+        if name in ("emer_flow_warp_fwd", "emer_flow_warp_bwd"):
+            return f"N{args[9] if name == 'emer_flow_warp_fwd' else args[8]}"
         if name == "emer_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("_save" if args[19].value else "")
     except Exception:

@@ -851,6 +851,232 @@ def field_chain(enc: Tensor, ray_bias: Tensor, samples: int, base, head, want_ge
     return _FieldChain.apply(enc, ray_bias, samples, want_geo, *base, *head)
 
 
+# ----------------------------------------------------------------------------- flow variants' dynamic branch
+# "fused": RadianceField.forward runs the flow configs' temporal aggregation through flow_warp, one dynamic-table gather
+# over the stacked [current | forward | backward] coordinates and emer_flow_field_fwd / _bwd; "layers": the per-layer path
+FLOW_BRANCH = os.environ.get("EMER_FLOW_BRANCH", "layers")
+FLOW_K_ENC = (40, 64)           # emer_flow_field_*: the dynamic grid's L*F (40: the shipped configs)
+
+
+class _FlowWarp(torch.autograd.Function):
+    """(pos [N,3], flow [N,6], noise [N] | None, t [N]) -> the [2N, 4] grid coordinates of both flow warps
+    (``emer_flow_warp_fwd``); the backward hands d_flow to the flow MLP (time and noise take no gradient)."""
+
+    @staticmethod
+    def forward(ctx, pos: Tensor, flow: Tensor, noise: Optional[Tensor], t: Tensor, aabb: Tensor, time_diff,
+                unbounded: bool):
+        ctx.set_materialize_grads(False)
+        _need_cuda(pos, flow, t, aabb)
+        pos2, flow2 = _f32c(pos.reshape(-1, 3)), _f32c(flow.reshape(-1, 6))
+        n = pos2.shape[0]
+        t2 = _f32c(t.reshape(-1))
+        nz, ldn = (None, 0) if noise is None else _rows(noise.reshape(n, 1), 1)
+        box = _f32c(aabb.reshape(-1))
+        # the model's time step is a 0-d device tensor when it comes from the registered timesteps: read on the device
+        if isinstance(time_diff, Tensor):
+            td = _f32c(time_diff.reshape(1))
+        else:
+            td = torch.full((1,), float(time_diff), dtype=torch.float32, device=pos2.device)
+        coords = torch.empty((2 * n, 4), dtype=torch.float32, device=pos2.device)
+        _lib.call("emer_flow_warp_fwd", _ptr(pos2), _ptr(flow2), _ptr(nz), ldn, _ptr(t2), _ptr(box), _ptr(td),
+                  int(unbounded), _ptr(coords), n, _stream())
+        ctx.save_for_backward(pos2, flow2, nz, box)
+        ctx.meta = (ldn, int(unbounded), flow.shape)
+        return coords
+
+    @staticmethod
+    def backward(ctx, d_coords):
+        if d_coords is None or not ctx.needs_input_grad[1]:
+            return (None,) * 7
+        pos2, flow2, nz, box = ctx.saved_tensors
+        ldn, unbounded, flow_shape = ctx.meta
+        n = pos2.shape[0]
+        d_flow = torch.empty((n, 6), dtype=torch.float32, device=pos2.device)
+        _lib.call("emer_flow_warp_bwd", _ptr(pos2), _ptr(flow2), _ptr(nz), ldn, _ptr(box), unbounded,
+                  _ptr(_f32c(d_coords)), _ptr(d_flow), n, _stream())
+        return None, d_flow.view(flow_shape), None, None, None, None, None
+
+
+def flow_warp(pos: Tensor, flow: Tensor, noise: Optional[Tensor], t: Tensor, aabb: Tensor, time_diff,
+              unbounded: bool) -> Tensor:
+    """Rows [0, N): contract(pos + flow[..., :3] noise) | clamp(t + time_diff noise, 0, 1); rows [N, 2N): the backward
+    warp with flow[..., 3:] and -time_diff (radiance_field.py:449-452).  ``noise`` None: 1 (the eval renders)."""
+    return _FlowWarp.apply(pos, flow, noise, t, aabb, time_diff, unbounded)
+
+
+class _GridEncodeRows(torch.autograd.Function):
+    """grid_encode of the stacked rows [x_fixed ; x_var] in one gather; the backward scatters all rows into the table and
+    computes the input gradient of the x_var rows only (x_fixed takes none)."""
+
+    @staticmethod
+    def forward(ctx, x_fixed: Tensor, x_var: Tensor, params: Tensor, desc: GridDesc):
+        ctx.set_materialize_grads(False)
+        _need_cuda(x_fixed, x_var, params)
+        x = torch.cat([_f32c(x_fixed), _f32c(x_var)])
+        params = _f32c(params)
+        n = x.shape[0]
+        y = torch.empty((n, desc.n_output_dims), dtype=torch.float32, device=x.device)
+        _lib.call("emer_grid_fwd", ctypes.byref(desc.c), _ptr(x), _ptr(params), _ptr(y), n, _stream())
+        ctx.save_for_backward(x, params)
+        ctx.desc, ctx.n0 = desc, x_fixed.shape[0]
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        if dy is None:
+            return None, None, None, None
+        x, params = ctx.saved_tensors
+        desc, n0 = ctx.desc, ctx.n0
+        dy = _f32c(dy)
+        need_x, need_p = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        sink = _grad_sink(params) if need_p else None
+        dparams = sink[0] if sink is not None else (torch.zeros_like(params) if need_p else None)
+        if need_p:
+            _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(x), _ptr(params), _ptr(dy), _ptr(dparams), _ptr(None),
+                      x.shape[0], _stream())
+        dx = None
+        if need_x:
+            dx = torch.empty((x.shape[0] - n0, x.shape[1]), dtype=torch.float32, device=x.device)
+            _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(x[n0:]), _ptr(params), _ptr(dy[n0:]), _ptr(None),
+                      _ptr(dx), dx.shape[0], _stream())
+        if sink is not None:
+            sink[1]()
+            dparams = None
+        return None, dx, dparams, None
+
+
+def grid_encode_rows(x_fixed: Tensor, x_var: Tensor, params: Tensor, desc: GridDesc) -> Tensor:
+    """[N0 + N1, L*F] features of the rows [x_fixed ; x_var] (each [., D]); only x_var takes an input gradient."""
+    return _GridEncodeRows.apply(x_fixed, x_var, params, desc)
+
+
+class _FlowFieldChain(torch.autograd.Function):
+    """enc [3N, k_enc] = [current | forward-warped | backward-warped] encodings -> (sigma [N], rgb [N, 3] | None,
+    geo [N, 64], sem [N, 64] | None) of the blended features (F_c + 0.5 F_f + 0.5 F_b) / 2: base MLP per query, blend,
+    density and colour head in one kernel (``emer_flow_field_fwd``).  ``ray_bias`` None: density only (the lidar pass).
+
+    Backward: ``emer_flow_field_bwd`` for the data path (d_enc for all 3N rows), then the weight gradients from
+    ``emer_field_wgrad``: the colour head and the base MLP over the current N rows in one launch, the base MLP over the
+    2N warped rows in a second (density only: the base MLP over all 3N rows in one)."""
+
+    @staticmethod
+    def forward(ctx, enc: Tensor, ray_bias: Optional[Tensor], samples: int, wb0: Tensor, bb0: Tensor, wb1: Tensor,
+                bb1: Tensor, w0: Tensor, w1: Tensor, w2: Tensor, b2: Tensor):
+        ctx.set_materialize_grads(False)
+        _need_cuda(enc, wb0, wb1, w0, w1, w2)
+        enc2, ld_enc = _rows(enc, enc.shape[-1])
+        if ld_enc % 8 or enc2.data_ptr() % 32:
+            enc2, ld_enc = enc2.contiguous(), enc2.shape[1]
+        n3, k_enc = enc2.shape
+        n = n3 // 3
+        n_feat = wb1.shape[0]
+        n_ray_cols = w0.shape[1] - 64
+        ws = [_f32c(t) for t in (wb0, bb0, wb1, bb1, w0, w1, w2, b2)]
+        wb0c, bb0c, wb1c, bb1c, w0c, w1c, w2c, b2c = ws
+        head = ray_bias is not None
+        rb = _f32c(ray_bias) if head else None
+        if head and rb.shape != ((n + samples - 1) // samples, 128):
+            raise ValueError(f"flow_field_chain: ray_bias {tuple(rb.shape)} for {n} points x {samples} samples per ray")
+        dev = enc.device
+        train = any(ctx.needs_input_grad)
+        f32 = dict(dtype=torch.float32, device=dev)
+        sigma = torch.empty(n, **f32)
+        rgb = torch.empty((n, 3), **f32) if head else None
+        hb = torch.empty((n3, 64), **f32) if train else None
+        hg = torch.empty((n, 128), **f32)                 # the geometry half carries the blend
+        h1 = torch.empty((n, 64), **f32) if (train and head) else None
+        sem = torch.empty((n, 64), **f32) if n_feat == 128 else None
+        _lib.call("emer_flow_field_fwd", _ptr(enc2), ld_enc, k_enc, _ptr(wb0c), _ptr(bb0c), _ptr(wb1c), _ptr(bb1c), n_feat,
+                  _ptr(w0c[:, n_ray_cols:]), w0c.shape[1], _ptr(w1c[:, :64]), _ptr(w1c[:, 64 + n_ray_cols:]), w1c.shape[1],
+                  _ptr(w2c), _ptr(b2c), _ptr(rb), samples, _ptr(sigma), _ptr(rgb), _ptr(hb), _ptr(hg), _ptr(h1), _ptr(sem),
+                  n, _stream())
+        if train:
+            ctx.sinks = {k: _grad_sink(t) for k, t in zip(("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"), ws)}
+            ctx.save_for_backward(enc2, hb, hg, h1, rgb, sigma, wb0c, wb1c, w0c, w1c, w2c)
+            ctx.meta = (samples, n_ray_cols, n_feat, enc.shape, ld_enc, head)
+        return sigma, rgb, hg[:, 64:], sem
+
+    @staticmethod
+    def backward(ctx, d_sigma, d_rgb, d_geo, d_sem):
+        enc2, hb, hg, h1, rgb, sigma, wb0, wb1, w0, w1, w2 = ctx.saved_tensors
+        samples, n_ray_cols, n_feat, enc_shape, ld_enc, head = ctx.meta
+        n3, k_enc = enc2.shape
+        n = n3 // 3
+        dev = enc2.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        if d_sigma is None and d_rgb is None and d_geo is None and d_sem is None:
+            return (None,) * 11
+        n_rays = (n + samples - 1) // samples
+        w1hg = torch.cat([w1[:, :64], w1[:, 64 + n_ray_cols:]], dim=1)            # [64, 128] = [hidden | geo] columns
+        w0g = w0[:, n_ray_cols:].contiguous()
+        c = lambda g, w: None if g is None else _f32c(g.reshape(n, w))
+        d_geo, d_sem = c(d_geo, 64), c(d_sem, 64)
+        d_rgb2 = c(d_rgb, 3) if head else None
+        d_sig = None if d_sigma is None else _f32c(d_sigma).reshape(n)
+        D1 = torch.empty((n3, 128), **f32)         # rows [0, n): [dZ0 | dF_c]; rows [n, 3n): [unused | dF_f, dF_b]
+        dz2 = torch.empty((n, 3), **f32) if d_rgb2 is not None else None
+        dz1 = torch.empty((n, 64), **f32) if head else None
+        dzb = torch.empty((n3, 64), **f32)
+        d_enc = torch.empty((n3, k_enc), **f32) if ctx.needs_input_grad[0] else None
+        d_sem_q = torch.empty((n3, 64), **f32) if d_sem is not None else None
+        ray_sums = dz2 is not None and samples % 32 == 0
+        d_rb = torch.zeros((n_rays, 128), **f32) if ray_sums else None
+        _lib.call("emer_flow_field_bwd", _ptr(d_rgb2), _ptr(rgb), _ptr(d_sig), _ptr(sigma), _ptr(d_geo), _ptr(d_sem),
+                  _ptr(hb), _ptr(hg if head else None), _ptr(h1), _ptr(wb0), k_enc, _ptr(wb1), n_feat, _ptr(w0g), 64,
+                  _ptr(w1hg), _ptr(w1hg[:, 64:]), 128, _ptr(w2), _ptr(dz2), _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_enc),
+                  k_enc, _ptr(d_rb), _ptr(d_sem_q), samples, n, _stream())
+        if dz2 is not None and not ray_sums:            # ragged rays: the per-ray sums of [dZ0 | dZ1] on the host side
+            ray = torch.arange(n, device=dev) // samples
+            d_rb = torch.zeros((n_rays, 128), **f32)
+            d_rb[:, :64].index_add_(0, ray, D1[:n, :64])
+            d_rb[:, 64:].index_add_(0, ray, dz1)
+
+        sk = ctx.sinks
+        shapes = dict(wb0=wb0.shape, bb0=(64,), wb1=wb1.shape, bb1=(n_feat,), w0=w0.shape, w1=w1.shape, w2=w2.shape,
+                      b2=(3,))
+        keys = list(shapes) if dz2 is not None else ["wb0", "bb0", "wb1", "bb1"]
+        out, grads = {}, {}
+        for k in keys:
+            if sk[k] is None:
+                out[k] = grads[k] = torch.zeros(shapes[k], **f32)
+            else:
+                out[k] = sk[k][0]
+        o = lambda k: _ptr(out[k]) if k in out else None
+        rows = lambda t, r0: None if t is None else t[r0:]
+
+        def wgrad(r0: int, rn: int, with_head: bool):
+            if with_head:
+                w0g_d, ld_w0, w1g_d, ld_w1 = out["w0"][:, n_ray_cols:], out["w0"].stride(0), out["w1"][:, 64 + n_ray_cols:], out["w1"].stride(0)
+                hd = (hg, h1, dz2, dz1)
+            else:
+                w0g_d, ld_w0, w1g_d, ld_w1 = None, 0, None, 0
+                hd = (None, None, None, None)
+            _lib.call("emer_field_wgrad", _ptr(enc2[r0:]), ld_enc, k_enc, _ptr(hb[r0:]), _ptr(hd[0]), _ptr(hd[1]),
+                      _ptr(hd[2]), _ptr(hd[3]), _ptr(D1[r0:]), _ptr(dzb[r0:]), _ptr(rows(d_sem_q, r0)), n_feat, o("wb0"),
+                      o("bb0"), o("wb1"), o("bb1"), _ptr(w0g_d), ld_w0, o("w1") if with_head else None, _ptr(w1g_d),
+                      ld_w1, o("w2") if with_head else None, o("b2") if with_head else None, rn, _stream())
+
+        if dz2 is not None:
+            wgrad(0, n, True)                           # colour head + base MLP over the current rows
+            wgrad(n, 2 * n, False)                      # base MLP over the warped rows
+        else:
+            wgrad(0, n3, False)
+        for k in keys:
+            if sk[k] is not None:
+                sk[k][1]()
+        g = tuple(grads.get(k) for k in ("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"))
+        if d_enc is not None:
+            d_enc = d_enc.reshape(enc_shape)
+        return (d_enc, d_rb, None) + g
+
+
+def flow_field_chain(enc: Tensor, ray_bias: Optional[Tensor], samples: int, base, head):
+    """The three-query chain of the flow variants: ``enc`` [3N, k_enc] stacked [current | forward | backward]
+    encodings, ``base`` / ``head`` / ``ray_bias`` as :func:`field_chain`; ``ray_bias`` None: density only.
+    Returns (sigma [N], rgb [N, 3] | None, geo [N, 64], sem [N, 64] | None) of the blended features."""
+    return _FlowFieldChain.apply(enc, ray_bias, samples, *base, *head)
+
+
 # ----------------------------------------------------------------------------- sampling
 @torch.no_grad()
 def pdf_resample(vals: Tensor, cdfs: Tensor, n: int, bias: Optional[Tensor], s_min: float, s_max: float,

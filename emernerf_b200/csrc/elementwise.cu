@@ -43,38 +43,10 @@ __global__ void contract_bwd_kernel(const float* __restrict__ pos, const float* 
 #pragma unroll
     for (int d = 0; d < 3; ++d) g[d] = sel ? __ldg(dout + i * out_dim + d) : 0.0f;
     if (dtime && out_dim == 4) dtime[i] = __ldg(dout + i * 4 + 3);
-    float gxn[3];
-    if (unbounded) {
+    float dp[3];
+    contract_point_bwd(g, xn, mag, am, lo, hi, unbounded, dp);
 #pragma unroll
-        for (int d = 0; d < 3; ++d) g[d] *= 0.25f;
-        if (mag < 1.0f) {
-#pragma unroll
-            for (int d = 0; d < 3; ++d) gxn[d] = g[d];
-        } else {
-            const float inv = 1.0f / mag;
-            const float u = 2.0f - inv;
-            float dot = 0.0f;
-#pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                gxn[d] = u * inv * g[d];
-                dot = fmaf(g[d], xn[d], dot);
-            }
-            // d/dmag of (2 - 1/mag) * xn/mag, routed to the arg-max coordinate (inf-norm subgradient)
-            const float sgn = xn[am] > 0.0f ? 1.0f : (xn[am] < 0.0f ? -1.0f : 0.0f);
-            const float extra = dot * (2.0f * inv - 2.0f) * inv * inv * sgn;
-#pragma unroll
-            for (int d = 0; d < 3; ++d)
-                if (d == am) gxn[d] += extra;
-        }
-    } else {
-#pragma unroll
-        for (int d = 0; d < 3; ++d) gxn[d] = g[d];
-    }
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        float k = (unbounded ? 2.0f : 1.0f) / (hi[d] - lo[d]);
-        dpos[i * 3 + d] = gxn[d] * k;
-    }
+    for (int d = 0; d < 3; ++d) dpos[i * 3 + d] = dp[d];
 }
 
 __global__ void trunc_exp_fwd_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y,

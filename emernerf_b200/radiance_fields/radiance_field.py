@@ -359,6 +359,11 @@ class RadianceField(nn.Module):
                 dynamic_density, dynamic_rgb, dyn_geo, dyn_sem = self._run_chain(
                     self.dynamic_xyz_encoder, self.dynamic_base_mlp, self._space_time(normed, t), ray_bias,
                     want_geo=self.enable_shadow_head)
+            elif self._flow_branch_usable(positions, chain, return_density_only):
+                # EMER_FLOW_BRANCH=fused: the temporal aggregation inside the three-query chain
+                dynamic_density, dynamic_rgb, dyn_geo, dyn_sem, flow_out = self._flow_branch(
+                    positions, normed, t, ray_bias if chain else None)
+                out.update(flow_out)
             else:
                 dyn_feats, dyn_enc = self.forward_dynamic_hash(normed, t, return_hash_encodings=True)
                 if self.flow_xyz_encoder is not None:
@@ -432,17 +437,63 @@ class RadianceField(nn.Module):
             out.update(self.query_sky(directions[:, 0], data_dict=first))
         return out
 
+    def _temporal_noise(self, forward_flow: Tensor) -> Optional[Tensor]:
+        """The warp's noise as the reference draws it (radiance_field.py:563-568): the same generator call in the same
+        place, so the generator state after a step does not depend on the path; None for the eval renders' ones."""
+        if self._noise_override is not None:
+            return self._noise_override.to(forward_flow)
+        if self.training:
+            return torch.rand_like(forward_flow)[..., 0:1]
+        return None
+
+    def _flow_branch_usable(self, positions: Tensor, chain: bool, density_only: bool) -> bool:
+        return (_ops.FLOW_BRANCH == "fused" and self.flow_xyz_encoder is not None and self._fused_density
+                and (chain or density_only) and positions.dim() == 3 and _ops.on_device(positions)
+                and self.dynamic_xyz_encoder.n_output_dims in _ops.FLOW_K_ENC
+                and self._chain_usable(self.dynamic_xyz_encoder, self.dynamic_base_mlp))
+
+    def _flow_branch(self, positions: Tensor, normed: Tensor, t: Tensor, ray_bias: Optional[Tensor]):
+        """``forward``'s dynamic + flow branch with the temporal aggregation fused (EMER_FLOW_BRANCH=fused): the flow
+        field at the points, both warps in one launch, ONE dynamic-table gather over the stacked [current | forward |
+        backward] coordinates, ONE flow-table gather + flow MLP over the 2N warped rows, and the three-query chain.
+        ``ray_bias`` None: density only.  Returns (density, rgb | None, geo, sem | None, the flow keys of the
+        per-layer path: flows, predicted flows, the three hash encodings and ``dynamic_feats``)."""
+        lead = positions.shape[:-1]
+        n = positions[..., 0].numel()
+        G = self.geometry_feature_dim
+        flow = self.forward_flow_hash(normed, t)
+        fwd, bwd = flow[..., :3], flow[..., 3:]
+        noise = self._temporal_noise(fwd)
+        coords_w = _ops.flow_warp(positions, flow, noise, t, self.aabb, self.time_diff, self.unbounded)
+        pred, _ = self._encode_mlp(self.flow_xyz_encoder, self.flow_mlp, coords_w)
+        enc_d = self.dynamic_xyz_encoder
+        enc = _ops.grid_encode_rows(self._space_time(normed, t).reshape(n, -1), coords_w, enc_d.tcnn_encoding.params,
+                                    enc_d.desc)
+        lin = [m for m in self.dynamic_base_mlp if isinstance(m, nn.Linear)]
+        l0, l1, l2 = self.rgb_head.layers
+        sigma, rgb, geo, sem = _ops.flow_field_chain(
+            enc, ray_bias, lead[-1], (lin[0].weight, lin[0].bias, lin[1].weight, lin[1].bias),
+            (l0.weight, l1.weight, l2.weight, l2.bias))
+        k = enc.shape[-1]
+        feats = geo if sem is None else torch.cat([geo, sem], dim=-1)
+        res = {"forward_flow": fwd, "backward_flow": bwd,
+               "forward_dynamic_hash_encodings": enc[n:2 * n].view(*lead, k),
+               "forward_pred_backward_flow": pred[:n, 3:].view(*lead, 3),
+               "backward_dynamic_hash_encodings": enc[2 * n:].view(*lead, k),
+               "backward_pred_forward_flow": pred[n:, :3].view(*lead, 3),
+               "dynamic_feats": feats.view(*lead, -1),
+               "current_dynamic_hash_encodings": enc[:n].view(*lead, k)}
+        return (sigma.view(lead), None if rgb is None else rgb.view(*lead, 3), geo.view(*lead, G),
+                None if sem is None else sem.view(*lead, -1), res)
+
     def temporal_aggregation(self, positions: Tensor, normed_timestamps: Tensor, forward_flow: Tensor,
                              backward_flow: Tensor, dynamic_feats: Tensor) -> Dict[str, Tensor]:
         """Eq. (8) of the paper (radiance_field.py:553-620): re-query the dynamic and flow fields at
         the flow-warped positions / neighbouring times and blend."""
         if normed_timestamps.shape[-1] != 1:
             normed_timestamps = normed_timestamps.unsqueeze(-1)
-        if self._noise_override is not None:
-            noise = self._noise_override.to(forward_flow)
-        elif self.training:
-            noise = torch.rand_like(forward_flow)[..., 0:1]
-        else:
+        noise = self._temporal_noise(forward_flow)
+        if noise is None:
             noise = torch.ones_like(forward_flow)[..., 0:1]
         results = {}
         warped_feats = []

@@ -219,6 +219,45 @@ int emer_field_bwd(const float* d_rgb, const float* rgb, const float* d_sigma, c
                    float* d1, float* dzb, float* d_enc, int64_t ld_denc, float* d_ray_bias, int samples,
                    int64_t n, void* stream);
 
+/* The flow variants' dynamic branch on the same chain (csrc/field_fused.cu, the kernels above with three queries per
+ * row).  enc holds 3N rows: rows [0, N) the current encodings, [N, 2N) the forward-warped and [2N, 3N) the
+ * backward-warped ones.  Each goes through the base MLP, and the features blend before the density and the colour head
+ * (radiance_field.py:449-460, the same operation order):
+ *   F_q = relu(enc_q wb0^T + bb0) wb1^T + bb1,  feats = (F_c + 0.5 F_f + 0.5 F_b) / 2;  sigma, rgb as emer_field_fwd.
+ * save_hb is [3N, 64]; save_hg [N, 128] (required: its geometry half carries the blend) and save_sem [N, 64] hold the
+ * blended features.  rgb == NULL: density only (the lidar pass); the colour head is skipped and ray_bias, save_h1 may be
+ * NULL. */
+int emer_flow_field_fwd(const float* enc, int64_t ld_enc, int k_enc, const float* wb0, const float* bb0,
+                        const float* wb1, const float* bb1, int n_feat, const float* w0g, int64_t ld_w0,
+                        const float* w1h, const float* w1g, int64_t ld_w1, const float* w2, const float* b2,
+                        const float* ray_bias, int samples, float* sigma, float* rgb, float* save_hb, float* save_hg,
+                        float* save_h1, float* save_sem, int64_t n, void* stream);
+
+/* Backward of emer_flow_field_fwd: emer_field_bwd's data path for the blended features, whose gradient dF fans out to the
+ * three queries as dF / 2, dF / 4, dF / 4.  d1 is [3N, 128]: rows [0, N) = [dz0 | dF_c], rows N.. = [unused | dF_q];
+ * dzb and d_enc (row stride ld_denc) hold 3N rows, d_sem_q [3N, 64] the three queries' d_sem (required with d_sem).  The
+ * base MLP's weight gradients are emer_field_wgrad over the 3N rows (the colour head's over the first N);
+ * h1 == NULL: density only (no d_rgb, dz2, d_ray_bias). */
+int emer_flow_field_bwd(const float* d_rgb, const float* rgb, const float* d_sigma, const float* sigma,
+                        const float* d_geo, const float* d_sem, const float* hb, const float* hg, const float* h1,
+                        const float* wb0, int k_enc, const float* wb1, int n_feat, const float* w0g, int64_t ld_w0,
+                        const float* w1h, const float* w1g, int64_t ld_w1, const float* w2, float* dz2, float* dz1,
+                        float* d1, float* dzb, float* d_enc, int64_t ld_denc, float* d_ray_bias, float* d_sem_q,
+                        int samples, int64_t n, void* stream);
+
+/* The flow warp of the temporal aggregation (csrc/flow_branch.cu; radiance_field.py:449-452), both directions in one
+ * launch.  pos [N,3], flow [N,6] = [forward | backward], noise [N] (row stride ld_noise; NULL: 1, the eval renders),
+ * t [N], time_diff: one float on the device (the model's time step may be a device tensor; reading it on the host would
+ * stall the stream).  coords [2N,4] (16-byte aligned): row i = [contract(pos + flow[:,0:3] noise) | clamp(t + time_diff noise, 0, 1)],
+ * row N + i = [contract(pos + flow[:,3:6] noise) | clamp(t - time_diff noise, 0, 1)], with the in-cube selector. */
+int emer_flow_warp_fwd(const float* pos, const float* flow, const float* noise, int64_t ld_noise, const float* t,
+                       const float* aabb6, const float* time_diff, int unbounded, float* coords, int64_t n, void* stream);
+
+/* Backward of emer_flow_warp_fwd: d_flow [N,6] (written) from d_coords [2N,4] (the grid input gradient of those rows;
+ * the time column is ignored) through the contraction's Jacobian, the selector and noise. */
+int emer_flow_warp_bwd(const float* pos, const float* flow, const float* noise, int64_t ld_noise, const float* aabb6,
+                       int unbounded, const float* d_coords, float* d_flow, int64_t n, void* stream);
+
 /* Weight gradients of the fused field chain from emer_field_bwd's buffers, in one launch that reads every row buffer
  * once (csrc/field_wgrad.cu).  All outputs accumulate (+=; the caller zeroes):
  *   dwb0 [64, k_enc] += dzb^T enc,                 dbb0 [64]     += column sums of dzb
