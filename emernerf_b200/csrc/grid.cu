@@ -19,8 +19,10 @@
 // instruction: a row's sector holds a pair of F = 4 levels, and lane pairs swap halves.  Per 524 288
 // ray-coherent points of the static 122 MB grid (H100 80GB HBM3, 700 W): gather 0.34 -> 0.21 ms,
 // scatter 0.48 -> 0.43 ms against one level per group (DESIGN.md §4).  All 2^D corner gathers of a
-// level are issued back to back (16-byte LDG for F=4) before the first use.  The input gradient
-// (never needed in training) stays one thread per point, all levels.
+// level are issued back to back (16-byte LDG for F=4) before the first use; for F = 4 a lane pair
+// fetches the two x-neighbour corners of a cell in one load instruction (gather_corner_pairs), and
+// the scatter reduces them in one instruction where a warp has no same-cell runs.  The input
+// gradient (never needed in training) stays one thread per point, all levels.
 #include "common.cuh"
 #include "grid_common.cuh"
 
@@ -129,6 +131,9 @@ __global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd, con
 #pragma unroll
     for (int d = 0; d < D; ++d) p[d] = 0.0f;
     if (active) load_point<D>(x, i, p);
+    float pq[D];                                // the position of the lane pair's other row (F = 4)
+#pragma unroll
+    for (int d = 0; d < D; ++d) pq[d] = F == 4 ? __shfl_xor_sync(0xffffffffu, p[d], 1) : 0.0f;
     // F = 4 level pairs of an even L are the 32-byte sectors of the rows
     const bool sector_pairs = !EMER_GRID_DIAG_LEVEL_MAJOR && F == 4 && cnt == 2 && !(L & 1);
     float4 held = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -148,11 +153,25 @@ __global__ void __launch_bounds__(256) grid_fwd_kernel(const GridDescDev gd, con
         Vec<F> val[1 << D];
         float wt[1 << D];
 #pragma unroll
-        for (int c = 0; c < (1 << D); ++c) {
-            uint32_t cc[D];
-            corner_cell<D>(c, c0, cc);
-            wt[c] = corner_weight<D>(c, w);
-            val[c] = load_entry<F>(lt, grid_index<D>(cc, res, size, hashed));
+        for (int c = 0; c < (1 << D); ++c) wt[c] = corner_weight<D>(c, w);
+        if constexpr (F == 4) {
+            // the x-neighbour corners of a cell in one load instruction of a lane pair (gather_corner_pairs)
+            uint32_t c0q[D];
+            float wq[D];
+            locate<D>(pq, scale, c0q, wq);
+            float4 v4[1 << D];
+            gather_corner_pairs<D>(reinterpret_cast<const float4*>(lt), c0, c0q, res, size, hashed, v4);
+#pragma unroll
+            for (int c = 0; c < (1 << D); ++c) {
+                val[c].v[0] = v4[c].x; val[c].v[1] = v4[c].y; val[c].v[2] = v4[c].z; val[c].v[3] = v4[c].w;
+            }
+        } else {
+#pragma unroll
+            for (int c = 0; c < (1 << D); ++c) {
+                uint32_t cc[D];
+                corner_cell<D>(c, c0, cc);
+                val[c] = load_entry<F>(lt, grid_index<D>(cc, res, size, hashed));
+            }
         }
         float acc[F];
 #pragma unroll
@@ -247,6 +266,9 @@ __global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev g
 #pragma unroll
     for (int d = 0; d < D; ++d) p[d] = 0.0f;
     if (active) load_point<D>(x, i, p);
+    float pq[D];                                // the position of the lane pair's other row (F = 4)
+#pragma unroll
+    for (int d = 0; d < D; ++d) pq[d] = F == 4 ? __shfl_xor_sync(0xffffffffu, p[d], 1) : 0.0f;
     const int64_t ia = active ? i : 0;
 #pragma unroll
     for (int j = 0; j < (F == 4 ? 2 * G : G); ++j) {
@@ -325,6 +347,40 @@ __global__ void __launch_bounds__(256) grid_bwd_table_kernel(const GridDescDev g
 #pragma unroll
                 for (int f = 0; f < F; ++f) nz |= (v[f] != 0.0f);
                 if (head && active && nz) red_add_entry<F>(lt, idx[c], v);
+            }
+        } else if (F == 4 && !EMER_GRID_DIAG_XHIGH_REUSE) {
+            // No runs in this warp (a warp-uniform branch): a lane pair (rows r, r + 1) issues the reductions of a
+            // cell's two x-neighbour corners in one instruction, as the gather loads them (gather_corner_pairs):
+            // row r's corners 2h (even lane) and 2h + 1 (odd lane), then row r + 1's, for each h.  Each lane sends its
+            // partner the value that the partner reduces.  A row with a zero upstream gradient adds nothing.
+            const bool odd = threadIdx.x & 1;
+            const bool any_q = __shfl_xor_sync(0xffffffffu, any, 1);
+            const bool any_r = odd ? any_q : any, any_s = odd ? any : any_q;
+            uint32_t c0q[D];
+            float wq[D];
+            locate<D>(pq, scale, c0q, wq);
+            uint32_t cr[D], cs[D];                  // cells of rows r and r + 1
+#pragma unroll
+            for (int d = 0; d < D; ++d) {
+                cr[d] = odd ? c0q[d] : c0[d];
+                cs[d] = odd ? c0[d] : c0q[d];
+            }
+#pragma unroll
+            for (int h = 0; h < (1 << (D - 1)); ++h) {
+                const float tl = corner_weight<D>(2 * h, w), th = corner_weight<D>(2 * h + 1, w);
+                float va[F], vb[F];
+#pragma unroll
+                for (int f = 0; f < F; ++f) {
+                    const float lo = tl * g_out[f], hi = th * g_out[f];
+                    const float r = __shfl_xor_sync(0xffffffffu, odd ? lo : hi, 1);
+                    va[f] = odd ? r : lo;           // row r, corner 2h + odd
+                    vb[f] = odd ? hi : r;           // row r + 1, corner 2h + odd
+                }
+                uint32_t cc[D];
+                corner_cell<D>(2 * h + odd, cr, cc);
+                if (any_r) red_add_entry<F>(lt, grid_index<D>(cc, res, size, hashed), va);
+                corner_cell<D>(2 * h + odd, cs, cc);
+                if (any_s) red_add_entry<F>(lt, grid_index<D>(cc, res, size, hashed), vb);
             }
         } else if (any) {
 #pragma unroll

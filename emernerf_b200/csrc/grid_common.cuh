@@ -58,4 +58,71 @@ __device__ __forceinline__ float corner_weight(int c, const float (&w)[D]) {
     return t;
 }
 
+// Diagnostic build only (tools/microbench_grid_corners.py): the x-high corner of each pair (c, c + 1) is not loaded
+// and takes the x-low corner's value, so each gather issues half its corner loads.  The outputs are wrong; the time
+// bounds what fetching a pair in one instruction can save.  It also turns off the table scatter's paired reductions.
+// Never set in the library.
+#ifndef EMER_GRID_DIAG_XHIGH_REUSE
+#define EMER_GRID_DIAG_XHIGH_REUSE 0
+#endif
+
+__device__ __forceinline__ float shfl_xor1(float v) { return __shfl_xor_sync(0xffffffffu, v, 1); }
+__device__ __forceinline__ float4 shfl_xor1(float4 v) {
+    return make_float4(shfl_xor1(v.x), shfl_xor1(v.y), shfl_xor1(v.z), shfl_xor1(v.w));
+}
+
+// The table entries (T = float for F = 1, float4 for F = 4) of the 2^D corners of this lane's cell c0, in corner
+// order, fetched with loads that a lane pair shares.  Corners c and c + 1 (c even) differ only in x, and the hash's x
+// prime is 1, so they usually share a line: idx(x + 1) = idx(x) ^ (2^(k+1) - 1) for k trailing one bits of x, and a
+// dense level gives idx + 1 unless the far face wraps.  So for the rows (r, r + 1) of a lane pair, the first half of
+// the loads fetches corner c of row r on the even lane and corner c + 1 of row r on the odd lane, the second half the
+// same for row r + 1; then each lane swaps the half of its values that belongs to its partner.  Each load instruction
+// then touches about half as many lines as one lane per corner.  c0q is the partner row's cell (every address is
+// computed before the first load).  Called by all 32 lanes of the warp; the values are those of one load per corner.
+template <int D, typename T>
+__device__ __forceinline__ void gather_corner_pairs(const T* __restrict__ lt, const uint32_t (&c0)[D],
+                                                    const uint32_t (&c0q)[D], uint32_t res, uint32_t size,
+                                                    bool hashed, T (&val)[1 << D]) {
+    constexpr int H = 1 << (D - 1);
+#if EMER_GRID_DIAG_XHIGH_REUSE
+    (void)c0q;
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+        uint32_t cc[D];
+        corner_cell<D>(2 * h, c0, cc);
+        val[2 * h] = __ldg(lt + grid_index<D>(cc, res, size, hashed));
+        val[2 * h + 1] = val[2 * h];
+    }
+#else
+    const bool odd = threadIdx.x & 1;
+    uint32_t cr[D], cs[D];                      // cells of rows r and r + 1
+#pragma unroll
+    for (int d = 0; d < D; ++d) {
+        cr[d] = odd ? c0q[d] : c0[d];
+        cs[d] = odd ? c0[d] : c0q[d];
+    }
+    T a[H], b[H];
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+        uint32_t cc[D];
+        corner_cell<D>(2 * h + odd, cr, cc);
+        a[h] = __ldg(lt + grid_index<D>(cc, res, size, hashed));
+    }
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+        uint32_t cc[D];
+        corner_cell<D>(2 * h + odd, cs, cc);
+        b[h] = __ldg(lt + grid_index<D>(cc, res, size, hashed));
+    }
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+        // even lane: a = its corner 2h, the partner's a = its corner 2h + 1; odd lane: b = its corner 2h + 1, the
+        // partner's b = its corner 2h
+        const T r = shfl_xor1(odd ? a[h] : b[h]);
+        val[2 * h] = odd ? r : a[h];
+        val[2 * h + 1] = odd ? b[h] : r;
+    }
+#endif
+}
+
 }  // namespace emer

@@ -59,7 +59,8 @@ __device__ __forceinline__ PlRay pl_load_ray(const float* origins, const float* 
 }
 
 // Interval midpoint -> contracted, selector-masked grid coordinate xc -> hash-grid features enc.  ONE body for the
-// forward and the backward kernel, so the backward re-derives bit for bit what the forward saw.
+// forward and the backward kernel, so the backward re-derives bit for bit what the forward saw.  Called by all 32
+// lanes of the warp (lanes past the ray's last sample repeat it): with LF_T > 0, lane pairs share the corner loads.
 template <int LF_T>
 __device__ __forceinline__ void pl_encode(const emer_grid_desc& g, const float* __restrict__ table, int unbounded,
                                           const PlRay& rc, float t0, float t1, float (&xc)[3],
@@ -72,6 +73,9 @@ __device__ __forceinline__ void pl_encode(const emer_grid_desc& g, const float* 
     int amax;
     bool sel;
     contract_point(pos, rc.lo3, rc.hi3, unbounded, 1, xc, xn, mag, amax, sel);
+    float xq[3];                                // the lane pair's other sample (LF_T > 0)
+#pragma unroll
+    for (int d = 0; d < 3; ++d) xq[d] = LF_T > 0 ? shfl_xor1(xc[d]) : 0.0f;
 #pragma unroll
     for (int l = 0; l < L; ++l) {
         const uint32_t res = g.resolution[l], off = g.offset[l], size = g.offset[l + 1] - off;
@@ -80,14 +84,25 @@ __device__ __forceinline__ void pl_encode(const emer_grid_desc& g, const float* 
         float w[3];
         locate<3>(xc, g.scale[l], c0, w);
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
+        if constexpr (LF_T > 0) {
+            // F = 1: the x-neighbour corners of a cell in one load instruction of a lane pair (gather_corner_pairs);
+            // the same values, accumulated in the same order
+            uint32_t c0q[3];
+            float wq[3];
+            locate<3>(xq, g.scale[l], c0q, wq);
+            float val[8];
+            gather_corner_pairs<3>(table + off, c0, c0q, res, size, hashed, val);
 #pragma unroll
-        for (int cc = 0; cc < 8; ++cc) {
-            const float wt = corner_weight<3>(cc, w);
-            uint32_t ci[3];
-            corner_cell<3>(cc, c0, ci);
-            const float* e = table + ((size_t)off + grid_index<3>(ci, res, size, hashed)) * F;
-            if (LF_T > 0) acc[0] = fmaf(wt, __ldg(e), acc[0]);
-            else for (int f = 0; f < F; ++f) acc[f] = fmaf(wt, __ldg(e + f), acc[f]);
+            for (int cc = 0; cc < 8; ++cc) acc[0] = fmaf(corner_weight<3>(cc, w), val[cc], acc[0]);
+        } else {
+#pragma unroll
+            for (int cc = 0; cc < 8; ++cc) {
+                const float wt = corner_weight<3>(cc, w);
+                uint32_t ci[3];
+                corner_cell<3>(cc, c0, ci);
+                const float* e = table + ((size_t)off + grid_index<3>(ci, res, size, hashed)) * F;
+                for (int f = 0; f < F; ++f) acc[f] = fmaf(wt, __ldg(e + f), acc[f]);
+            }
         }
         if (LF_T > 0) enc[l] = acc[0];
         else for (int f = 0; f < F; ++f) enc[l * F + f] = acc[f];
@@ -104,9 +119,10 @@ __device__ __forceinline__ void pl_load_row(const float* __restrict__ row16, flo
 }
 
 // LF_T > 0: compile-time feature count with F = 1 (the shipped proposal grids: 8 levels x 1 feature);
-// LF_T == 0: generic run-time loops.
+// LF_T == 0: generic run-time loops.  Two CTAs per SM, as the ~100 registers allow: left to itself, ptxas squeezes
+// <8> into 80 registers and spills.
 template <int LF_T>
-__global__ void __launch_bounds__(PL_WARPS * 32) prop_level_kernel(const PropParams p) {
+__global__ void __launch_bounds__(PL_WARPS * 32, 2) prop_level_kernel(const PropParams p) {
     __shared__ float t_edges[PL_WARPS][PL_MAX_EDGES + 3];
     __shared__ __align__(16) float w0s[PL_HID * PL_MAX_IN];
     __shared__ float b0s[PL_HID], w1s[PL_HID];
@@ -139,11 +155,12 @@ __global__ void __launch_bounds__(PL_WARPS * 32) prop_level_kernel(const PropPar
         const int k = k0 + lane;
         const bool ok = k < n;
         float xdelta = 0.0f;
+        const int kc = ok ? k : n - 1;
+        const float t0 = t_edges[wid][kc], t1 = t_edges[wid][kc + 1];
+        float xc[3];
+        float enc[LF_T > 0 ? LF_T : PL_MAX_IN];
+        pl_encode<LF_T>(p.g, p.table, p.unbounded, rc, t0, t1, xc, enc);
         if (ok) {
-            const float t0 = t_edges[wid][k], t1 = t_edges[wid][k + 1];
-            float xc[3];
-            float enc[LF_T > 0 ? LF_T : PL_MAX_IN];
-            pl_encode<LF_T>(p.g, p.table, p.unbounded, rc, t0, t1, xc, enc);
             // Linear(LF, 64) - ReLU - Linear(64, 1) - trunc_exp(. - 1)
             float raw = b1;
 #pragma unroll 4
@@ -267,8 +284,12 @@ __global__ void __launch_bounds__(PL_WARPS * 32) prop_level_bwd_kernel(const Pro
             float d_raw = 0.0f;
 #pragma unroll
             for (int i = 0; i < LF; ++i) { enc[i] = 0.0f; d_enc[i] = 0.0f; }
-            if (ok) {
-                pl_encode<LF>(p.g, p.table, p.unbounded, rc, t_edges[wid][k], t_edges[wid][k + 1], xc, enc);
+            const int kc = ok ? k : n - 1;
+            pl_encode<LF>(p.g, p.table, p.unbounded, rc, t_edges[wid][kc], t_edges[wid][kc + 1], xc, enc);
+            if (!ok) {
+#pragma unroll
+                for (int i = 0; i < LF; ++i) enc[i] = 0.0f;
+            } else {
                 d_raw = d_raw_s[wid][k];
 #pragma unroll 4
                 for (int j = 0; j < PL_HID; ++j) {
