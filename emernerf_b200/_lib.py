@@ -131,6 +131,8 @@ _SIGNATURES = {
     "emer_ray_loss_fwd": [c_int, _P, _P, _P, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, _P, _P, _P],
     "emer_ray_loss_bwd": [c_int, _P, _P, _P, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, _P, _P, _P,
                           _P],
+    "emer_ray_loss_live_fwd": [c_int, _P, _P, _P, c_int64, c_int, _P, c_float, _P, _P, _P],
+    "emer_ray_loss_live_bwd": [c_int, _P, _P, _P, c_int64, c_int, _P, c_float, _P, _P, _P, _P],
     "emer_cycle_loss_fwd": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, _P, _P, _P],
     "emer_cycle_loss_bwd": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, _P, _P, _P, _P, _P],
     "emer_render_fwd": [POINTER(EmerRenderIn), POINTER(EmerRenderOut), _P],
@@ -215,7 +217,7 @@ def tag_of(name: str, args) -> str:
             return f"k{args[2]}_f{args[11]}_N{args[23]}"
         if name in ("emer_pointwise_loss_fwd", "emer_pointwise_loss_bwd"):
             return f"kind{args[0]}_N{args[3]}"
-        if name in ("emer_ray_loss_fwd", "emer_ray_loss_bwd"):
+        if name in ("emer_ray_loss_fwd", "emer_ray_loss_bwd", "emer_ray_loss_live_fwd", "emer_ray_loss_live_bwd"):
             return f"kind{args[0]}_R{args[4]}_S{args[5]}"
         if name in ("emer_cycle_loss_fwd", "emer_cycle_loss_bwd"):
             return f"N{args[8]}"

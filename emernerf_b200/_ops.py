@@ -10,7 +10,7 @@ from __future__ import annotations
 import ctypes
 import math
 import weakref
-from typing import Callable, Dict, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 from torch import Tensor
@@ -1578,7 +1578,9 @@ def pointwise_loss(kind: str, a: Tensor, b: Optional[Tensor], p0: float = 0.0, p
 
 
 class _RayLoss(torch.autograd.Function):
-    """Per-ray sums over [R, S] rows (EMER_RAY_LOSS_*); differentiable w.r.t. the weights only."""
+    """Per-ray sums over [R, S] rows (EMER_RAY_LOSS_*); differentiable w.r.t. the weights only.  ``consts`` is the
+    three Python floats of the kind, or a device tensor of four (``sight_consts``, with ``pre`` last) that the kernels
+    read when they run."""
 
     @staticmethod
     def forward(ctx, w: Tensor, t: Optional[Tensor], gt: Tensor, kind: int, consts: Tuple[float, float, float],
@@ -1592,8 +1594,13 @@ class _RayLoss(torch.autograd.Function):
             raise ValueError(f"ray loss: weights {tuple(w.shape)}, t {None if t is None else tuple(t.shape)}, "
                              f"per-ray {tuple(gt.shape)}")
         out = torch.empty(2, dtype=torch.float32, device=wc.device)
-        _lib.call("emer_ray_loss_fwd", kind, _ptr(wc), _ptr(tc), _ptr(gc), r, s, *consts, pre, post, _ptr(out),
-                  _ptr(_workspace(_LOSS_WS, wc.device, LOSS_WORKSPACE_BYTES, "losses")), _stream())
+        ws = _ptr(_workspace(_LOSS_WS, wc.device, LOSS_WORKSPACE_BYTES, "losses"))
+        if torch.is_tensor(consts):
+            _lib.call("emer_ray_loss_live_fwd", kind, _ptr(wc), _ptr(tc), _ptr(gc), r, s, _ptr(consts), post, _ptr(out),
+                      ws, _stream())
+        else:
+            _lib.call("emer_ray_loss_fwd", kind, _ptr(wc), _ptr(tc), _ptr(gc), r, s, *consts, pre, post, _ptr(out), ws,
+                      _stream())
         ctx.save_for_backward(wc, tc, gc, out)
         ctx.args = (kind, consts, pre, post)
         return out[0]
@@ -1605,8 +1612,12 @@ class _RayLoss(torch.autograd.Function):
         w, t, gt, out = ctx.saved_tensors
         kind, consts, pre, post = ctx.args
         dw = torch.empty_like(w)
-        _lib.call("emer_ray_loss_bwd", kind, _ptr(w), _ptr(t), _ptr(gt), w.shape[0], w.shape[1], *consts, pre, post,
-                  _ptr(out), _ptr(_f32c(g)), _ptr(dw), _stream())
+        if torch.is_tensor(consts):
+            _lib.call("emer_ray_loss_live_bwd", kind, _ptr(w), _ptr(t), _ptr(gt), w.shape[0], w.shape[1], _ptr(consts),
+                      post, _ptr(out), _ptr(_f32c(g)), _ptr(dw), _stream())
+        else:
+            _lib.call("emer_ray_loss_bwd", kind, _ptr(w), _ptr(t), _ptr(gt), w.shape[0], w.shape[1], *consts, pre,
+                      post, _ptr(out), _ptr(_f32c(g)), _ptr(dw), _stream())
         return dw, None, None, None, None, None, None
 
 
@@ -1617,10 +1628,30 @@ def _sight_consts(epsilon: float) -> Tuple[float, float, float]:
     return float(epsilon), 2 * sigma**2, 1 / (math.sqrt(2 * math.pi * sigma**2))
 
 
-def line_of_sight_loss(weights: Tensor, t_vals: Tensor, gt_depth: Tensor, epsilon: float, pre: float = 1.0,
-                       post: float = 1.0) -> Tensor:
+def sight_consts(epsilon: float, pre: float = 1.0) -> List[float]:
+    """[epsilon, 2 sigma^2, 1 / sqrt(2 pi sigma^2), pre] as the fp32 values the float entry points receive: derived in
+    double by ``_sight_consts``, each rounded once.  What a live call reads from device memory."""
+    return [float(v) for v in torch.tensor([*_sight_consts(epsilon), float(pre)], dtype=torch.float32).tolist()]
+
+
+def _live_consts(consts: Tensor) -> Tensor:
+    if not (torch.is_tensor(consts) and consts.dtype == torch.float32 and consts.shape == (4,) and on_device(consts)
+            and consts.is_contiguous()):
+        raise ValueError("live line-of-sight constants: a contiguous float32 CUDA tensor of 4 values "
+                         "[epsilon, 2 sigma^2, 1 / sqrt(2 pi sigma^2), pre] (see sight_consts)")
+    return consts
+
+
+def line_of_sight_loss(weights: Tensor, t_vals: Tensor, gt_depth: Tensor, epsilon: Union[float, Tensor],
+                       pre: float = 1.0, post: float = 1.0) -> Tensor:
     """post * mean(pre * compute_line_of_sight_loss(gt_depth, weights, t_vals, epsilon)); t_vals and gt_depth are
-    constants."""
+    constants.  ``epsilon`` may be the device form of ``sight_consts(epsilon, pre)`` instead, whose ``pre`` replaces
+    the argument: the kernels then read the constants when they run, so a CUDA graph replays with the current ones."""
+    if torch.is_tensor(epsilon):
+        if pre != 1.0:
+            raise ValueError("line_of_sight_loss: with device constants, pre is their last value")
+        return _RayLoss.apply(weights, t_vals.detach(), gt_depth.detach(), RAY_LOSS_KINDS["line_of_sight"],
+                              _live_consts(epsilon), 1.0, float(post))
     return _RayLoss.apply(weights, t_vals.detach(), gt_depth.detach(), RAY_LOSS_KINDS["line_of_sight"],
                           _sight_consts(epsilon), float(pre), float(post))
 

@@ -49,7 +49,19 @@ struct LossParams {
     const float* g;          // backward: upstream gradient (device scalar)
     float* da;
     float* db;
+    const float* live;       // per-ray kinds, live entry points: one {p0, p1, p2, pre} for the launch, else null
 };
+
+// the per-step constants of a live call replace the launch's; a float call keeps its own
+__device__ __forceinline__ LossParams with_live(LossParams p) {
+    if (p.live) {
+        p.p0 = __ldg(p.live);
+        p.p1 = __ldg(p.live + 1);
+        p.p2 = __ldg(p.live + 2);
+        p.pre = __ldg(p.live + 3);
+    }
+    return p;
+}
 
 // ---------------------------------------------------------------------------------------------- the terms
 __device__ __forceinline__ float real_term(int base, float d) {       // base: 0 l1, 1 l2, 2 smooth_l1 (beta 1)
@@ -206,7 +218,8 @@ __device__ __forceinline__ float dirac(float t, float gt, float two_sigma_sq, fl
     return amp * expf(-(x * x) / two_sigma_sq);
 }
 
-__global__ void __launch_bounds__(LOSS_THREADS) ray_loss_fwd_kernel(const LossParams p) {
+__global__ void __launch_bounds__(LOSS_THREADS) ray_loss_fwd_kernel(const LossParams launch) {
+    const LossParams p = with_live(launch);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     float sa = 0.0f, sb = 0.0f;
     long long cnt = 0;
@@ -254,7 +267,8 @@ __global__ void __launch_bounds__(LOSS_THREADS) ray_loss_fwd_kernel(const LossPa
     }
 }
 
-__global__ void __launch_bounds__(LOSS_THREADS) ray_loss_bwd_kernel(const LossParams p) {
+__global__ void __launch_bounds__(LOSS_THREADS) ray_loss_bwd_kernel(const LossParams launch) {
+    const LossParams p = with_live(launch);
     const float rays = (float)p.n;
     const float g = __ldg(p.g) * p.post / rays;
     // line of sight: every ray's sum enters through mean(empty) + mean(near), scaled by pre and the count of gt > 0
@@ -440,6 +454,33 @@ extern "C" int emer_ray_loss_bwd(int kind, const float* w, const float* t, const
                  nullptr};
     ray_loss_bwd_kernel<<<loss_grid(n_rays * n_samples, LOSS_THREADS), LOSS_THREADS, 0, (cudaStream_t)stream>>>(p);
     return check_launch("emer_ray_loss_bwd");
+}
+
+extern "C" int emer_ray_loss_live_fwd(int kind, const float* w, const float* t, const float* gt, int64_t n_rays,
+                                      int n_samples, const float* consts, float post, float* out, void* workspace,
+                                      void* stream) {
+    EMER_REQUIRE(kind == EMER_RAY_LOSS_LINE_OF_SIGHT || kind == EMER_RAY_LOSS_SIGHT,
+                 "emer_ray_loss_live_fwd: kind %d has no live constants", kind);
+    EMER_REQUIRE(w && t && gt && consts && out && workspace, "emer_ray_loss_live_fwd: NULL pointer");
+    EMER_REQUIRE(n_rays >= 0 && n_samples >= 1, "emer_ray_loss_live_fwd: bad shape");
+    LossParams p{kind, w, t, gt, n_rays, n_samples, 0.0f, 0.0f, 0.0f, 0.0f, post, out, (LossWorkspace*)workspace,
+                 nullptr, nullptr, nullptr, consts};
+    ray_loss_fwd_kernel<<<loss_grid(n_rays, LOSS_WARPS), LOSS_THREADS, 0, (cudaStream_t)stream>>>(p);
+    return check_launch("emer_ray_loss_live_fwd");
+}
+
+extern "C" int emer_ray_loss_live_bwd(int kind, const float* w, const float* t, const float* gt, int64_t n_rays,
+                                      int n_samples, const float* consts, float post, const float* fwd_out,
+                                      const float* g, float* dw, void* stream) {
+    EMER_REQUIRE(kind == EMER_RAY_LOSS_LINE_OF_SIGHT || kind == EMER_RAY_LOSS_SIGHT,
+                 "emer_ray_loss_live_bwd: kind %d has no live constants", kind);
+    EMER_REQUIRE(w && t && gt && consts && fwd_out && g && dw, "emer_ray_loss_live_bwd: NULL pointer");
+    EMER_REQUIRE(n_rays >= 0 && n_samples >= 1, "emer_ray_loss_live_bwd: bad shape");
+    if (n_rays == 0) return 0;
+    LossParams p{kind, w, t, gt, n_rays, n_samples, 0.0f, 0.0f, 0.0f, 0.0f, post, (float*)fwd_out, nullptr, g, dw,
+                 nullptr, consts};
+    ray_loss_bwd_kernel<<<loss_grid(n_rays * n_samples, LOSS_THREADS), LOSS_THREADS, 0, (cudaStream_t)stream>>>(p);
+    return check_launch("emer_ray_loss_live_bwd");
 }
 
 static CycleParams cycle_params(const float* f, int64_t ld_f, const float* b, int64_t ld_b, const float* fpb,

@@ -17,7 +17,8 @@ Differences from the op-by-op reference, all deliberate:
   * ``check_nan=True`` keeps the reference's NaN check, which reads the value on the host (a sync); the default
     configuration has it off.
   * A CUDA graph that captures a loss call bakes in its Python scalars (``coef``, ``coef_decay``, ``epsilon``): recapture
-    when they change (the line-of-sight ``epsilon`` decays every step in the reference's schedule).
+    when they change, or give ``LineOfSightLoss`` its ``epsilon`` and ``coef_decay`` as device constants
+    (``line_of_sight_consts``), which the kernels read when they run.
 """
 from __future__ import annotations
 
@@ -31,7 +32,7 @@ from torch import Tensor
 from . import _ops
 
 __all__ = ["normalize_depth", "Loss", "RealValueLoss", "SkyLoss", "DepthLoss", "LineOfSightLoss",
-           "DynamicRegularizationLoss", "dirac_delta_approx", "compute_line_of_sight_loss", "flow_cycle_loss"]
+           "DynamicRegularizationLoss", "line_of_sight_consts", "dirac_delta_approx", "compute_line_of_sight_loss", "flow_cycle_loss"]
 
 
 def _unsupported(what: str):
@@ -177,7 +178,11 @@ class DepthLoss(Loss):
 
 class LineOfSightLoss(Loss):
     """``coef * mean(coef_decay * compute_line_of_sight_loss(gt_depth, weights, t_vals, epsilon))``; ``pred_depth``
-    gets no gradient and ``t_vals`` is detached, as in the reference."""
+    gets no gradient and ``t_vals`` is detached, as in the reference.
+
+    ``epsilon`` may also be a float32 CUDA tensor holding ``line_of_sight_consts(epsilon, coef_decay)`` (then leave
+    ``coef_decay`` at 1): the kernels read the four values when they run, so a captured CUDA graph follows whatever
+    was last written there.  Value and gradient are bit-identical to the float call with the same two numbers."""
 
     def __init__(
         self,
@@ -212,7 +217,12 @@ class LineOfSightLoss(Loss):
         if self.loss_type != "my":
             raise NotImplementedError(f"Unknown loss type: {self.loss_type}")
         name = self.name if name is None else name
-        value = _ops.line_of_sight_loss(weights, t_vals, gt_depth, epsilon, pre=coef_decay, post=self.coef)
+        if torch.is_tensor(epsilon):
+            if coef_decay != 1.0:
+                raise ValueError("LineOfSightLoss: with device constants, coef_decay is their last value")
+            value = _ops.line_of_sight_loss(weights, t_vals, gt_depth, epsilon, post=self.coef)
+        else:
+            value = _ops.line_of_sight_loss(weights, t_vals, gt_depth, epsilon, pre=coef_decay, post=self.coef)
         return self._result(name, value)
 
 
@@ -274,6 +284,13 @@ def flow_cycle_loss(extras: Dict[str, Tensor], coef: float = 0.01,
     value, stats = _ops.cycle_loss(extras["forward_flow"], extras["backward_flow"],
                                    extras["forward_pred_backward_flow"], extras["backward_pred_forward_flow"], coef)
     return {name: value}, dict(zip(FLOW_STAT_KEYS, stats.unbind(0)))
+
+
+def line_of_sight_consts(epsilon: float, coef_decay: float = 1.0) -> list:
+    """The four fp32 values a live ``LineOfSightLoss`` call reads, ``[epsilon, 2 sigma^2, 1 / sqrt(2 pi sigma^2),
+    coef_decay]`` with ``sigma = epsilon / 3``, derived in double and rounded once, as the float call rounds them.
+    Copy them into a float32 CUDA tensor of 4 and pass that as ``epsilon``."""
+    return _ops.sight_consts(epsilon, coef_decay)
 
 
 def dirac_delta_approx(x, mu=0, sigma=1e-5):

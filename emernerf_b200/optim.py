@@ -140,6 +140,22 @@ class FusedAdam(torch.optim.Optimizer):
         self._touched.clear()
 
     # ------------------------------------------------------------------ the step
+    @staticmethod
+    def _sync_group_lr(group, g: _Group) -> None:
+        if group["lr"] != g.lr_host:
+            g.hyper[1].fill_(group["lr"])
+            g.lr_host = group["lr"]
+
+    @torch.no_grad()
+    def sync_lr(self) -> None:
+        """Write every group's ``lr`` to the device where the Adam kernel reads it, if it changed since the last write.
+        ``step()`` does this itself; a CUDA graph that captured ``step()`` does not (the write is a host decision), so
+        call this before each replay, and once before the capture, so that the capture records no write."""
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("FusedAdam.sync_lr: call it outside graph capture")
+        for group, g in zip(self.param_groups, self._groups):
+            self._sync_group_lr(group, g)
+
     @torch.no_grad()
     def step(self, closure=None):
         loss = None
@@ -151,9 +167,7 @@ class FusedAdam(torch.optim.Optimizer):
             active = tuple(i for i, p in enumerate(g.params) if id(p) in self._touched)
             if not active:
                 continue
-            if group["lr"] != g.lr_host:
-                g.hyper[1].fill_(group["lr"])
-                g.lr_host = group["lr"]
+            self._sync_group_lr(group, g)
             g.hyper[0].add_(1.0)
             lo, hi = 0, g.total
             if self.shard is not None:

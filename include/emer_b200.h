@@ -578,6 +578,14 @@ int emer_ray_loss_fwd(int kind, const float* w, const float* t, const float* gt,
 int emer_ray_loss_bwd(int kind, const float* w, const float* t, const float* gt, int64_t n_rays, int n_samples, float eps,
                       float two_sigma_sq, float amp, float pre, float post, const float* fwd_out, const float* g,
                       float* dw, void* stream);
+/* The same for LINE_OF_SIGHT and SIGHT, with the per-step constants read from device memory at kernel start:
+ * consts [4] fp32 = {eps, two_sigma_sq, amp, pre}.  A CUDA graph that captures these calls replays with whatever the
+ * caller last wrote there.  With the values the float entries receive, value and gradient are bit-identical to theirs. */
+int emer_ray_loss_live_fwd(int kind, const float* w, const float* t, const float* gt, int64_t n_rays, int n_samples,
+                           const float* consts, float post, float* out, void* workspace, void* stream);
+int emer_ray_loss_live_bwd(int kind, const float* w, const float* t, const float* gt, int64_t n_rays, int n_samples,
+                           const float* consts, float post, const float* fwd_out, const float* g, float* dw,
+                           void* stream);
 
 /* ---- the flow variants' cycle loss and flow statistics (replaces the inline block of train_emernerf.py:700-740)
  * f = forward_flow, b = backward_flow, fpb = forward_pred_backward_flow, bpf = backward_pred_forward_flow: each n rows
