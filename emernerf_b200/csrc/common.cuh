@@ -64,6 +64,22 @@ __device__ __forceinline__ float warp_scan_incl(float v, int lane) {
     return v;
 }
 
+__device__ __forceinline__ double warp_scan_incl(double v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        double t = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += t;
+    }
+    return v;
+}
+
+// exclusive warp scan (sum) from the inclusive one: the inclusive sum of the lane below.  Never incl - v: where v
+// outweighs the lanes below by 2^24 (a far interval's sigma * delta after near-empty space) that difference is 0.
+__device__ __forceinline__ float warp_scan_excl(float incl, int lane) {
+    const float below = __shfl_up_sync(0xffffffffu, incl, 1);
+    return lane == 0 ? 0.0f : below;
+}
+
 // inclusive warp scan from the top lane downwards (suffix sum)
 __device__ __forceinline__ float warp_scan_incl_rev(float v, int lane) {
 #pragma unroll

@@ -15,6 +15,9 @@
 //   term_k  = max(dq_k - dP_k, 0)^2 / (dP_k + 1e-5),  dP_k = prop_cdf_{k+1} - prop_cdf_k                 (:232-238)
 //   out: sum_k term_k (accumulated into *loss_sum), d(sum term)/d prop_cdf -> d_prop_cdf [R, n+1]
 // The caller divides by R n (the reference's .mean()) and applies the upstream gradient.
+// The row is computed in fp64 from the fp32 inputs: dq_k is a difference of neighbouring values of a cumulative area
+// that reaches ~1, and the hinge divides it by dP_k + 1e-5, so in fp32 the rounding of cdf_r alone (6e-8) put the
+// gradient of a fine level (pulse width 0.003) 4e-3 off its fp64 value.
 #include "common.cuh"
 
 namespace emer {
@@ -37,38 +40,38 @@ struct InterlevelParams {
 };
 
 __global__ void __launch_bounds__(IL_WARPS * 32) interlevel_loss_kernel(const InterlevelParams p) {
-    __shared__ float knot[IL_WARPS][IL_MAX_K + 2];
-    __shared__ float wv[IL_WARPS][IL_MAX_K + 2];       // the blurred heights w
-    __shared__ float cr[IL_WARPS][IL_MAX_K + 2];       // cdf of the blurred step function
-    __shared__ float qv[IL_WARPS][IL_MAX_K + 2];       // merged +-slope jumps; later the interpolated cdf at the proposal edges
+    __shared__ double knot[IL_WARPS][IL_MAX_K + 2];
+    __shared__ double wv[IL_WARPS][IL_MAX_K + 2];      // the blurred heights w
+    __shared__ double cr[IL_WARPS][IL_MAX_K + 2];      // cdf of the blurred step function
+    __shared__ double qv[IL_WARPS][IL_MAX_K + 2];       // merged +-slope jumps; later the interpolated cdf at the proposal edges
     static_assert(IL_MAX_K + 2 >= IL_MAX_N1, "qv holds both");
-    __shared__ float blk[IL_WARPS];
+    __shared__ double blk[IL_WARPS];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int m = p.m, n1 = p.n1, K = 2 * m;
-    const float r = p.r;
-    float loss = 0.0f;
+    const double r = p.r;
+    double loss = 0.0;
     for (int64_t ray = (int64_t)blockIdx.x * IL_WARPS + wid; ray < p.n_rays; ray += (int64_t)gridDim.x * IL_WARPS) {
         const float* s = p.s + ray * m;
         const float* c = p.cdf + ray * m;
         __syncwarp();
         // ---- merge s - r and s + r; the slope jump of knot j travels with it
         for (int j = lane; j < m; j += 32) {
-            const float sj = __ldg(s + j);
-            const float a = sj - r, b = sj + r;
-            const float y_hi = j < m - 1 ? (__ldg(c + j + 1) - __ldg(c + j)) / (__ldg(s + j + 1) - sj) : 0.0f;
-            const float y_lo = j > 0 ? (__ldg(c + j) - __ldg(c + j - 1)) / (sj - __ldg(s + j - 1)) : 0.0f;
-            const float slope = (y_hi - y_lo) / (2.0f * r);
+            const double sj = __ldg(s + j);
+            const double a = sj - r, b = sj + r;
+            const double y_hi = j < m - 1 ? ((double)__ldg(c + j + 1) - __ldg(c + j)) / (__ldg(s + j + 1) - sj) : 0.0;
+            const double y_lo = j > 0 ? ((double)__ldg(c + j) - __ldg(c + j - 1)) / (sj - __ldg(s + j - 1)) : 0.0;
+            const double slope = (y_hi - y_lo) / (2.0 * r);
             // rank of a_j: j + #{i: s_i + r < a_j};  rank of b_j: j + #{i: s_i - r <= b_j}
             int lo = 0, hi = m;
             while (lo < hi) {
                 const int mid = (lo + hi) >> 1;
-                if (__ldg(s + mid) + r < a) lo = mid + 1; else hi = mid;
+                if ((double)__ldg(s + mid) + r < a) lo = mid + 1; else hi = mid;
             }
             const int ra = j + lo;
             lo = 0; hi = m;
             while (lo < hi) {
                 const int mid = (lo + hi) >> 1;
-                if (__ldg(s + mid) - r <= b) lo = mid + 1; else hi = mid;
+                if ((double)__ldg(s + mid) - r <= b) lo = mid + 1; else hi = mid;
             }
             const int rb = j + lo;
             knot[wid][ra] = a; qv[wid][ra] = slope;
@@ -76,64 +79,64 @@ __global__ void __launch_bounds__(IL_WARPS * 32) interlevel_loss_kernel(const In
         }
         __syncwarp();
         // ---- heights: w_0 = 0, w_{i+1} = max(cumsum_i((knot_{i+1} - knot_i) * cumsum_i(dslope)), 0); areas -> cdf_r
-        float carry_s = 0.0f, carry_h = 0.0f, carry_a = 0.0f, w_prev_last = 0.0f;
+        double carry_s = 0.0, carry_h = 0.0, carry_a = 0.0, w_prev_last = 0.0;
         for (int i0 = 0; i0 < K - 1; i0 += 32) {
             const int i = i0 + lane;
             const bool ok = i < K - 1;
-            const float ds = ok ? qv[wid][i] : 0.0f;
-            const float dk = ok ? knot[wid][i + 1] - knot[wid][i] : 0.0f;
-            const float cs = carry_s + warp_scan_incl(ds, lane);
-            const float inc = dk * cs;
-            const float hs = carry_h + warp_scan_incl(inc, lane);
-            const float w_next = fmaxf(hs, 0.0f);                              // w_{i+1}
-            float w_cur = __shfl_up_sync(0xffffffffu, w_next, 1);              // w_i
+            const double ds = ok ? qv[wid][i] : 0.0;
+            const double dk = ok ? knot[wid][i + 1] - knot[wid][i] : 0.0;
+            const double cs = carry_s + warp_scan_incl(ds, lane);
+            const double inc = dk * cs;
+            const double hs = carry_h + warp_scan_incl(inc, lane);
+            const double w_next = fmax(hs, 0.0);                               // w_{i+1}
+            double w_cur = __shfl_up_sync(0xffffffffu, w_next, 1);             // w_i
             if (lane == 0) w_cur = w_prev_last;
-            const float area = ok ? 0.5f * (w_next + w_cur) * dk : 0.0f;
-            const float ca = carry_a + warp_scan_incl(area, lane);
+            const double area = ok ? 0.5 * (w_next + w_cur) * dk : 0.0;
+            const double ca = carry_a + warp_scan_incl(area, lane);
             if (ok) { wv[wid][i + 1] = w_next; cr[wid][i + 1] = ca; }
             carry_s = __shfl_sync(0xffffffffu, cs, 31);
             carry_h = __shfl_sync(0xffffffffu, hs, 31);
             carry_a = __shfl_sync(0xffffffffu, ca, 31);
             w_prev_last = __shfl_sync(0xffffffffu, w_next, 31);
         }
-        if (lane == 0) { wv[wid][0] = 0.0f; cr[wid][0] = 0.0f; }
+        if (lane == 0) { wv[wid][0] = 0.0; cr[wid][0] = 0.0; }
         __syncwarp();
         // ---- quadratic interpolation of cdf_r at the proposal edges
         const float* ps = p.prop_s + ray * n1;
         const float* pc = p.prop_cdf + ray * n1;
         for (int k = lane; k < n1; k += 32) {
-            const float x = __ldg(ps + k);
+            const double x = __ldg(ps + k);
             int lo = 0, hi = K;                                                // #{knots <= x}
             while (lo < hi) {
                 const int mid = (lo + hi) >> 1;
                 if (knot[wid][mid] <= x) lo = mid + 1; else hi = mid;
             }
             const int i_lo = max(lo - 1, 0), i_hi = min(lo, K - 1);
-            const float x_lo = knot[wid][i_lo], x_hi = knot[wid][i_hi];
-            const float p_lo = wv[wid][i_lo], p_hi = wv[wid][i_hi];
-            float f = (x - x_lo) / (x_hi - x_lo);
-            if (f != f) f = 0.0f;                                              // nan_to_num(., 0); +-inf clip below
-            f = fminf(fmaxf(f, 0.0f), 1.0f);
-            qv[wid][k] = cr[wid][i_lo] + (x - x_lo) * (p_lo + p_hi * f + p_lo * (1.0f - f)) / 2.0f;
+            const double x_lo = knot[wid][i_lo], x_hi = knot[wid][i_hi];
+            const double p_lo = wv[wid][i_lo], p_hi = wv[wid][i_hi];
+            double f = (x - x_lo) / (x_hi - x_lo);
+            if (f != f) f = 0.0;                                               // nan_to_num(., 0); +-inf clip below
+            f = fmin(fmax(f, 0.0), 1.0);
+            qv[wid][k] = cr[wid][i_lo] + (x - x_lo) * (p_lo + p_hi * f + p_lo * (1.0 - f)) / 2.0;
         }
         __syncwarp();
         // ---- terms and their derivative w.r.t. dP_k
-        float g_prev_last = 0.0f;                                              // g_{k0 - 1}
+        double g_prev_last = 0.0;                                              // g_{k0 - 1}
         for (int k0 = 0; k0 < n1; k0 += 32) {                                  // k = n1 - 1 only closes the gradient row
             const int k = k0 + lane;
-            float g = 0.0f;
+            double g = 0.0;
             if (k < n1 - 1) {
-                const float dq = qv[wid][k + 1] - qv[wid][k];
-                const float dp = __ldg(pc + k + 1) - __ldg(pc + k);
-                const float d = fmaxf(dq - dp, 0.0f);
-                const float den = dp + 1e-5f;
+                const double dq = qv[wid][k + 1] - qv[wid][k];
+                const double dp = (double)__ldg(pc + k + 1) - __ldg(pc + k);
+                const double d = fmax(dq - dp, 0.0);
+                const double den = dp + 1e-5;
                 loss += d * d / den;
-                g = -2.0f * d / den - (d * d) / (den * den);
+                g = -2.0 * d / den - (d * d) / (den * den);
             }
             if (p.d_prop_cdf) {
-                float g_prev = __shfl_up_sync(0xffffffffu, g, 1);
+                double g_prev = __shfl_up_sync(0xffffffffu, g, 1);
                 if (lane == 0) g_prev = g_prev_last;
-                if (k < n1) p.d_prop_cdf[ray * n1 + k] = g_prev - g;           // dP_{k-1} = P_k - P_{k-1}, dP_k = P_{k+1} - P_k
+                if (k < n1) p.d_prop_cdf[ray * n1 + k] = (float)(g_prev - g);          // dP_{k-1} = P_k - P_{k-1}, dP_k = P_{k+1} - P_k
                 g_prev_last = __shfl_sync(0xffffffffu, g, 31);
             }
         }
@@ -143,9 +146,9 @@ __global__ void __launch_bounds__(IL_WARPS * 32) interlevel_loss_kernel(const In
     if (lane == 0) blk[wid] = loss;
     __syncthreads();
     if (threadIdx.x == 0) {
-        float t = 0.0f;
+        double t = 0.0;
         for (int w = 0; w < IL_WARPS; ++w) t += blk[w];
-        if (t != 0.0f) atomicAdd(p.loss_sum, t);
+        if (t != 0.0) atomicAdd(p.loss_sum, (float)t);
     }
 }
 

@@ -176,7 +176,7 @@ __global__ void __launch_bounds__(PL_WARPS * 32, 2) prop_level_kernel(const Prop
             if (p.out_sigma) p.out_sigma[ray * n + k] = sigma;
         }
         const float incl = warp_scan_incl(xdelta, lane);
-        const float e_excl = carry + (incl - xdelta);
+        const float e_excl = carry + warp_scan_excl(incl, lane);
         if (ok) p.out_cdf[ray * (n + 1) + k] = 1.0f - expf(-e_excl);
         carry += __shfl_sync(0xffffffffu, incl, 31);
     }
@@ -255,7 +255,7 @@ __global__ void __launch_bounds__(PL_WARPS * 32) prop_level_bwd_kernel(const Pro
             float xdelta = 0.0f;
             if (ok) xdelta = __ldg(p.sigma + ray * n + k) * (t_edges[wid][k + 1] - t_edges[wid][k]);
             const float incl = warp_scan_incl(xdelta, lane);
-            const float e_excl = carry + (incl - xdelta);
+            const float e_excl = carry + warp_scan_excl(incl, lane);   // bit-identical to the forward
             if (ok) d_raw_s[wid][k] = __ldg(p.d_cdf + ray * (n + 1) + k) * expf(-e_excl);
             carry += __shfl_sync(0xffffffffu, incl, 31);
         }
@@ -267,7 +267,7 @@ __global__ void __launch_bounds__(PL_WARPS * 32) prop_level_bwd_kernel(const Pro
             const bool ok = k < n;
             const float v = ok ? d_raw_s[wid][k] : 0.0f;
             const float incl = warp_scan_incl(v, lane);
-            const float g_excl = tail + (incl - v);    // sum over the samples behind k
+            const float g_excl = tail + warp_scan_excl(incl, lane);    // sum over the samples behind k
             if (ok) {
                 const float sg = __ldg(p.sigma + ray * n + k);
                 d_raw_s[wid][k] = g_excl * (t_edges[wid][k + 1] - t_edges[wid][k]) * fminf(sg, 3269017.372472111f);   // e^15

@@ -111,7 +111,7 @@ def _fma32(a: Tensor, b: Tensor, c: Tensor) -> Tensor:
 
 def corner_indices_and_weights(x: Tensor, geom: GridGeometry, lvl: int):
     """x: [N, D] fp32. Returns (idx int64 [N, 2^D] absolute entry index, w fp32 [N, 2^D], frac [N,D], cell)."""
-    scale = torch.tensor(geom.scales[lvl], dtype=torch.float32)
+    scale = torch.tensor(geom.scales[lvl], dtype=torch.float32, device=x.device)
     pos = _fma32(scale.expand_as(x), x, torch.full_like(x, 0.5))
     fl = torch.floor(pos)
     frac = pos - fl

@@ -406,8 +406,9 @@ def test_fused_proposal_level_backward_vs_oracle(n_levels, n, R):
     """emer_prop_level_bwd (+ emer_grid_bwd for the scatter): gradient of a proposal level's CDF row w.r.t. the hash
     table and the 8->64->1 MLP, against autograd through the oracle's DensityField + transmittance on CPU
     (third_party/nerfacc_prop_net.py:161-170 -> render_utils.py:314-324 -> radiance_field.py:825-841 of the reference).
-    The forward of the training form is the no-grad kernel itself (bit-identical samples and CDF).  R = 2100 makes a
-    warp of the persistent kernel walk several rays (444 resident CTAs x 8 warps)."""
+    The forward of the training form is the no-grad kernel itself (bit-identical samples and CDF).  Every warp of the
+    persistent backward handles at most one ray at these sizes (2100 rays need 263 CTAs, fewer than 3 per SM);
+    test_gpu_prop_level_grad.py holds the rays-per-warp loop and the benchmark's 8192 rays to fp64."""
     from emernerf_b200 import _ops
     from emernerf_b200.radiance_fields import build_density_field
     from oracle import adapters

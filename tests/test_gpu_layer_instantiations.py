@@ -206,14 +206,15 @@ def elsewhere():
     """Template instantiations the case tables of other suites launch against their own references."""
     import test_gpu_field_chain
     import test_gpu_field_wgrad
+    import test_gpu_prop_level_grad
 
     out = {f"emer::ff::field_bwd_kernel<{k},{f}>": "test_gpu_field_chain.py" for k, f in test_gpu_field_chain.INSTANCES}
     out.update({f"emer::fw::field_wgrad_kernel<{c[0]},{int(c[3])}>": "test_gpu_field_wgrad.py"
                 for c in test_gpu_field_wgrad.CASES})
     out.update({f"emer::grid_indices_kernel<{d}>": "test_gpu_kernels.py::test_grid_corner_indices_bit_exact"
                 for d in (3, 4)})
-    out.update({f"emer::prop_level_bwd_kernel<{lf}>": "test_gpu_kernels.py::test_fused_proposal_level_backward_vs_oracle"
-                for lf in (4, 8)})
+    out.update({f"emer::prop_level_bwd_kernel<{c[0]}>": "test_gpu_prop_level_grad.py::test_level_backward_vs_fp64"
+                for c in test_gpu_prop_level_grad.CASES.values()})
     return out
 
 
