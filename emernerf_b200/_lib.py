@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_void_p
 
 from .grid_desc import EmerGridDesc
 
@@ -74,6 +74,21 @@ class EmerImageRaysIn(ctypes.Structure):
 class EmerImageRaysOut(ctypes.Structure):
     _fields_ = [(k, _P) for k in IMAGE_RAYS_OUT_PTRS]
 
+
+# host structs of emer_trajectory_rays (include/emer_b200.h): field names and order as there
+TRAJECTORY_RAYS_OUT_PTRS = ("origins", "viewdirs", "norms", "pixel_coords", "timestamps", "img_idx", "cam_idx",
+                            "sky_masks")
+
+
+class EmerTrajectoryRaysIn(ctypes.Structure):
+    _fields_ = [("c2w", _P), ("intrinsics", _P), ("timestamps", _P), ("n_images", c_int64), ("image_a", c_int64),
+                ("image_b", c_int64), ("cam_id", c_int64), ("offset", c_double * 3), ("frac_num", c_int32),
+                ("frac_den", c_int32), ("h", c_int32), ("w", c_int32), ("downscale", c_float)]
+
+
+class EmerTrajectoryRaysOut(ctypes.Structure):
+    _fields_ = [(k, _P) for k in TRAJECTORY_RAYS_OUT_PTRS]
+
 # number of kernels this library launched through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = 0
 
@@ -119,6 +134,7 @@ _SIGNATURES = {
     "emer_topk_ratio": [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P],
     "emer_pixel_batch": [POINTER(EmerPixelBatchIn), POINTER(EmerPixelBatchOut), _P],
     "emer_image_rays": [POINTER(EmerImageRaysIn), POINTER(EmerImageRaysOut), _P],
+    "emer_trajectory_rays": [POINTER(EmerTrajectoryRaysIn), POINTER(EmerTrajectoryRaysOut), _P],
     "emer_error_map": [_P, _P, _P, c_int64, _P, _P, _P],
     "emer_error_map_normalize": [_P, c_int64, _P, _P],
     "emer_adam_step": [_P, _P, c_int, c_int64, _P, c_float, c_float, c_float, c_float, c_int, _P],

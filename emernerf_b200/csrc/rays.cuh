@@ -1,5 +1,5 @@
-// The per-pixel arithmetic shared by gen_rays_kernel (raygen.cu), pixel_batch_kernel (raybatch.cu) and
-// image_rays_kernel (errormap.cu), so they produce the same values bit for bit.
+// The per-pixel arithmetic shared by gen_rays_kernel (raygen.cu), pixel_batch_kernel (raybatch.cu), image_rays_kernel
+// and trajectory_rays_kernel (errormap.cu), so they produce the same values bit for bit.
 //
 // The ray, in the reference's order (datasets/base/pixel_source.py:39-76; -fmad=false: every product and sum rounds
 // separately):
@@ -11,16 +11,18 @@
 
 namespace emer {
 
-// C: the camera's c2w [4, 4] (row-major, device memory); (fx, cx, fy, cy): its intrinsics; (px, py): the pixel.
-__device__ __forceinline__ void pixel_ray(const float* __restrict__ C, float fx, float cx, float fy, float cy, float px,
-                                          float py, float origin[3], float viewdir[3], float& nrm) {
+// at(e): element e of the camera's c2w ([4, 4] row-major; rows 0-2 are read), wherever it lives; (fx, cx, fy, cy): its
+// intrinsics; (px, py): the pixel.
+template <class At>
+__device__ __forceinline__ void pixel_ray_at(At at, float fx, float cx, float fy, float cy, float px, float py,
+                                             float origin[3], float viewdir[3], float& nrm) {
     const float cam[3] = {(px - cx + 0.5f) / fx, (py - cy + 0.5f) / fy, 1.0f};
     float d[3], sq = 0.0f;
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
-        float s = cam[0] * __ldg(C + r * 4 + 0);
-        s = s + cam[1] * __ldg(C + r * 4 + 1);
-        s = s + cam[2] * __ldg(C + r * 4 + 2);
+        float s = cam[0] * at(r * 4 + 0);
+        s = s + cam[1] * at(r * 4 + 1);
+        s = s + cam[2] * at(r * 4 + 2);
         d[r] = s;
         sq = sq + s * s;
     }
@@ -28,9 +30,15 @@ __device__ __forceinline__ void pixel_ray(const float* __restrict__ C, float fx,
     const float inv = nrm + 1e-8f;
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
-        origin[r] = __ldg(C + r * 4 + 3);
+        origin[r] = at(r * 4 + 3);
         viewdir[r] = d[r] / inv;
     }
+}
+
+// C: the camera's c2w [4, 4] (row-major, device memory).
+__device__ __forceinline__ void pixel_ray(const float* __restrict__ C, float fx, float cx, float fy, float cy, float px,
+                                          float py, float origin[3], float viewdir[3], float& nrm) {
+    pixel_ray_at([C](int e) { return __ldg(C + e); }, fx, cx, fy, cy, px, py, origin, viewdir, nrm);
 }
 
 // K: the camera's intrinsics [3, 3] (row-major, device memory).

@@ -14,6 +14,9 @@ replaces ``get_render_rays`` and ``update_pixel_error_maps``, and with ``refresh
 refresh of the training loop (``emer_image_rays``, ``emer_error_map`` and ``emer_error_map_normalize``,
 csrc/errormap.cu; INTEGRATION.md section 12).  ``LidarRaySampler`` also replaces the lidar sources' ``get_render_rays``
 with a frame table (INTEGRATION.md section 10).
+
+``CameraTrajectory`` renders the scene from cameras moving between the source's poses: a dataset for the reference's
+``render_pixels`` whose items come from one ``emer_trajectory_rays`` launch each (INTEGRATION.md section 14).
 """
 from __future__ import annotations
 
@@ -423,6 +426,110 @@ class PixelRaySampler:
             self._fold_error(data["pixels"], out["rgb"], out.get("dynamic_opacity") if decomposition else None,
                              maps[i])
         self._publish(maps)
+
+
+class CameraTrajectory:
+    """Render rays of cameras moving between the source's own poses: a dataset the reference's ``render_pixels`` and
+    ``render`` (radiance_fields/video_utils.py:50-468) take as it is, for new-view videos.
+
+    For each camera in ``cams`` (default: every camera of ``source.cam_ids``, in the order they first appear there),
+    the keyframes are that camera's images in increasing image index, the reference's timestep-major order.  With T
+    keyframes per camera and m = ``frames_per_keyframe``, each camera has ``num_frames = (T - 1) m + 1`` frames: frame
+    j lies in segment j // m at fraction (j % m) / m, so every m-th frame is a keyframe.  Item k is frame
+    k // len(cams) of camera cams[k % len(cams)], the layout of ``save_videos(..., num_timestamps=num_frames,
+    num_cams=len(cams))``.
+
+    ``traj[k]`` holds ``get_render_rays``' ray keys, in its order and with its ``[h, w, ...]`` shapes and dtypes, at the
+    source's current ``downscale_factor``: origins, viewdirs, direction_norm, pixel_coords, normed_timestamps (when the
+    source has timestamps), img_idx, cam_idx, and all-zero sky_masks when the source has sky masks (``render`` reads
+    them for the feature PCA).  The pose slerps the keyframes' rotations and lerps their origins, then moves the origin
+    by ``offset`` along the camera's own axes; the time is lerped.  ``img_idx`` is the nearer keyframe's, so the
+    per-image appearance embedding stays defined.  A keyframe with a zero offset is ``get_render_rays`` of that image
+    on every shared key.  Each item is one ``emer_trajectory_rays`` launch (csrc/errormap.cu) without a host sync; the
+    keyframes are found with one sync at construction."""
+
+    split = "trajectory"
+
+    def __init__(self, sampler: PixelRaySampler, cams=None, frames_per_keyframe: int = 1,
+                 offset=(0.0, 0.0, 0.0)):
+        if int(frames_per_keyframe) != frames_per_keyframe or frames_per_keyframe < 1:
+            raise ValueError(f"CameraTrajectory: frames_per_keyframe must be an integer >= 1, "
+                             f"got {frames_per_keyframe}")
+        offset = tuple(float(v) for v in offset)
+        if len(offset) != 3 or not all(np.isfinite(offset)):
+            raise ValueError(f"CameraTrajectory: the offset must be 3 finite numbers, got {offset}")
+        s = sampler.source
+        cam_ids = _dense(s.cam_ids, "cam_ids", torch.int64)
+        if cam_ids is None:
+            raise ValueError("CameraTrajectory: the keyframes need source.cam_ids")
+        _ops._need_cuda(cam_ids)
+        ids = cam_ids.tolist()                           # the one host sync
+        known = list(dict.fromkeys(ids))
+        n_cams = getattr(s, "num_cams", None)
+        cams = known if cams is None else [int(c) for c in cams]
+        keyframes = []
+        for c in cams:
+            if c not in known and not (n_cams is not None and 0 <= c < n_cams):
+                raise ValueError(f"CameraTrajectory: the source has no camera {c} (cameras {known})")
+            keys = [i for i, v in enumerate(ids) if v == c]
+            if not keys:
+                raise ValueError(f"CameraTrajectory: camera {c} has no image")
+            keyframes.append(keys)
+        if len({len(k) for k in keyframes}) > 1:
+            raise ValueError("CameraTrajectory: the cameras have different numbers of images: "
+                             + ", ".join(f"{c}: {len(k)}" for c, k in zip(cams, keyframes)))
+        self.sampler, self.cams, self.keyframes = sampler, cams, keyframes
+        self.frames_per_keyframe, self.offset = int(frames_per_keyframe), offset
+        self.num_frames = (len(keyframes[0]) - 1) * self.frames_per_keyframe + 1
+
+    def __len__(self) -> int:
+        return self.num_frames * len(self.cams)
+
+    def segment(self, k: int) -> Tuple[int, int, int, int]:
+        """(image a, image b, i, m) of item k: the frame lies between keyframes a and b at fraction i / m."""
+        frame, c = divmod(k, len(self.cams))
+        keys, m = self.keyframes[c], self.frames_per_keyframe
+        seg, i = divmod(frame, m)
+        if seg == len(keys) - 1:                        # the last keyframe
+            return keys[seg], keys[seg], 0, m
+        return keys[seg], keys[seg + 1], i, m
+
+    @torch.no_grad()
+    def __getitem__(self, k: int) -> Dict[str, Tensor]:
+        k = int(k)
+        if not -len(self) <= k < len(self):
+            raise IndexError(f"CameraTrajectory: item {k} out of range for {len(self)} items")
+        k %= len(self)
+        s = self.source
+        c2w, intr = _dense(s.cam_to_worlds, "cam_to_worlds"), _dense(s.intrinsics, "intrinsics")
+        times, sky = _dense(s.normalized_timestamps, "normalized_timestamps"), _dense(s.sky_masks, "sky_masks")
+        images = _dense(s.images, "images")
+        if images is None:
+            raise ValueError("CameraTrajectory: the frame size needs source.images")
+        _ops._need_cuda(c2w, intr, times, images)
+        d = float(s.downscale_factor)
+        h, w = self.sampler._images_at(images, d).shape[1:3]
+        a, b, i, m = self.segment(k)
+        f32, dev = dict(dtype=torch.float32, device=c2w.device), c2w.device
+        out = {"origins": torch.empty((h, w, 3), **f32), "viewdirs": torch.empty((h, w, 3), **f32),
+               "direction_norm": torch.empty((h, w, 1), **f32), "pixel_coords": torch.empty((h, w, 2), **f32)}
+        if times is not None:
+            out["normed_timestamps"] = torch.empty((h, w), **f32)
+        out["img_idx"] = torch.empty((h, w), dtype=torch.int64, device=dev)
+        out["cam_idx"] = torch.empty((h, w), dtype=torch.int64, device=dev)
+        if sky is not None:
+            out["sky_masks"] = torch.empty((h, w), **f32)
+        p = _ops._ptr
+        args_in = _lib.EmerTrajectoryRaysIn(p(c2w), p(intr), p(times), len(c2w), a, b, self.cams[k % len(self.cams)],
+                                            (ctypes.c_double * 3)(*self.offset), i, m, h, w, d)
+        names = dict(norms="direction_norm", timestamps="normed_timestamps")
+        args_out = _lib.EmerTrajectoryRaysOut(*(p(out.get(names.get(n, n))) for n in _lib.TRAJECTORY_RAYS_OUT_PTRS))
+        _lib.call("emer_trajectory_rays", ctypes.byref(args_in), ctypes.byref(args_out), _ops._stream())
+        return out
+
+    @property
+    def source(self):
+        return self.sampler.source
 
 
 class LidarRaySampler:

@@ -506,6 +506,42 @@ typedef struct EmerImageRaysOut {
  * at get_features' cell. */
 int emer_image_rays(const EmerImageRaysIn* in, const EmerImageRaysOut* out, void* stream);
 
+/* ---- render rays of a camera that moves between two keyframe images (csrc/errormap.cu; the producer of
+ *      raygen.CameraTrajectory's frames, a new-view counterpart of get_render_rays) -------------------------------- */
+/* Inputs: the source's full-size tables, as EmerImageRaysIn; timestamps may be NULL. */
+typedef struct EmerTrajectoryRaysIn {
+    const float* c2w;                         /* [N, 4, 4]                                                          */
+    const float* intrinsics;                  /* [N, 3, 3]                                                          */
+    const float* timestamps;                  /* [N]                                                                */
+    int64_t n_images;                         /* N                                                                  */
+    int64_t image_a, image_b;                 /* the keyframes of the segment                                       */
+    int64_t cam_id;                           /* written to cam_idx                                                 */
+    double offset[3];                         /* added to the origin along the camera's own axes (columns of c2w)   */
+    int32_t frac_num, frac_den;               /* the frame lies at f = frac_num / frac_den, 0 <= frac_num < frac_den */
+    int32_t h, w;                             /* rendered size                                                      */
+    float downscale;                          /* the source's downscale_factor d, as fp32: K * d                    */
+} EmerTrajectoryRaysIn;
+
+/* Outputs, [R = h * w] rows in (y, x) order; timestamps must be NULL when its input is, sky_masks may be NULL. */
+typedef struct EmerTrajectoryRaysOut {
+    float* origins;                           /* [R, 3]                                                             */
+    float* viewdirs;                          /* [R, 3]                                                             */
+    float* norms;                             /* [R, 1]                                                             */
+    float* pixel_coords;                      /* [R, 2] (y * (1/h), x * (1/w)), as emer_image_rays                 */
+    float* timestamps;                        /* [R] t_a + f (t_b - t_a) in fp32                                    */
+    int64_t* img_idx;                         /* [R] image_a when 2 frac_num <= frac_den, else image_b              */
+    int64_t* cam_idx;                         /* [R] cam_id                                                         */
+    float* sky_masks;                         /* [R] zeros                                                          */
+} EmerTrajectoryRaysOut;
+
+/* One launch, no allocation.  The pose: keyframe a's c2w bit for bit when frac_num == 0; otherwise the slerp of the two
+ * keyframes' rotations (as unit quaternions, q_b negated when q_a . q_b < 0; a normalised lerp when the dot exceeds
+ * 0.9995) and the lerp of their origins, in fp64, rounded to fp32.  Then origin += R offset (fp64, rounded), R the
+ * frame's rotation.  The intrinsics are keyframe a's times d.  Each pixel's ray and pixel coordinates are
+ * emer_image_rays' with that pose, so a frame with frac_num == 0 and a zero offset equals emer_image_rays of
+ * image a. */
+int emer_trajectory_rays(const EmerTrajectoryRaysIn* in, const EmerTrajectoryRaysOut* out, void* stream);
+
 /* workspace: at least EMER_ERRORMAP_WORKSPACE_BYTES of device memory, zeroed once by its owner and left zeroed by
  * emer_error_map_normalize (as the raybatch workspace above).  Between the two calls it holds the running minimum and
  * maximum of the map. */
