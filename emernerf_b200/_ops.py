@@ -937,7 +937,10 @@ class _GridEncodeRows(torch.autograd.Function):
         dx = None
         if need_x:
             dx = torch.empty((x.shape[0] - n0, x.shape[1]), dtype=torch.float32, device=x.device)
-            _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(x[n0:]), _ptr(params), _ptr(dy[n0:]), _ptr(None),
+            # the kernel loads rows with vector instructions: a half that starts off a 16-byte boundary (an odd n0 with
+            # 12-byte rows of x, or rows of dy that are not a multiple of 16 bytes) is copied
+            xv, dyv = (t if t.data_ptr() % 16 == 0 else t.clone() for t in (x[n0:], dy[n0:]))
+            _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(xv), _ptr(params), _ptr(dyv), _ptr(None),
                       _ptr(dx), dx.shape[0], _stream())
         if sink is not None:
             sink[1]()

@@ -22,7 +22,10 @@
 // level are issued back to back (16-byte LDG for F=4) before the first use; for F = 4 a lane pair
 // fetches the two x-neighbour corners of a cell in one load instruction (gather_corner_pairs), and
 // the scatter reduces them in one instruction where a warp has no same-cell runs.  The input
-// gradient (never needed in training) stays one thread per point, all levels.
+// gradient stays one thread per point, all levels.  The flow variants train through it: their loss reaches the flow
+// field through the dynamic and flow grids' input gradients at the flow-warped points (grid_encode_rows and
+// grid_encode in RadianceField._flow_branch, the encoders in temporal_aggregation); the static and dynamic-only
+// fields never request it.
 #include "common.cuh"
 #include "grid_common.cuh"
 

@@ -134,6 +134,62 @@ def corner_indices_and_weights(x: Tensor, geom: GridGeometry, lvl: int):
     return torch.stack(idxs, -1), torch.stack(ws, -1), frac, cell
 
 
+def grid_input_grad64(x: Tensor, params: Tensor, dy: Tensor, geom: GridGeometry):
+    """float64 input gradient of the encoding at the fp32 positions x [N, D], on x's device: per level
+    s_c = <dy_l, table[idx_c]> and dx_d += scale_l sum_{c: bit d clear} prod_{e != d} w_e (s_{c|d} - s_c), with w_e the
+    fraction or one minus it as bit e of c says.  Cells, fractions and indices are those of
+    :func:`corner_indices_and_weights` (the kernels' own: the derivative jumps at cell faces).
+
+    Returns (dx, mag), both [N, D] float64.  mag_d is the same sum over |dy_l| . |table[idx]| of both corners of each
+    difference: it bounds every partial result an fp32 evaluation of dx_d forms, so an error bound is a multiple of it."""
+    N, D, F = x.shape[0], geom.n_dims, geom.n_feat
+    table = params.detach().double().view(-1, F)
+    dyl = dy.detach().double().view(N, geom.n_levels, F)
+    dx = torch.zeros(N, D, dtype=torch.float64, device=x.device)
+    mag = torch.zeros_like(dx)
+    for lvl in range(geom.n_levels):
+        idx, _, frac, _ = corner_indices_and_weights(x, geom, lvl)
+        fr = frac.double()
+        v = table[idx]                                          # [N, 2^D, F]
+        g = dyl[:, lvl, None, :]
+        s = (v * g).sum(-1)
+        a = (v.abs() * g.abs()).sum(-1)
+        for d in range(D):
+            for c in range(1 << D):
+                if (c >> d) & 1:
+                    continue
+                t = torch.full_like(fr[:, 0], geom.scales[lvl])
+                for e in range(D):
+                    if e != d:
+                        t = t * (fr[:, e] if (c >> e) & 1 else 1.0 - fr[:, e])
+                hi = c | (1 << d)
+                dx[:, d] += t * (s[:, hi] - s[:, c])
+                mag[:, d] += t * (a[:, hi] + a[:, c])
+    return dx, mag
+
+
+def grid_table_grad64(x: Tensor, dy: Tensor, geom: GridGeometry):
+    """float64 table gradient of the encoding at the fp32 positions x [N, D], on x's device: sum over rows of w_c dy_l
+    into entry idx_c, with the fp32 corner weights the kernels use.  Returns (grad, mag, count) over the flat parameter
+    vector: mag sums |w_c dy_l|, count the contributions each entry receives (its fp32 sum has count - 1 additions)."""
+    N, F = x.shape[0], geom.n_feat
+    dyl = dy.detach().double().view(N, geom.n_levels, F)
+    n_entries = geom.offsets[-1]
+    grad = torch.zeros(n_entries, F, dtype=torch.float64, device=x.device)
+    mag = torch.zeros_like(grad)
+    count = torch.zeros(n_entries, dtype=torch.float64, device=x.device)
+    for lvl in range(geom.n_levels):
+        idx, w, _, _ = corner_indices_and_weights(x, geom, lvl)
+        g = dyl[:, lvl]
+        live = (g != 0).any(-1).double()                        # a row with a zero gradient adds nothing
+        for c in range(idx.shape[1]):
+            t = w[:, c : c + 1].double() * g
+            grad.index_add_(0, idx[:, c], t)
+            mag.index_add_(0, idx[:, c], t.abs())
+            count.index_add_(0, idx[:, c], live)
+    return grad.view(-1), mag.view(-1), count[:, None].expand(-1, F).reshape(-1)
+
+
 def grid_forward(x: Tensor, params: Tensor, geom: GridGeometry, fused: bool = True) -> Tensor:
     """[N, D] -> [N, L*F].  Differentiable w.r.t. ``params`` and ``x`` (through the weights,
     matching tcnn's dy_dx: derivative of the D-linear weights times ``scale``)."""

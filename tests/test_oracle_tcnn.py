@@ -60,3 +60,42 @@ def test_input_gradient_is_scale_times_finite_difference():
         fd = (tcnn_ref.grid_forward(xp, params, g).sum(-1) - tcnn_ref.grid_forward(xm, params, g).sum(-1)) / (2 * eps)
         ok = (fd - gx[:, d]).abs() < 5e-2 * gx[:, d].abs().clamp_min(1.0)
         assert ok.float().mean() > 0.9     # cells crossed by the +-eps stencil are the exceptions
+
+
+def test_fp64_grid_gradients_match_autograd():
+    """grid_input_grad64 / grid_table_grad64, the float64 references of the GPU input-gradient tests, against float64
+    autograd of the interpolation at the same cells and fractions, on a dense + hashed 4-D grid, a 3-D F = 1 grid and
+    the dynamic grid; levels with a zero upstream gradient included."""
+    for D, args in ((4, (3, 4, 24, 9, 2)), (3, (4, 16, 96, 12, 1)), (4, (10, 32, 8192, 18, 4))):
+        geom = tcnn_ref.grid_geometry(D, hotpath.hash_encoder_config(*args))
+        L, F = geom.n_levels, geom.n_feat
+        gen = torch.Generator().manual_seed(D * 100 + L)
+        x = torch.rand(500, D, generator=gen)
+        x[:50] = x[:50].round()
+        params = torch.randn(geom.n_params, generator=gen)
+        dy = torch.randn(500, L * F, generator=gen)
+        dy[::3, :F] = 0.0
+        dx, mag = tcnn_ref.grid_input_grad64(x, params, dy, geom)
+        tab, tmag, count = tcnn_ref.grid_table_grad64(x, dy, geom)
+
+        table = params.double().view(-1, F).requires_grad_(True)
+        dyl = dy.double().view(500, L, F)
+        loss, fracs = 0.0, []
+        for lvl in range(L):
+            idx, _, frac, _ = tcnn_ref.corner_indices_and_weights(x, geom, lvl)
+            fr = frac.double().requires_grad_(True)
+            fracs.append(fr)
+            for c in range(1 << D):
+                w = torch.ones_like(fr[:, 0])
+                for d in range(D):
+                    w = w * (fr[:, d] if (c >> d) & 1 else 1.0 - fr[:, d])
+                loss = loss + (w[:, None] * table[idx[:, c]] * dyl[:, lvl]).sum()
+        g_table, *g_frac = torch.autograd.grad(loss, [table] + fracs)
+        want = sum(geom.scales[lvl] * g for lvl, g in enumerate(g_frac))
+        assert (dx - want).abs().max() <= 1e-12 * want.abs().max()
+        assert (mag >= dx.abs()).all() and (mag > 0).all()
+        # the table reference weights with the kernels' fp32 corner weights: 2^-24 relative of the products
+        assert (tab - g_table.view(-1)).abs().max() <= 1e-6 * g_table.abs().max()
+        assert (tmag >= tab.abs()).all()
+        live = sum(int((dyl[:, lvl] != 0).any(-1).sum()) for lvl in range(L))
+        assert count.sum() == live * (1 << D) * F
