@@ -73,6 +73,16 @@ __device__ __forceinline__ double warp_scan_incl(double v, int lane) {
     return v;
 }
 
+// inclusive warp scan (minimum)
+__device__ __forceinline__ float warp_scan_min(float v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        float t = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v = fminf(v, t);
+    }
+    return v;
+}
+
 // exclusive warp scan (sum) from the inclusive one: the inclusive sum of the lane below.  Never incl - v: where v
 // outweighs the lanes below by 2^24 (a far interval's sigma * delta after near-empty space) that difference is 0.
 __device__ __forceinline__ float warp_scan_excl(float incl, int lane) {
@@ -88,6 +98,13 @@ __device__ __forceinline__ float warp_scan_incl_rev(float v, int lane) {
         if (lane + o < 32) v += t;
     }
     return v;
+}
+
+// exclusive suffix sum from the inclusive one: the inclusive suffix sum of the lane above (0 on lane 31), for the same
+// reason as warp_scan_excl -- an opaque sample's term can outweigh the suffix behind it by 2^24.
+__device__ __forceinline__ float warp_scan_excl_rev(float incl_rev, int lane) {
+    const float above = __shfl_down_sync(0xffffffffu, incl_rev, 1);
+    return lane == 31 ? 0.0f : above;
 }
 
 // Layer activations (EMER_ACT_*); the backward takes the stored OUTPUT y.

@@ -39,7 +39,10 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32) composite_fwd_kernel(
         if (ok) {
             if (weights) weights[base + s] = w;
             if (trans) trans[base + s] = T;
-            if (cdf) cdf[ray * (S + 1) + s] = 1.0f - T;
+        }
+        if (cdf) {                      // uniform across the warp
+            const float Tm = scan.monotone(T, lane);
+            if (ok) cdf[ray * (S + 1) + s] = 1.0f - Tm;
         }
     }
     float op, dep, med;
@@ -103,7 +106,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32) composite_bwd_kernel(
         const float G = gw + g_opraw + g_D * mid;
         const float q = ok ? fmaf(G, w, gT * T) : 0.0f;
         const float suf_incl = warp_scan_incl_rev(q, lane);
-        const float suffix_excl = carry + (suf_incl - q);
+        const float suffix_excl = carry + warp_scan_excl_rev(suf_incl, lane);
         const float ex = expf(-(sg * delta));
         const float dx = G * T * ex - suffix_excl;
         if (ok) dsigma[base + s] = dx * delta;

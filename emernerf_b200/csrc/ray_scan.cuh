@@ -13,6 +13,7 @@ template <bool MEDIAN>
 struct RayScan {
     float carry_e = 0.0f;     // sum of sigma*delta before this chunk
     float carry_w = 0.0f;     // sum of weights before this chunk
+    float carry_t = 1.0f;     // monotone(): the smallest transmittance before this chunk
     float sum_w = 0.0f, sum_wm = 0.0f;
     float med = 0.0f;
     bool med_found = false;
@@ -22,7 +23,7 @@ struct RayScan {
     __device__ __forceinline__ float step(float a, float b, float sg, bool ok, int s0, int S, int lane, float& T) {
         const float x = ok ? sg * (b - a) : 0.0f;
         const float incl = warp_scan_incl(x, lane);
-        const float e_excl = carry_e + (incl - x);
+        const float e_excl = carry_e + warp_scan_excl(incl, lane);
         T = expf(-e_excl);
         const float alpha = 1.0f - expf(-x);
         const float w = ok ? T * alpha : 0.0f;
@@ -46,6 +47,16 @@ struct RayScan {
         sum_wm = fmaf(w, mid, sum_wm);
         carry_e += __shfl_sync(0xffffffffu, incl, 31);
         return w;
+    }
+
+    // after step(), on every lane of the chunk: the running minimum of T along the ray, for the CDF 1 - T.  The scans
+    // of two neighbouring lanes are different trees and can invert by an ulp where a sample adds (next to) nothing, so
+    // T itself may rise by an ulp and the CDF would fall.  The minimum is some T_j, j <= i, whose prefix and error
+    // bound are no larger than sample i's, so it stays within T_i's bound.
+    __device__ __forceinline__ float monotone(float T, int lane) {
+        const float m = fminf(warp_scan_min(T, lane), carry_t);
+        carry_t = __shfl_sync(0xffffffffu, m, 31);
+        return m;
     }
 
     // on every lane after the last chunk: opacity clamped to [1e-6, 1], depth = sum w*mid / opacity, median depth

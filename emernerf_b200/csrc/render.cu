@@ -370,7 +370,7 @@ __global__ void __launch_bounds__(RENDER_WARPS * 32) render_bwd_kernel(const eme
         const float G = gw + gx + g_opraw + g_D * mid;
         const float q = ok ? fmaf(G, w, gT * T) : 0.0f;
         const float suf_incl = warp_scan_incl_rev(q, lane);
-        const float suffix_excl = carry + (suf_incl - q);
+        const float suffix_excl = carry + warp_scan_excl_rev(suf_incl, lane);
         const float ex = expf(-(sg * delta));
         const float dx = G * T * ex - suffix_excl;
         if (ok) {

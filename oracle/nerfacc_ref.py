@@ -82,6 +82,80 @@ def accumulate_along_rays(
     return torch.sum(src, dim=-2)
 
 
+def warp_sum32(v: Tensor) -> Tensor:
+    """The fp32 ray sum of the compositing kernels (csrc/ray_scan.cuh, csrc/composite.cu pass 1), bit for bit: lane l
+    adds v[s] for s = l, l + 32, ... in order, then the xor butterfly over 16, 8, 4, 2, 1 lanes.  [R, S] -> [R]."""
+    r, s = v.shape
+    ch = (s + 31) // 32
+    pad = torch.zeros((r, ch * 32), dtype=torch.float32)
+    pad[:, :s] = v.float()
+    pad = pad.reshape(r, ch, 32)
+    acc = torch.zeros((r, 32), dtype=torch.float32)
+    for c in range(ch):
+        acc = acc + pad[:, c]
+    lane = torch.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        acc = acc + acc[:, lane ^ o]
+    return acc[:, 0]
+
+
+def composite64(t0: Tensor, t1: Tensor, sigma: Tensor, weights32: Optional[Tensor] = None,
+                g_w: Optional[Tensor] = None, g_t: Optional[Tensor] = None, g_o: Optional[Tensor] = None,
+                g_d: Optional[Tensor] = None, g_cdf: Optional[Tensor] = None) -> dict:
+    """Volume compositing of fp32 rays [R, S] in float64, with the discrete choices of emer_composite_fwd / _bwd.
+
+    The interval length and midpoint are the kernel's fp32 ones, delta = fl(t1 - t0), mid = fl(fl(t0 + t1) / 2); from
+    there on everything is float64: x = sigma delta, E_i = sum_{j<i} x_j, T = exp(-E), alpha = 1 - exp(-x), w = T alpha,
+    opacity = clamp(sum w, 1e-6, 1), depth = sum w mid / opacity, cdf = 1 - cat(T, 0), the median (first sample whose
+    cumulative weight reaches 0.5, else the last).  The opacity clamp is a branch: with ``weights32`` (the kernel's own
+    weights) the branch is the kernel's, decided on ``warp_sum32`` of them; otherwise on the float64 sum.
+
+    Given upstream gradients (None for absent ones) the backward runs by autograd on this graph, the weights retaining
+    their gradient G (the total gradient reaching w_i).  Returned alongside, for error bounds: ``E``, ``wmid_abs`` =
+    sum |w mid|, ``G``, ``gT`` (the gradient reaching T directly: g_t - g_cdf[:, :S]), ``A`` = |G| T exp(-x) and
+    ``B`` = sum_{k>i} (|G_k| w_k + |gT_k| T_k)."""
+    f64 = torch.float64
+    delta32 = t1.float() - t0.float()
+    mid = ((t0.float() + t1.float()) / 2.0).to(f64)
+    delta = delta32.to(f64)
+    sig = sigma.to(f64).clone().requires_grad_(True)
+    x = sig * delta
+    E = exclusive_sum(x)
+    T = torch.exp(-E)
+    alpha = 1.0 - torch.exp(-x)
+    w = T * alpha
+    w.retain_grad()
+    sw = w.sum(-1, keepdim=True)
+    sw_branch = warp_sum32(weights32)[:, None].to(f64) if weights32 is not None else sw.detach()
+    in_range = (sw_branch >= 1e-6) & (sw_branch <= 1.0)
+    op = torch.where(in_range, sw, sw_branch.clamp(1e-6, 1.0))
+    depth = (w * mid).sum(-1, keepdim=True) / op
+    cdf = 1.0 - torch.cat([T, torch.zeros_like(T[:, :1])], -1)
+    cw = torch.cumsum(w.detach(), -1)
+    S = sigma.shape[-1]
+    med_idx = torch.searchsorted(cw, torch.full_like(cw[:, :1], 0.5), side="left").clamp(0, S - 1)
+    out = {"weights": w, "trans": T, "opacity": op, "depth": depth, "cdf": cdf, "median_idx": med_idx[:, 0],
+           "median_depth": mid.gather(-1, med_idx), "cw": cw, "in_range": in_range[:, 0], "delta": delta, "mid": mid,
+           "x": x.detach(), "E": E.detach(), "wmid_abs": (w * mid).abs().sum(-1, keepdim=True).detach()}
+    ups = [(w, g_w), (T, g_t), (op, g_o), (depth, g_d), (cdf, g_cdf)]
+    ups = [(o, g.to(f64)) for o, g in ups if g is not None]
+    if ups:
+        torch.autograd.backward([o for o, _ in ups], [g for _, g in ups])
+        G = w.grad if w.grad is not None else torch.zeros_like(w)
+        gT = torch.zeros_like(T)
+        if g_t is not None:
+            gT = gT + g_t.to(f64)
+        if g_cdf is not None:
+            gT = gT - g_cdf[:, :S].to(f64)
+        wd, Td = w.detach(), T.detach()
+        q = G.abs() * wd + gT.abs() * Td
+        out.update(dsigma=sig.grad if sig.grad is not None else torch.zeros_like(sig), G=G, gT=gT,
+                   A=G.abs() * Td * torch.exp(-x.detach()),
+                   B=torch.flip(exclusive_sum(torch.flip(q, [-1])), [-1]))
+    out = {k: v.detach() if isinstance(v, Tensor) else v for k, v in out.items()}
+    return out
+
+
 def importance_sampling_bins(cdfs: Tensor, n: int, bias: Tensor):
     """Shared arithmetic of ``importance_sampling``: for every output edge k in [0, n]
     returns (u [R, n+1] fp32, p0, p1 int64) with
