@@ -10,7 +10,7 @@ from __future__ import annotations
 import ctypes
 import math
 import weakref
-from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
+from typing import Callable, Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import torch
 from torch import Tensor
@@ -72,34 +72,68 @@ def _need_cuda(*ts: Tensor) -> None:
 # -- instead of allocating and zero-filling a fresh tensor that autograd would then copy or add: for the 122 MB hash
 # table that is a 122 MB memset per backward.  It returns None for that input (autograd has nothing left to do) and
 # tells the optimizer the parameter was touched.  Without a registered sink (the reference's own torch.optim.Adam) the
-# ordinary autograd path runs.
-_GRAD_SINKS: Dict[int, Tuple[Tensor, Callable, "weakref.ref"]] = {}
+# ordinary autograd path runs.  Every op looks its sinks up in forward, and its backward goes through _grad_bufs and
+# _grad_outputs.
+class _Sink(NamedTuple):
+    buf: Tensor                         # the parameter's contiguous fp32 slice of the optimizer's gradient buffer
+    touch: Callable[[], None]           # tells the optimizer the parameter received a gradient
+    touched: Callable[[], bool]         # whether it has received one since the optimizer last consumed its gradient
 
 
-def register_grad_sink(param: Tensor, sink: Tensor, on_touch: Callable) -> None:
+_GRAD_SINKS: Dict[int, Tuple[Tensor, "weakref.ref", Callable[[Tensor], None], Callable[[Tensor], bool]]] = {}
+
+
+def _always_touched(param: Tensor) -> bool:
+    return True
+
+
+def register_grad_sink(param: Tensor, sink: Tensor, mark: Callable[[Tensor], None],
+                       touched: Callable[[Tensor], bool] = _always_touched) -> None:
+    """Library backward passes accumulate ``param``'s gradient into ``sink`` and then call ``mark(param)``;
+    ``touched(param)`` answers whether ``mark`` was called since the optimizer last consumed the gradient.  Without
+    ``touched`` the parameter always counts as touched: nothing clears its sink, gradients are only ever added."""
     if sink.shape != param.shape or sink.dtype != torch.float32 or not sink.is_contiguous():
         raise ValueError("grad sink must be a contiguous fp32 tensor of the parameter's shape")
-    _GRAD_SINKS[param.data_ptr()] = (sink, on_touch, weakref.ref(param))
+    _GRAD_SINKS[param.data_ptr()] = (sink, weakref.ref(param), mark, touched)
 
 
 def clear_grad_sinks() -> None:
     _GRAD_SINKS.clear()
 
 
-def _grad_sink(t: Optional[Tensor]):
-    """(sink, touch) for a registered parameter's storage, else None."""
+def _grad_sink(t: Optional[Tensor]) -> Optional[_Sink]:
+    """The sink of the registered parameter whose storage ``t`` is, else None (also when that parameter is gone or
+    its address or shape changed: another tensor now lives there)."""
     if t is None or not _GRAD_SINKS:
         return None
     e = _GRAD_SINKS.get(t.data_ptr())
     if e is None:
         return None
-    sink, on_touch, ref = e
+    sink, ref, mark, touched = e
     p = ref()
     if p is None or p.data_ptr() != t.data_ptr() or sink.shape != t.shape:
         return None
-    touched = getattr(on_touch, "__self__", None)
-    is_touched = (lambda: id(p) in touched._touched) if hasattr(touched, "_touched") else None
-    return sink, (lambda: on_touch(p)), is_touched
+    return _Sink(sink, lambda: mark(p), lambda: touched(p))
+
+
+def _grad_bufs(shapes: Sequence[Optional[Sequence[int]]], sinks: Sequence[Optional[_Sink]],
+               device) -> List[Optional[Tensor]]:
+    """Where a backward's kernels accumulate each parameter gradient: the parameter's sink, else zeros of its shape;
+    None where ``shapes`` has None (no gradient wanted)."""
+    return [None if shape is None else s.buf if s is not None else torch.zeros(shape, dtype=torch.float32, device=device)
+            for shape, s in zip(shapes, sinks)]
+
+
+def _grad_outputs(bufs: Sequence[Optional[Tensor]], sinks: Sequence[Optional[_Sink]]) -> List[Optional[Tensor]]:
+    """After the launches that filled ``bufs``: what autograd receives -- None for a sink, which is marked touched
+    (autograd has nothing left to do), the filled buffer for any other parameter."""
+    out = []
+    for b, s in zip(bufs, sinks):
+        if b is not None and s is not None:
+            s.touch()
+            b = None
+        out.append(b)
+    return out
 
 
 # ----------------------------------------------------------------------------- weight gradients on a side stream
@@ -188,7 +222,7 @@ class _GridEncode(torch.autograd.Function):
         y = torch.empty((n, desc.n_output_dims), dtype=torch.float32, device=x.device)
         _lib.call("emer_grid_fwd", ctypes.byref(desc.c), _ptr(x), _ptr(params), _ptr(y), n, _stream())
         ctx.save_for_backward(x, params)
-        ctx.desc = desc
+        ctx.desc, ctx.sinks = desc, [_grad_sink(params)]
         return y
 
     @staticmethod
@@ -199,19 +233,12 @@ class _GridEncode(torch.autograd.Function):
         desc = ctx.desc
         dy = _f32c(dy)
         need_x, need_p = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        sink = _grad_sink(params) if need_p else None
-        if sink is not None:
-            dparams = sink[0]                     # the optimizer's pre-zeroed slice: scatter straight into it
-        else:
-            dparams = torch.zeros_like(params) if need_p else None
+        (dparams,) = _grad_bufs([params.shape if need_p else None], ctx.sinks, x.device)
         dx = torch.empty_like(x) if need_x else None
         if need_x or need_p:
             _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(x), _ptr(params), _ptr(dy), _ptr(dparams),
                       _ptr(dx), x.shape[0], _stream())
-        if sink is not None:
-            sink[1]()
-            dparams = None
-        return dx, dparams, None
+        return (dx, *_grad_outputs([dparams], ctx.sinks), None)
 
 
 def grid_encode(x: Tensor, params: Tensor, desc: GridDesc) -> Tensor:
@@ -356,34 +383,32 @@ def _layer_fwd(x2: Tensor, ldx: int, w: Tensor, b: Optional[Tensor], y: Tensor, 
 
 
 def _layer_bwd_data(dz: Tensor, lddz: int, w: Tensor, dx: Tensor, lddx: int, n: int,
-                    relu_src: Optional[Tensor], ld_relu: int, relu_cols: int) -> None:
-    """dx[n, k] = dz[n, n_out] @ w, then dx[:, :relu_cols] *= (relu_src > 0) (the dZ of the layer below)."""
+                    relu_src: Optional[Tensor], ld_relu: int, relu_cols: int, accumulate: bool = False) -> None:
+    """dx[n, k] = dz[n, n_out] @ w (``accumulate``: dx +=), then dx[:, :relu_cols] *= (relu_src > 0) (the dZ of the
+    layer below)."""
     n_out, k = w.shape
     if _narrow_ok(k, n_out):
+        if accumulate:
+            raise ValueError(f"_layer_bwd_data: the narrow kernel ({n_out} x {k}) has no accumulating form")
         _lib.call("emer_linear_narrow_bwd_data", _ptr(dz), lddz, _ptr(w), _ptr(dx), lddx, _ptr(relu_src), ld_relu,
                   relu_cols, n, k, n_out, _stream())
     elif _tc_rows_ok(n) and _tc_fits(n_out, k):
         _lib.call("emer_linear_tc_bwd_data", _ptr(dz), lddz, None, 0, ACT_NONE, _ptr(w), _ptr(dx), lddx,
-                  _ptr(relu_src), ld_relu, relu_cols, n, k, n_out, 0, _stream())
+                  _ptr(relu_src), ld_relu, relu_cols, n, k, n_out, int(accumulate), _stream())
     else:
-        _lib.call("emer_linear_bwd_data", _ptr(dz), lddz, None, 0, ACT_NONE, _ptr(w), _ptr(dx), lddx, n, k, n_out, 0,
-                  _stream())
+        _lib.call("emer_linear_bwd_data", _ptr(dz), lddz, None, 0, ACT_NONE, _ptr(w), _ptr(dx), lddx, n, k, n_out,
+                  int(accumulate), _stream())
         if relu_src is not None:
             dx[:, :relu_cols].mul_(relu_src[:, :relu_cols] > 0)
 
 
 def _layer_bwd_weight(x2: Tensor, ldx: int, dz: Tensor, lddz: int, w: Tensor, has_bias: bool, n: int,
-                      w_sink=None, b_sink=None):
+                      w_sink: Optional[_Sink] = None, b_sink: Optional[_Sink] = None):
     """(dW, db) of one layer.  With gradient sinks (``_grad_sink`` of the weight / bias parameter) the kernels
     accumulate into the optimizer's buffers and the returned entries are None."""
     n_out, k = w.shape
-    dw = w_sink[0] if w_sink is not None else torch.zeros_like(w)
-    if not has_bias:
-        db = None
-    elif b_sink is not None:
-        db = b_sink[0]
-    else:
-        db = torch.zeros(n_out, dtype=torch.float32, device=w.device)
+    sinks = (w_sink, b_sink)
+    dw, db = _grad_bufs((w.shape, (n_out,) if has_bias else None), sinks, w.device)
     tc = (_tc_rows_ok(n) and LINEAR_WGRAD_IMPL != "simt" and _tc_wgrad_fits(k, n_out) and n_out % 4 == 0
           and _aligned(x2, ldx) and _aligned(dz, lddz) and _pad4(k) <= ldx)
     if _narrow_ok(k, n_out):
@@ -395,13 +420,7 @@ def _layer_bwd_weight(x2: Tensor, ldx: int, dz: Tensor, lddz: int, w: Tensor, ha
     else:
         _lib.call("emer_linear_bwd_weight", _ptr(x2), ldx, _ptr(dz), lddz, None, 0, ACT_NONE, _ptr(dw), _ptr(db), n, k,
                   n_out, _stream())
-    if w_sink is not None:
-        w_sink[1]()
-        dw = None
-    if has_bias and b_sink is not None:
-        b_sink[1]()
-        db = None
-    return dw, db
+    return tuple(_grad_outputs((dw, db), sinks))
 
 
 class _MLPChain(torch.autograd.Function):
@@ -658,11 +677,83 @@ CHAIN_BWD = os.environ.get("EMER_CHAIN_BWD", "fused")          # "layers": data 
 CHAIN_K_ENC = (32, 40, 64)
 
 
-def _tc_bwd_data_acc(dz: Tensor, lddz: int, w: Tensor, dx: Tensor, lddx: int, n: int) -> None:
-    """dx[n, k] += dz[n, n_out] @ w on the tensor-core layer kernel (accumulating form)."""
-    n_out, k = w.shape
-    _lib.call("emer_linear_tc_bwd_data", _ptr(dz), lddz, None, 0, ACT_NONE, _ptr(w), _ptr(dx), lddx, None, 0, 0, n, k,
-              n_out, 1, _stream())
+def _chain_prep(what: str, enc: Tensor, ray_bias: Optional[Tensor], samples: int, queries: int, params):
+    """What both fused chains' forwards start from: (enc2, ld_enc, weights, ray_bias, n_ray_cols, n_feat, sinks) --
+    ``enc`` as rows the kernel can read, the eight parameters (wb0, bb0, wb1, bb1, w0, w1, w2, b2) in fp32 with their
+    gradient sinks, and ``ray_bias`` (None: density only) checked against the rays of the enc rows' points
+    (``queries`` rows per point)."""
+    _need_cuda(enc, ray_bias, *params)
+    enc2, ld_enc = _rows(enc, enc.shape[-1])
+    if ld_enc % 8 or enc2.data_ptr() % 32:          # the kernel reads its rows 32 bytes at a time
+        enc2, ld_enc = enc2.contiguous(), enc2.shape[1]
+    ws = [_f32c(t) for t in params]
+    rb = None if ray_bias is None else _f32c(ray_bias)
+    n = enc2.shape[0] // queries
+    if rb is not None and rb.shape != ((n + samples - 1) // samples, 128):
+        raise ValueError(f"{what}: ray_bias {tuple(rb.shape)} for {n} points x {samples} samples per ray")
+    n_ray_cols = ws[4].shape[1] - 64                # [dir | emb] columns in front of geo (radiance_field.py:647)
+    return enc2, ld_enc, ws, rb, n_ray_cols, ws[2].shape[0], [_grad_sink(t) for t in ws]
+
+
+def _chain_weight_args(ws: Sequence[Tensor], n_ray_cols: int, n_feat: int) -> tuple:
+    """The parameter arguments of emer_field_fwd / emer_flow_field_fwd: the base MLP, then the colour head with layer 0's
+    geo columns and layer 1's hidden and geo column blocks, each with the row stride of its whole weight."""
+    wb0, bb0, wb1, bb1, w0, w1, w2, b2 = ws
+    return (_ptr(wb0), _ptr(bb0), _ptr(wb1), _ptr(bb1), n_feat, _ptr(w0[:, n_ray_cols:]), w0.shape[1], _ptr(w1[:, :64]),
+            _ptr(w1[:, 64 + n_ray_cols:]), w1.shape[1], _ptr(w2), _ptr(b2))
+
+
+def _chain_bwd_weights(w0: Tensor, w1: Tensor, n_ray_cols: int) -> Tuple[Tensor, Tensor]:
+    """(w1hg [64, 128]: layer 1's [hidden | geo] columns, w0g [64, 64]: layer 0's geo columns), as the backward reads
+    them."""
+    return torch.cat([w1[:, :64], w1[:, 64 + n_ray_cols:]], dim=1), w0[:, n_ray_cols:].contiguous()
+
+
+def _chain_upstream(n: int, d_sigma, d_rgb, d_geo, d_sem):
+    """The upstream gradients as fp32 rows: d_sigma [n], d_rgb [n, 3], d_geo and d_sem [n, 64] (None stays None)."""
+    rows = lambda g, w: None if g is None else _f32c(g.reshape(n, w))
+    return None if d_sigma is None else _f32c(d_sigma).reshape(n), rows(d_rgb, 3), rows(d_geo, 64), rows(d_sem, 64)
+
+
+def _ray_sums(n_rays: int, samples: int, dz0: Tensor, dz1: Tensor) -> Tensor:
+    """d_ray_bias [n_rays, 128] = the per-ray sums [dZ0 | dZ1] over the rows there are (the last ray may be ragged)."""
+    ray = torch.arange(dz0.shape[0], device=dz0.device) // samples
+    d_rb = torch.zeros((n_rays, 128), dtype=torch.float32, device=dz0.device)
+    d_rb[:, :64].index_add_(0, ray, dz0)
+    d_rb[:, 64:].index_add_(0, ray, dz1)
+    return d_rb
+
+
+def _chain_grad_shapes(wb0: Tensor, wb1: Tensor, w0: Tensor, w1: Tensor, w2: Tensor, n_feat: int, head: bool):
+    """The shapes of the eight parameters' gradients for _grad_bufs; the colour head's None without a gradient."""
+    return [wb0.shape, (64,), wb1.shape, (n_feat,)] + ([w0.shape, w1.shape, w2.shape, (3,)] if head else [None] * 4)
+
+
+def _field_wgrad(enc2: Tensor, ld_enc: int, hb: Tensor, D1: Tensor, dzb: Tensor, d_sem: Optional[Tensor], n_feat: int,
+                 n_ray_cols: int, *, rows: Tuple[int, int], bufs: Sequence[Optional[Tensor]], head=None,
+                 deferred: Optional[list] = None) -> None:
+    """One ``emer_field_wgrad`` launch: X^T dZ of the chain's layers over ``rows`` = (first, count) of the saved
+    buffers, added to ``bufs`` (the eight parameters' gradient buffers from _grad_bufs).  The base MLP always; the
+    colour head when ``head`` = (hg, h1, dz2, dz1) has a dz2 (the library's own rule) -- of w0 / w1 only the geo and
+    hidden column blocks, as strided blocks of the whole buffers: the per-ray columns take theirs through ray_bias.
+    ``deferred``: the head's w0 / w1 blocks go to fresh zeros instead and their adds to ``bufs`` are appended to this
+    list -- on the side stream, because autograd adds the per-ray columns' gradient to the same buffers on the main
+    stream with an in-place add of the whole tensor, which would race the kernel's atomics."""
+    r0, n = rows
+    wb0, bb0, wb1, bb1, w0, w1, w2, b2 = bufs
+    hg, h1, dz2, dz1 = (None,) * 4 if head is None else head
+    if dz2 is None:
+        dw0g, ld_w0, dw1g, ld_w1, w1, w2, b2 = None, 0, None, 0, None, None, None
+    else:
+        if deferred is not None:
+            z0, z1 = torch.zeros_like(w0), torch.zeros_like(w1)
+            deferred += [lambda dst=w0, src=z0: dst.add_(src), lambda dst=w1, src=z1: dst.add_(src)]
+            w0, w1 = z0, z1
+        dw0g, ld_w0, dw1g, ld_w1 = w0[:, n_ray_cols:], w0.stride(0), w1[:, 64 + n_ray_cols:], w1.stride(0)
+    _lib.call("emer_field_wgrad", _ptr(enc2[r0:]), ld_enc, enc2.shape[1], _ptr(hb[r0:]), _ptr(hg), _ptr(h1), _ptr(dz2),
+              _ptr(dz1), _ptr(D1[r0:]), _ptr(dzb[r0:]), _ptr(None if d_sem is None else d_sem[r0:]), n_feat, _ptr(wb0),
+              _ptr(bb0), _ptr(wb1), _ptr(bb1), _ptr(dw0g), ld_w0, _ptr(w1), _ptr(dw1g), ld_w1, _ptr(w2), _ptr(b2), n,
+              _stream())
 
 
 class _FieldChain(torch.autograd.Function):
@@ -681,18 +772,9 @@ class _FieldChain(torch.autograd.Function):
     def forward(ctx, enc: Tensor, ray_bias: Tensor, samples: int, want_geo: bool, wb0: Tensor, bb0: Tensor, wb1: Tensor,
                 bb1: Tensor, w0: Tensor, w1: Tensor, w2: Tensor, b2: Tensor):
         ctx.set_materialize_grads(False)
-        _need_cuda(enc, ray_bias, wb0, wb1, w0, w1, w2)
-        enc2, ld_enc = _rows(enc, enc.shape[-1])
+        enc2, ld_enc, ws, rb, n_ray_cols, n_feat, sinks = _chain_prep("field_chain", enc, ray_bias, samples, 1,
+                                                                      (wb0, bb0, wb1, bb1, w0, w1, w2, b2))
         n, k_enc = enc2.shape
-        if ld_enc % 8 or enc2.data_ptr() % 32:          # the kernel reads its rows 32 bytes at a time
-            enc2, ld_enc = enc2.contiguous(), k_enc
-        n_feat = wb1.shape[0]
-        n_ray_cols = w0.shape[1] - 64                   # [dir | emb] columns in front of geo (radiance_field.py:647)
-        ws = [_f32c(t) for t in (wb0, bb0, wb1, bb1, w0, w1, w2, b2)]
-        wb0c, bb0c, wb1c, bb1c, w0c, w1c, w2c, b2c = ws
-        rb = _f32c(ray_bias)
-        if rb.shape != ((n + samples - 1) // samples, 128):
-            raise ValueError(f"field_chain: ray_bias {tuple(rb.shape)} for {n} points x {samples} samples per ray")
         dev = enc.device
         train = any(ctx.needs_input_grad)          # (False under torch.no_grad(): no saves, inference traffic only)
         f32 = dict(dtype=torch.float32, device=dev)
@@ -702,14 +784,12 @@ class _FieldChain(torch.autograd.Function):
         hg = torch.empty((n, 128), **f32) if (train or want_geo) else None
         h1 = torch.empty((n, 64), **f32) if train else None
         sem = torch.empty((n, 64), **f32) if n_feat == 128 else None
-        w0g = w0c[:, n_ray_cols:]
-        w1h, w1g = w1c[:, :64], w1c[:, 64 + n_ray_cols:]
-        _lib.call("emer_field_fwd", _ptr(enc2), ld_enc, k_enc, _ptr(wb0c), _ptr(bb0c), _ptr(wb1c), _ptr(bb1c), n_feat,
-                  _ptr(w0g), w0c.shape[1], _ptr(w1h), _ptr(w1g), w1c.shape[1], _ptr(w2c), _ptr(b2c), _ptr(rb), samples,
-                  _ptr(sigma), _ptr(rgb), _ptr(hb), _ptr(hg), _ptr(h1), _ptr(sem), n, _stream())
+        _lib.call("emer_field_fwd", _ptr(enc2), ld_enc, k_enc, *_chain_weight_args(ws, n_ray_cols, n_feat), _ptr(rb),
+                  samples, _ptr(sigma), _ptr(rgb), _ptr(hb), _ptr(hg), _ptr(h1), _ptr(sem), n, _stream())
         geo = hg[:, 64:] if want_geo else None
         if train:
-            ctx.sinks = {k: _grad_sink(t) for k, t in zip(("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"), ws)}
+            ctx.sinks = sinks
+            wb0c, _, wb1c, _, w0c, w1c, w2c, _ = ws
             ctx.save_for_backward(enc2, hb, hg, h1, rgb, sigma, wb0c, wb1c, w0c, w1c, w2c)
             ctx.meta = (samples, n_ray_cols, n_feat, enc.shape, ld_enc)
         return sigma, rgb, geo, sem
@@ -721,48 +801,36 @@ class _FieldChain(torch.autograd.Function):
         n, k_enc = enc2.shape
         dev = enc2.device
         f32 = dict(dtype=torch.float32, device=dev)
-        none = (None,) * 12
         if d_sigma is None and d_rgb is None and d_geo is None and d_sem is None:
-            return none
+            return (None,) * 12
         n_rays = (n + samples - 1) // samples
-        sk = ctx.sinks
-        w1hg = torch.cat([w1[:, :64], w1[:, 64 + n_ray_cols:]], dim=1)            # [64, 128] = [hidden | geo] columns
-        w0g = w0[:, n_ray_cols:].contiguous()
+        w1hg, w0g = _chain_bwd_weights(w0, w1, n_ray_cols)
+        d_sigma, d_rgb, d_geo, d_sem = _chain_upstream(n, d_sigma, d_rgb, d_geo, d_sem)
         D1 = torch.empty((n, 128), **f32)          # [dZ0 | dF] side by side (row stride 128)
         dz2 = dz1 = d_rb = d_enc = None
-        c = lambda g, w: None if g is None else _f32c(g.reshape(n, w))
-        d_geo, d_sem = c(d_geo, 64), c(d_sem, 64)
         if CHAIN_BWD == "fused" and samples % 32 == 0 and _tc_rows_ok(n):
             # ---- the whole data path in one kernel (csrc/field_fused.cu: field_bwd_kernel)
-            d_rgb2 = c(d_rgb, 3)
-            d_sig = None if d_sigma is None else _f32c(d_sigma).reshape(n)
             dz2 = torch.empty((n, 3), **f32) if d_rgb is not None else None
             dz1 = torch.empty((n, 64), **f32)
             dzb = torch.empty((n, 64), **f32)
             if ctx.needs_input_grad[0]:
                 d_enc = torch.empty((n, k_enc), **f32)
             d_rb = torch.zeros((n_rays, 128), **f32) if d_rgb is not None else None
-            _lib.call("emer_field_bwd", _ptr(d_rgb2), _ptr(rgb), _ptr(d_sig), _ptr(sigma), _ptr(d_geo), _ptr(d_sem), _ptr(hb),
-                      _ptr(hg), _ptr(h1), _ptr(wb0), k_enc, _ptr(wb1), n_feat, _ptr(w0g), 64, _ptr(w1hg), _ptr(w1hg[:, 64:]),
-                      128, _ptr(w2), _ptr(dz2), _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_enc), k_enc, _ptr(d_rb), samples, n,
-                      _stream())
+            _lib.call("emer_field_bwd", _ptr(d_rgb), _ptr(rgb), _ptr(d_sigma), _ptr(sigma), _ptr(d_geo), _ptr(d_sem),
+                      _ptr(hb), _ptr(hg), _ptr(h1), _ptr(wb0), k_enc, _ptr(wb1), n_feat, _ptr(w0g), 64, _ptr(w1hg),
+                      _ptr(w1hg[:, 64:]), 128, _ptr(w2), _ptr(dz2), _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_enc), k_enc,
+                      _ptr(d_rb), samples, n, _stream())
         else:
             # ---- layer by layer on the same buffers (ragged rays, tiny batches, EMER_CHAIN_BWD=layers)
             if d_rgb is not None:
-                dz2 = _f32c(d_rgb.reshape(n, 3)) * (rgb * (1.0 - rgb))
+                dz2 = d_rgb * (rgb * (1.0 - rgb))
                 dz1 = torch.empty((n, 64), **f32)
                 _layer_bwd_data(dz2, 3, w2, dz1, 64, n, h1, 64, 64)                   # relu'(h1) applied
                 _layer_bwd_data(dz1, 64, w1hg, D1, 128, n, hg, 128, 64)               # [relu'(h0) dH0 | dGeo(layer 1)]
                 dz0 = D1[:, :64]
-                if _tc_rows_ok(n):
-                    _tc_bwd_data_acc(dz0, 128, w0g, D1[:, 64:], 128, n)              # dGeo += dZ0 W0g
-                else:
-                    _lib.call("emer_linear_bwd_data", _ptr(dz0), 128, None, 0, ACT_NONE, _ptr(w0g), _ptr(D1[:, 64:]), 128,
-                              n, 64, 64, 1, _stream())
+                _layer_bwd_data(dz0, 128, w0g, D1[:, 64:], 128, n, None, 0, 0, accumulate=True)     # dGeo += dZ0 W0g
                 if n_rays * samples - n:                   # ragged last ray: sum what is there
-                    d_rb = torch.zeros((n_rays, 128), **f32)
-                    d_rb[:, :64].index_add_(0, torch.arange(n, device=dev) // samples, dz0)
-                    d_rb[:, 64:].index_add_(0, torch.arange(n, device=dev) // samples, dz1)
+                    d_rb = _ray_sums(n_rays, samples, dz0, dz1)
                 else:
                     d_rb = torch.cat([D1.view(n_rays, samples, 128)[:, :, :64].sum(1),
                                       dz1.view(n_rays, samples, 64).sum(1)], dim=1)
@@ -773,7 +841,7 @@ class _FieldChain(torch.autograd.Function):
                 dgeo += d_geo
             if d_sigma is not None:
                 # trunc_exp backward (nerf_utils.py:72-75): g * exp(clamp(x, max=15)), x = feats[:, 0] - 1 = log(sigma)
-                dgeo[:, 0] += _f32c(d_sigma).reshape(n) * torch.clamp(sigma, max=3269017.25)
+                dgeo[:, 0] += d_sigma * torch.clamp(sigma, max=3269017.25)
             # [dF | d_sem]: the gradient of the base MLP's output (zeros for an absent semantic half)
             if n_feat == 128:
                 dfe = torch.cat([D1[:, 64:], torch.zeros((n, 64), **f32) if d_sem is None else d_sem], dim=1)
@@ -786,51 +854,20 @@ class _FieldChain(torch.autograd.Function):
                 _layer_bwd_data(dzb, 64, wb0, d_enc, d_enc.shape[1], n, None, 0, 0)
                 d_enc = d_enc[:, :k_enc]
 
-        shapes = dict(wb0=wb0.shape, bb0=(64,), wb1=wb1.shape, bb1=(n_feat,), w0=w0.shape, w1=w1.shape, w2=w2.shape,
-                      b2=(3,))
-        keys = list(shapes) if dz2 is not None else ["wb0", "bb0", "wb1", "bb1"]
-        side = WGRAD_STREAM and all(v is not None for v in sk.values())
-
-        def weight_gradients(deferred):
-            """The five layers' X^T dZ in one emer_field_wgrad launch, accumulated into the optimizer's buffers (or
-            into zeros shaped like the parameters, returned to autograd).  ``deferred``: the side stream's list of
-            updates to run after the join -- the head's w0 / w1 gradients then go to zeros and are added there,
-            because autograd adds the per-ray columns' gradient to the same buffers on the main stream with an
-            in-place add of the whole tensor, which would race the kernel's atomics."""
-            out, grads = {}, {}
-            for k in keys:
-                s = sk[k]
-                if s is None:
-                    out[k] = grads[k] = torch.zeros(shapes[k], **f32)
-                elif deferred is not None and k in ("w0", "w1"):
-                    out[k] = torch.zeros(shapes[k], **f32)
-                    deferred.append(lambda dst=s[0], src=out[k]: dst.add_(src))
-                else:
-                    out[k] = s[0]
-            o = lambda k: _ptr(out[k]) if k in out else None
-            if dz2 is not None:        # the head's geo / hidden column blocks; the per-ray ones come through ray_bias
-                w0g_d, ld_w0, w1g_d, ld_w1 = out["w0"][:, n_ray_cols:], out["w0"].stride(0), out["w1"][:, 64 + n_ray_cols:], out["w1"].stride(0)
-            else:
-                w0g_d, ld_w0, w1g_d, ld_w1 = None, 0, None, 0
-            _lib.call("emer_field_wgrad", _ptr(enc2), ld_enc, k_enc, _ptr(hb), _ptr(hg), _ptr(h1), _ptr(dz2),
-                      _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_sem), n_feat, o("wb0"), o("bb0"), o("wb1"), o("bb1"),
-                      _ptr(w0g_d), ld_w0, o("w1"), _ptr(w1g_d), ld_w1, o("w2"), o("b2"), n, _stream())
-            for k in keys:
-                if sk[k] is not None:
-                    sk[k][1]()
-            return tuple(grads.get(k) for k in ("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"))
-
-        if side:
+        bufs = _grad_bufs(_chain_grad_shapes(wb0, wb1, w0, w1, w2, n_feat, dz2 is not None), ctx.sinks, dev)
+        wgrad = lambda deferred=None: _field_wgrad(enc2, ld_enc, hb, D1, dzb, d_sem, n_feat, n_ray_cols, rows=(0, n),
+                                                   bufs=bufs, head=(hg, h1, dz2, dz1), deferred=deferred)
+        if WGRAD_STREAM and all(s is not None for s in ctx.sinks):
             # every weight gradient lands in the optimizer's buffers: nothing autograd waits for, so the kernel may
             # run beside the hash-grid scatter / the table's reduce-scatter (joined by FusedAdam.step /
             # DataParallel.reduce)
             with _on_side_stream(dev, enc2, hb, hg, h1, dz2, dz1, D1, dzb, d_sem):
-                dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(_AFTER_JOIN)
+                wgrad(_AFTER_JOIN)
         else:
-            dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2 = weight_gradients(None)
+            wgrad()
         if d_enc is not None:
             d_enc = d_enc.reshape(enc_shape)
-        return d_enc, d_rb, None, None, dwb0, dbb0, dwb1, dbb1, dw0, dw1, dw2, db2
+        return (d_enc, d_rb, None, None, *_grad_outputs(bufs, ctx.sinks))
 
 
 def field_chain_usable(k_enc: int, n_feat: int, width: int, head: Sequence[Tuple[int, int]]) -> bool:
@@ -918,7 +955,7 @@ class _GridEncodeRows(torch.autograd.Function):
         y = torch.empty((n, desc.n_output_dims), dtype=torch.float32, device=x.device)
         _lib.call("emer_grid_fwd", ctypes.byref(desc.c), _ptr(x), _ptr(params), _ptr(y), n, _stream())
         ctx.save_for_backward(x, params)
-        ctx.desc, ctx.n0 = desc, x_fixed.shape[0]
+        ctx.desc, ctx.n0, ctx.sinks = desc, x_fixed.shape[0], [_grad_sink(params)]
         return y
 
     @staticmethod
@@ -929,8 +966,7 @@ class _GridEncodeRows(torch.autograd.Function):
         desc, n0 = ctx.desc, ctx.n0
         dy = _f32c(dy)
         need_x, need_p = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        sink = _grad_sink(params) if need_p else None
-        dparams = sink[0] if sink is not None else (torch.zeros_like(params) if need_p else None)
+        (dparams,) = _grad_bufs([params.shape if need_p else None], ctx.sinks, x.device)
         if need_p:
             _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(x), _ptr(params), _ptr(dy), _ptr(dparams), _ptr(None),
                       x.shape[0], _stream())
@@ -942,10 +978,7 @@ class _GridEncodeRows(torch.autograd.Function):
             xv, dyv = (t if t.data_ptr() % 16 == 0 else t.clone() for t in (x[n0:], dy[n0:]))
             _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(xv), _ptr(params), _ptr(dyv), _ptr(None),
                       _ptr(dx), dx.shape[0], _stream())
-        if sink is not None:
-            sink[1]()
-            dparams = None
-        return None, dx, dparams, None
+        return (None, dx, *_grad_outputs([dparams], ctx.sinks), None)
 
 
 def grid_encode_rows(x_fixed: Tensor, x_var: Tensor, params: Tensor, desc: GridDesc) -> Tensor:
@@ -966,20 +999,11 @@ class _FlowFieldChain(torch.autograd.Function):
     def forward(ctx, enc: Tensor, ray_bias: Optional[Tensor], samples: int, wb0: Tensor, bb0: Tensor, wb1: Tensor,
                 bb1: Tensor, w0: Tensor, w1: Tensor, w2: Tensor, b2: Tensor):
         ctx.set_materialize_grads(False)
-        _need_cuda(enc, wb0, wb1, w0, w1, w2)
-        enc2, ld_enc = _rows(enc, enc.shape[-1])
-        if ld_enc % 8 or enc2.data_ptr() % 32:
-            enc2, ld_enc = enc2.contiguous(), enc2.shape[1]
+        enc2, ld_enc, ws, rb, n_ray_cols, n_feat, sinks = _chain_prep("flow_field_chain", enc, ray_bias, samples, 3,
+                                                                      (wb0, bb0, wb1, bb1, w0, w1, w2, b2))
         n3, k_enc = enc2.shape
         n = n3 // 3
-        n_feat = wb1.shape[0]
-        n_ray_cols = w0.shape[1] - 64
-        ws = [_f32c(t) for t in (wb0, bb0, wb1, bb1, w0, w1, w2, b2)]
-        wb0c, bb0c, wb1c, bb1c, w0c, w1c, w2c, b2c = ws
-        head = ray_bias is not None
-        rb = _f32c(ray_bias) if head else None
-        if head and rb.shape != ((n + samples - 1) // samples, 128):
-            raise ValueError(f"flow_field_chain: ray_bias {tuple(rb.shape)} for {n} points x {samples} samples per ray")
+        head = rb is not None
         dev = enc.device
         train = any(ctx.needs_input_grad)
         f32 = dict(dtype=torch.float32, device=dev)
@@ -989,12 +1013,11 @@ class _FlowFieldChain(torch.autograd.Function):
         hg = torch.empty((n, 128), **f32)                 # the geometry half carries the blend
         h1 = torch.empty((n, 64), **f32) if (train and head) else None
         sem = torch.empty((n, 64), **f32) if n_feat == 128 else None
-        _lib.call("emer_flow_field_fwd", _ptr(enc2), ld_enc, k_enc, _ptr(wb0c), _ptr(bb0c), _ptr(wb1c), _ptr(bb1c), n_feat,
-                  _ptr(w0c[:, n_ray_cols:]), w0c.shape[1], _ptr(w1c[:, :64]), _ptr(w1c[:, 64 + n_ray_cols:]), w1c.shape[1],
-                  _ptr(w2c), _ptr(b2c), _ptr(rb), samples, _ptr(sigma), _ptr(rgb), _ptr(hb), _ptr(hg), _ptr(h1), _ptr(sem),
-                  n, _stream())
+        _lib.call("emer_flow_field_fwd", _ptr(enc2), ld_enc, k_enc, *_chain_weight_args(ws, n_ray_cols, n_feat),
+                  _ptr(rb), samples, _ptr(sigma), _ptr(rgb), _ptr(hb), _ptr(hg), _ptr(h1), _ptr(sem), n, _stream())
         if train:
-            ctx.sinks = {k: _grad_sink(t) for k, t in zip(("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"), ws)}
+            ctx.sinks = sinks
+            wb0c, _, wb1c, _, w0c, w1c, w2c, _ = ws
             ctx.save_for_backward(enc2, hb, hg, h1, rgb, sigma, wb0c, wb1c, w0c, w1c, w2c)
             ctx.meta = (samples, n_ray_cols, n_feat, enc.shape, ld_enc, head)
         return sigma, rgb, hg[:, 64:], sem
@@ -1010,67 +1033,34 @@ class _FlowFieldChain(torch.autograd.Function):
         if d_sigma is None and d_rgb is None and d_geo is None and d_sem is None:
             return (None,) * 11
         n_rays = (n + samples - 1) // samples
-        w1hg = torch.cat([w1[:, :64], w1[:, 64 + n_ray_cols:]], dim=1)            # [64, 128] = [hidden | geo] columns
-        w0g = w0[:, n_ray_cols:].contiguous()
-        c = lambda g, w: None if g is None else _f32c(g.reshape(n, w))
-        d_geo, d_sem = c(d_geo, 64), c(d_sem, 64)
-        d_rgb2 = c(d_rgb, 3) if head else None
-        d_sig = None if d_sigma is None else _f32c(d_sigma).reshape(n)
+        w1hg, w0g = _chain_bwd_weights(w0, w1, n_ray_cols)
+        d_sigma, d_rgb, d_geo, d_sem = _chain_upstream(n, d_sigma, d_rgb, d_geo, d_sem)     # (no rgb, no d_rgb)
         D1 = torch.empty((n3, 128), **f32)         # rows [0, n): [dZ0 | dF_c]; rows [n, 3n): [unused | dF_f, dF_b]
-        dz2 = torch.empty((n, 3), **f32) if d_rgb2 is not None else None
+        dz2 = torch.empty((n, 3), **f32) if d_rgb is not None else None
         dz1 = torch.empty((n, 64), **f32) if head else None
         dzb = torch.empty((n3, 64), **f32)
         d_enc = torch.empty((n3, k_enc), **f32) if ctx.needs_input_grad[0] else None
         d_sem_q = torch.empty((n3, 64), **f32) if d_sem is not None else None
         ray_sums = dz2 is not None and samples % 32 == 0
         d_rb = torch.zeros((n_rays, 128), **f32) if ray_sums else None
-        _lib.call("emer_flow_field_bwd", _ptr(d_rgb2), _ptr(rgb), _ptr(d_sig), _ptr(sigma), _ptr(d_geo), _ptr(d_sem),
+        _lib.call("emer_flow_field_bwd", _ptr(d_rgb), _ptr(rgb), _ptr(d_sigma), _ptr(sigma), _ptr(d_geo), _ptr(d_sem),
                   _ptr(hb), _ptr(hg if head else None), _ptr(h1), _ptr(wb0), k_enc, _ptr(wb1), n_feat, _ptr(w0g), 64,
                   _ptr(w1hg), _ptr(w1hg[:, 64:]), 128, _ptr(w2), _ptr(dz2), _ptr(dz1), _ptr(D1), _ptr(dzb), _ptr(d_enc),
                   k_enc, _ptr(d_rb), _ptr(d_sem_q), samples, n, _stream())
         if dz2 is not None and not ray_sums:            # ragged rays: the per-ray sums of [dZ0 | dZ1] on the host side
-            ray = torch.arange(n, device=dev) // samples
-            d_rb = torch.zeros((n_rays, 128), **f32)
-            d_rb[:, :64].index_add_(0, ray, D1[:n, :64])
-            d_rb[:, 64:].index_add_(0, ray, dz1)
+            d_rb = _ray_sums(n_rays, samples, D1[:n, :64], dz1)
 
-        sk = ctx.sinks
-        shapes = dict(wb0=wb0.shape, bb0=(64,), wb1=wb1.shape, bb1=(n_feat,), w0=w0.shape, w1=w1.shape, w2=w2.shape,
-                      b2=(3,))
-        keys = list(shapes) if dz2 is not None else ["wb0", "bb0", "wb1", "bb1"]
-        out, grads = {}, {}
-        for k in keys:
-            if sk[k] is None:
-                out[k] = grads[k] = torch.zeros(shapes[k], **f32)
-            else:
-                out[k] = sk[k][0]
-        o = lambda k: _ptr(out[k]) if k in out else None
-        rows = lambda t, r0: None if t is None else t[r0:]
-
-        def wgrad(r0: int, rn: int, with_head: bool):
-            if with_head:
-                w0g_d, ld_w0, w1g_d, ld_w1 = out["w0"][:, n_ray_cols:], out["w0"].stride(0), out["w1"][:, 64 + n_ray_cols:], out["w1"].stride(0)
-                hd = (hg, h1, dz2, dz1)
-            else:
-                w0g_d, ld_w0, w1g_d, ld_w1 = None, 0, None, 0
-                hd = (None, None, None, None)
-            _lib.call("emer_field_wgrad", _ptr(enc2[r0:]), ld_enc, k_enc, _ptr(hb[r0:]), _ptr(hd[0]), _ptr(hd[1]),
-                      _ptr(hd[2]), _ptr(hd[3]), _ptr(D1[r0:]), _ptr(dzb[r0:]), _ptr(rows(d_sem_q, r0)), n_feat, o("wb0"),
-                      o("bb0"), o("wb1"), o("bb1"), _ptr(w0g_d), ld_w0, o("w1") if with_head else None, _ptr(w1g_d),
-                      ld_w1, o("w2") if with_head else None, o("b2") if with_head else None, rn, _stream())
-
+        bufs = _grad_bufs(_chain_grad_shapes(wb0, wb1, w0, w1, w2, n_feat, dz2 is not None), ctx.sinks, dev)
+        wgrad = lambda rows, head=None: _field_wgrad(enc2, ld_enc, hb, D1, dzb, d_sem_q, n_feat, n_ray_cols, rows=rows,
+                                                     bufs=bufs, head=head)
         if dz2 is not None:
-            wgrad(0, n, True)                           # colour head + base MLP over the current rows
-            wgrad(n, 2 * n, False)                      # base MLP over the warped rows
+            wgrad((0, n), (hg, h1, dz2, dz1))           # colour head + base MLP over the current rows
+            wgrad((n, 2 * n))                           # base MLP over the warped rows
         else:
-            wgrad(0, n3, False)
-        for k in keys:
-            if sk[k] is not None:
-                sk[k][1]()
-        g = tuple(grads.get(k) for k in ("wb0", "bb0", "wb1", "bb1", "w0", "w1", "w2", "b2"))
+            wgrad((0, n3))
         if d_enc is not None:
             d_enc = d_enc.reshape(enc_shape)
-        return (d_enc, d_rb, None) + g
+        return (d_enc, d_rb, None, *_grad_outputs(bufs, ctx.sinks))
 
 
 def flow_field_chain(enc: Tensor, ray_bias: Optional[Tensor], samples: int, base, head):
@@ -1162,16 +1152,14 @@ class _PropLevelTrain(torch.autograd.Function):
         lf = desc.n_output_dims
         xc = torch.empty((r * n, 3), dtype=torch.float32, device=dev)
         d_enc = torch.empty((r * n, lf), dtype=torch.float32, device=dev)
-        outs = []
-        for t, sink in zip((table, w0, b0, w1, b1), ctx.sinks):
-            if sink is not None:
-                outs.append(sink[0])
-            else:
-                outs.append(torch.zeros(t.shape, dtype=torch.float32, device=dev))
-        d_table, d_w0, d_b0, d_w1, d_b1 = outs
+        bufs = _grad_bufs([t.shape for t in (table, w0, b0, w1, b1)], ctx.sinks, dev)
+        d_table, d_w0, d_b0, d_w1, d_b1 = bufs
         tsink = ctx.sinks[0]
-        if tsink is not None and tsink[2] is not None and not tsink[2]():
-            d_table.zero_()                    # L2 write-allocate before the scatter (see _GridEncode.backward)
+        if tsink is not None and not tsink.touched():
+            # first gradient of this step: the slice is all zeros (the optimizer cleared it a step ago) but no longer in
+            # L2, and a red.add on a missing line is a DRAM read-modify-write; re-writing the zeros write-allocates the
+            # lines in L2 right before the scatter
+            d_table.zero_()
         o, d, box = _f32c(origins), _f32c(dirs), _f32c(aabb.reshape(-1))
         tab, w0c, b0c, w1c = _f32c(table), _f32c(w0), _f32c(b0), _f32c(w1.reshape(-1))
         _lib.call("emer_prop_level_bwd", ctypes.byref(desc.c), _ptr(t_edges), _ptr(sigma), _ptr(d_cdf), n, _ptr(o), _ptr(d),
@@ -1179,14 +1167,7 @@ class _PropLevelTrain(torch.autograd.Function):
                   _ptr(d_w0), _ptr(d_b0), _ptr(d_w1), _ptr(d_b1), r, _stream())
         _lib.call("emer_grid_bwd", ctypes.byref(desc.c), _ptr(xc), _ptr(tab), _ptr(d_enc), _ptr(d_table), None, r * n,
                   _stream())
-        grads = []
-        for g, sink in zip(outs, ctx.sinks):
-            if sink is not None:
-                sink[1]()
-                grads.append(None)
-            else:
-                grads.append(g)
-        return tuple(grads) + none
+        return (*_grad_outputs(bufs, ctx.sinks), *none)
 
 
 def prop_level_train_usable(desc: GridDesc) -> bool:

@@ -108,13 +108,16 @@ class FusedAdam(torch.optim.Optimizer):
             for i, p in enumerate(g.params):
                 sink = g.view(g.grad, i)
                 p.grad = sink
-                _ops.register_grad_sink(p, sink, self._mark)
+                _ops.register_grad_sink(p, sink, self._mark, self._is_touched)
                 p.register_post_accumulate_grad_hook(self._mark)          # gradients that arrive through torch autograd
                 self.state[p] = {"step": g.hyper[0], "exp_avg": g.view(g.exp_avg, i), "exp_avg_sq": g.view(g.exp_avg_sq, i)}
 
     # ------------------------------------------------------------------ bookkeeping
     def _mark(self, p: Tensor) -> None:
         self._touched.add(id(p))
+
+    def _is_touched(self, p: Tensor) -> bool:
+        return id(p) in self._touched
 
     def flat_grads(self) -> List[Tensor]:
         """One flat gradient buffer per param group (what data parallelism reduces)."""

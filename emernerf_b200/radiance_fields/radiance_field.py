@@ -262,16 +262,19 @@ class RadianceField(nn.Module):
         w = torch.cat([l0.weight[:, :c], l1.weight[:, h:h + c]], dim=0)
         return _ops.linear(_ops.cat_pad4([v]), w, torch.cat([l0.bias, l1.bias]))
 
+    def _chain_params(self, base: nn.Sequential):
+        """(base, head) parameter tuples of the fused chains: the base MLP's two nn.Linear layers, (wb0, bb0, wb1, bb1),
+        and the colour head's three layers, (w0, w1, w2, b2)."""
+        lin = [m for m in base if isinstance(m, nn.Linear)]
+        l0, l1, l2 = self.rgb_head.layers
+        return (lin[0].weight, lin[0].bias, lin[1].weight, lin[1].bias), (l0.weight, l1.weight, l2.weight, l2.bias)
+
     def _run_chain(self, encoder: HashEncoder, base: nn.Sequential, coords: Tensor, ray_bias: Tensor,
                    want_geo: bool = False):
         """(density [R,S], rgb [R,S,3], geo [R,S,64] | None, sem [R,S,64] | None) for grid coordinates [R,S,D]."""
         r, s_ = coords.shape[:2]
         enc = encoder(coords.reshape(-1, coords.shape[-1]))
-        lin = [m for m in base if isinstance(m, nn.Linear)]
-        l0, l1, l2 = self.rgb_head.layers
-        sigma, rgb, geo, sem = _ops.field_chain(
-            enc, ray_bias, s_, (lin[0].weight, lin[0].bias, lin[1].weight, lin[1].bias),
-            (l0.weight, l1.weight, l2.weight, l2.bias), want_geo=want_geo)
+        sigma, rgb, geo, sem = _ops.field_chain(enc, ray_bias, s_, *self._chain_params(base), want_geo=want_geo)
         return (sigma.view(r, s_), rgb.view(r, s_, 3), None if geo is None else geo.view(r, s_, -1),
                 None if sem is None else sem.view(r, s_, -1))
 
@@ -469,11 +472,7 @@ class RadianceField(nn.Module):
         enc_d = self.dynamic_xyz_encoder
         enc = _ops.grid_encode_rows(self._space_time(normed, t).reshape(n, -1), coords_w, enc_d.tcnn_encoding.params,
                                     enc_d.desc)
-        lin = [m for m in self.dynamic_base_mlp if isinstance(m, nn.Linear)]
-        l0, l1, l2 = self.rgb_head.layers
-        sigma, rgb, geo, sem = _ops.flow_field_chain(
-            enc, ray_bias, lead[-1], (lin[0].weight, lin[0].bias, lin[1].weight, lin[1].bias),
-            (l0.weight, l1.weight, l2.weight, l2.bias))
+        sigma, rgb, geo, sem = _ops.flow_field_chain(enc, ray_bias, lead[-1], *self._chain_params(self.dynamic_base_mlp))
         k = enc.shape[-1]
         feats = geo if sem is None else torch.cat([geo, sem], dim=-1)
         res = {"forward_flow": fwd, "backward_flow": bwd,

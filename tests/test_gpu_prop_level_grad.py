@@ -192,13 +192,16 @@ def test_restatement_in_fp32_matches_the_oracle(levels, unbounded):
 
 # ------------------------------------------------------------------------------------------------- GPU
 class _Touched:
-    """Stands in for FusedAdam's bookkeeping: ``_ops._grad_sink`` reads ``_touched`` off the bound ``mark``."""
+    """Stands in for FusedAdam's bookkeeping: the ``mark`` / ``touched`` pair a sink is registered with."""
 
     def __init__(self):
         self._touched = set()
 
     def mark(self, p):
         self._touched.add(id(p))
+
+    def touched(self, p):
+        return id(p) in self._touched
 
 
 @pytest.fixture
@@ -311,7 +314,7 @@ def test_level_backward_vs_fp64(case, restore_sinks):
     touch = _Touched()
     sinks = [torch.zeros_like(p) for p in params]
     for p, s in zip(params, sinks):
-        _ops.register_grad_sink(p, s, touch.mark)
+        _ops.register_grad_sink(p, s, touch.mark, touch.touched)
         touch.mark(p)                                   # "another term wrote it first": no zeroing, accumulate
     args = (prev_s, prev_cdf, n, bias, s_min, s_max, KIND, origins, dirs, net.aabb, unbounded, desc)
     s0, t0, cdf0 = _ops.prop_level(*args, *params)

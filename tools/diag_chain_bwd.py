@@ -5,7 +5,7 @@ for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden
     sys.path.insert(0, p)
 import torch
 from emernerf_b200 import _ops
-from emernerf_b200._ops import _layer_bwd_data, _layer_bwd_weight, _tc_bwd_data_acc
+from emernerf_b200._ops import _layer_bwd_data, _layer_bwd_weight
 DEV = "cuda"
 
 def err(a, b):
@@ -43,7 +43,7 @@ for rep in range(2):
     dw0g, _ = _layer_bwd_weight(hg[:, 64:], 128, dz0, 128, w0g, False, n)
     print(f"  dw0g (tc wgrad strided) {err(dw0g, d(dz0).T @ d(hg[:, 64:]))}")
     before = D1.clone()
-    _tc_bwd_data_acc(dz0, 128, w0g, D1[:, 64:], 128, n)
+    _layer_bwd_data(dz0, 128, w0g, D1[:, 64:], 128, n, None, 0, 0, accumulate=True)
     acc_w = d(before)
     acc_w[:, 64:] += d(before[:, :64]) @ d(w0g)
     print(f"  D1 after accumulate     {err(D1, acc_w)}")
