@@ -89,6 +89,12 @@ class EmerTrajectoryRaysIn(ctypes.Structure):
 class EmerTrajectoryRaysOut(ctypes.Structure):
     _fields_ = [(k, _P) for k in TRAJECTORY_RAYS_OUT_PTRS]
 
+
+# host struct of the voxel-lifting entry points (include/emer_b200.h): field names and order as there
+class EmerVoxelGrid(ctypes.Structure):
+    _fields_ = [("min", c_float * 3), ("voxel_size", c_float * 3), ("res", c_int64 * 3), ("bits", _P),
+                ("first_row", c_int64)]
+
 # number of kernels this library launched through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = 0
 
@@ -159,6 +165,10 @@ _SIGNATURES = {
     "emer_lidar_flow_accumulate": [_P, c_int64, _P, _P, _P, _P, c_int64, c_float, _P, _P, _P],
     "emer_occ_accumulate": [_P, c_int64, c_int, _P, c_int64, _P, c_int64, c_int, c_float, _P, _P, _P, _P],
     "emer_occ_classify": [_P, c_int64, c_int, _P, c_int64, _P, c_int64, _P, c_int, _P, c_float, _P, _P, _P],
+    "emer_voxel_mark": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_float, POINTER(EmerVoxelGrid),
+                        POINTER(EmerVoxelGrid), _P],
+    "emer_voxel_compact": [POINTER(EmerVoxelGrid), c_int, _P, _P, _P, _P],
+    "emer_voxel_select": [_P, _P, _P, c_int, c_float, _P, _P, c_int64, c_int, _P, _P, _P, c_int64, _P, _P, _P, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])
@@ -247,6 +257,12 @@ def tag_of(name: str, args) -> str:
             return f"C{args[2]}_K{args[7]}_N{args[6]}"
         if name == "emer_occ_classify":
             return f"C{args[2]}_K{args[8]}_N{args[6]}"
+        if name == "emer_voxel_mark":
+            return f"N{args[8]}" + ("_D" if args[11] is not None and args[11]._obj.bits else "")
+        if name == "emer_voxel_compact":
+            return f"G{args[1]}" + ("_write" if args[3].value else "_count")
+        if name == "emer_voxel_select":
+            return f"K{args[3]}_C{args[8]}_N{args[12]}"
         if name == "emer_flow_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("" if args[18].value else "_density")
         if name == "emer_flow_field_bwd":

@@ -719,6 +719,56 @@ int emer_occ_classify(const float* feat, int64_t ld_feat, int channels, const fl
                       const int64_t* labels, int64_t n, const float* centroids, int n_classes,
                       const int64_t* label_bank, float threshold, int64_t* counts, void* workspace, void* stream);
 
+/* ---- voxel lifting of the feature field (csrc/voxels.cu; replaces utils/visualization_tools.py:456-726,
+ *      visualize_voxels, with its boolean indexes per image, torch.nonzero over dense float grids and boolean
+ *      compaction per chunk).  A voxel grid is a bit grid of res[0] * res[1] * res[2] voxels (at most 2^32), voxel
+ *      (x, y, z) at linear index (x res[1] + y) res[2] + z, bit (index & 31) of uint32 word (index >> 5). ---------- */
+#define EMER_VOXEL_MAX_GRIDS 32                   /* grids per emer_voxel_compact call */
+#define EMER_VOXEL_BLOCK_WORDS 2048               /* bit-grid words per compaction block */
+#define EMER_VOXEL_SELECT_TILE 2048               /* rows per emer_voxel_select tile */
+#define EMER_VOXEL_SELECT_MAX_ROWS (1 << 24)      /* rows per emer_voxel_select call */
+#define EMER_VOXEL_SELECT_WORKSPACE_BYTES 65600   /* ticket + one flag per tile */
+#define EMER_VOXEL_MAX_CHANNELS 256
+typedef struct emer_voxel_grid {
+    float min[3];          /* box minimum */
+    float voxel_size[3];   /* per axis, (max - min) / res in fp32 */
+    int64_t res[3];
+    uint32_t* bits;        /* ceil(res[0] res[1] res[2] / 32) words (device) */
+    int64_t first_row;     /* emer_voxel_compact's write pass: the coords row of this grid's first voxel */
+} emer_voxel_grid;
+/* One image of rays: n rays, origins and viewdirs rows of 3 floats with row strides ld_origins / ld_viewdirs, depth
+ * and dynamic_depth with strides ld_depth / ld_dynamic_depth.  Per ray, in fp32 with separate roundings,
+ * p = o + d * depth and q = (p - min) / voxel_size per axis; the voxel trunc(q) is marked (atomicOr) when on every axis
+ * q > -1 and q < res (so q in (-1, 0) marks voxel 0, and NaN or +-inf marks nothing).  The static grid takes the rays
+ * with depth < max_depth (strict; NaN fails); the dynamic grid, when dynamic is not NULL and has bits, takes every ray
+ * at dynamic_depth.  Grids are host structs. */
+int emer_voxel_mark(const float* origins, int64_t ld_origins, const float* viewdirs, int64_t ld_viewdirs,
+                    const float* depth, int64_t ld_depth, const float* dynamic_depth, int64_t ld_dynamic_depth,
+                    int64_t n, float max_depth, const emer_voxel_grid* static_grid,
+                    const emer_voxel_grid* dynamic, void* stream);
+/* The set voxels of n_grids (<= EMER_VOXEL_MAX_GRIDS) grids (host array) as world coordinates, in linear-index order
+ * (torch.nonzero's): min + float(index) * voxel_size per axis, two roundings (the voxel's minimum corner).  Two passes
+ * of one launch each.  Count pass (coords NULL): counts[g] (int64, device) = set voxels of grid g.  Write pass (after
+ * the caller has read the counts): grid g's voxels go to coords rows [first_row, first_row + counts[g]) of 3 floats.
+ * workspace: 8 + 8 * sum_g ceil(words_g / EMER_VOXEL_BLOCK_WORDS) bytes, zeroed before the count pass; the count pass
+ * leaves the scanned block counts there for the write pass with the same grids.  Integer arithmetic only, so
+ * deterministic. */
+int emer_voxel_compact(const emer_voxel_grid* grids, int n_grids, int64_t* counts, float* coords, void* workspace,
+                       void* stream);
+/* One chunk of n queried voxels (n <= EMER_VOXEL_SELECT_MAX_ROWS): k (1..3) dense density columns d0..d2 and the gate
+ * ((d0 + d1) + d2) * ((float)n / (float)(n k)) > threshold, torch's mean over the stacked columns on the device
+ * (strict; NaN fails).  The kept voxels are appended in row order at *count (int64, device), which is advanced:
+ * out_points rows of 3 floats copied from points (dense [n, 3]), out_colors rows of
+ * clamp((f . M - color_min) / (color_max - color_min), 0, 1) with f the voxel's feature row of `channels` floats (row
+ * stride ld_feat; both multiples of 4, feat 16-byte aligned, channels <= EMER_VOXEL_MAX_CHANNELS), M the dense
+ * [channels, 3] reduction, the dot product in fp64 rounded once to fp32, and a NaN kept as torch.clamp keeps it.
+ * color_min / color_max: 3 floats each (device).  workspace: EMER_VOXEL_SELECT_WORKSPACE_BYTES, zeroed once by its
+ * owner and left zeroed by every call.  The order of the kept rows, and so the output, is deterministic. */
+int emer_voxel_select(const float* d0, const float* d1, const float* d2, int k, float threshold, const float* points,
+                      const float* feat, int64_t ld_feat, int channels, const float* reduction,
+                      const float* color_min, const float* color_max, int64_t n, float* out_points,
+                      float* out_colors, int64_t* count, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
