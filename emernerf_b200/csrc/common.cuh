@@ -73,12 +73,19 @@ __device__ __forceinline__ double warp_scan_incl(double v, int lane) {
     return v;
 }
 
-// inclusive warp scan (minimum)
+// min(a, b) that returns NaN when either is NaN (fminf returns the other operand)
+__device__ __forceinline__ float fmin_nan(float a, float b) {
+    float r;
+    asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+
+// inclusive warp scan (minimum); a NaN reaches every lane above it, as it does in a sum
 __device__ __forceinline__ float warp_scan_min(float v, int lane) {
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
         float t = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v = fminf(v, t);
+        if (lane >= o) v = fmin_nan(v, t);
     }
     return v;
 }

@@ -1,7 +1,8 @@
 // One proposal level in ONE launch (no-grad path of PropNetEstimator.sampling):
 //   inverse-CDF resampling of the previous level -> s->t warp -> ray march -> contraction+selector ->
 //   hash grid (3-D, F floats x L levels <= 16 features) -> Linear(LF,64)-ReLU-Linear(64,1) ->
-//   trunc_exp(x-1) -> sigma*delta -> exclusive scan along the ray -> CDF of this level.
+//   trunc_exp(x-1) -> sigma*delta -> exclusive scan along the ray -> CDF of this level, 1 - the running minimum of T
+//   (the composite's monotone_trans, ray_scan.cuh: non-decreasing along every ray).
 // Replaces, per level, ~15 launches of the modular path (third_party/nerfacc_prop_net.py:147-170 with
 // render_utils.py:314-324 and radiance_field.py:825-841 of the reference) and every intermediate
 // [R,S,*] tensor: the only HBM traffic is the table gathers (L2-resident: 18-22 MB tables) and the
@@ -14,6 +15,7 @@
 #include "common.cuh"
 #include "contract.cuh"
 #include "grid_common.cuh"
+#include "ray_scan.cuh"
 #include "sampling.cuh"
 
 namespace emer {
@@ -150,7 +152,7 @@ __global__ void __launch_bounds__(PL_WARPS * 32, 2) prop_level_kernel(const Prop
 
     // ---- 2. density at the interval midpoints, 3. scan -> CDF
     const PlRay rc = pl_load_ray(p.origins, p.dirs, p.aabb, ray);
-    float carry = 0.0f;
+    float carry = 0.0f, carry_t = 1.0f;
     for (int k0 = 0; k0 < n; k0 += 32) {
         const int k = k0 + lane;
         const bool ok = k < n;
@@ -177,7 +179,8 @@ __global__ void __launch_bounds__(PL_WARPS * 32, 2) prop_level_kernel(const Prop
         }
         const float incl = warp_scan_incl(xdelta, lane);
         const float e_excl = carry + warp_scan_excl(incl, lane);
-        if (ok) p.out_cdf[ray * (n + 1) + k] = 1.0f - expf(-e_excl);
+        const float T = monotone_trans(expf(-e_excl), carry_t, lane);    // the composite's CDF: never falls
+        if (ok) p.out_cdf[ray * (n + 1) + k] = 1.0f - T;
         carry += __shfl_sync(0xffffffffu, incl, 31);
     }
     if (lane == 0) p.out_cdf[ray * (n + 1) + n] = 1.0f;

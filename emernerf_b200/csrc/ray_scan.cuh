@@ -9,6 +9,17 @@
 
 namespace emer {
 
+// The running minimum of T along the ray, for the CDF 1 - T, on every lane of a 32-sample chunk; carry_t holds the
+// smallest T before the chunk (1 on the first).  The scans of two neighbouring lanes are different trees and can invert
+// by an ulp where a sample adds (next to) nothing, so T itself may rise by an ulp and the CDF would fall.  The minimum
+// is some T_j, j <= i, whose prefix and error bound are no larger than sample i's, so it stays within T_i's bound.  A
+// NaN prefix (an infinite density on a zero-length interval) stays NaN, as 1 - exp(-E) does.
+__device__ __forceinline__ float monotone_trans(float T, float& carry_t, int lane) {
+    const float m = fmin_nan(warp_scan_min(T, lane), carry_t);
+    carry_t = __shfl_sync(0xffffffffu, m, 31);
+    return m;
+}
+
 template <bool MEDIAN>
 struct RayScan {
     float carry_e = 0.0f;     // sum of sigma*delta before this chunk
@@ -49,15 +60,8 @@ struct RayScan {
         return w;
     }
 
-    // after step(), on every lane of the chunk: the running minimum of T along the ray, for the CDF 1 - T.  The scans
-    // of two neighbouring lanes are different trees and can invert by an ulp where a sample adds (next to) nothing, so
-    // T itself may rise by an ulp and the CDF would fall.  The minimum is some T_j, j <= i, whose prefix and error
-    // bound are no larger than sample i's, so it stays within T_i's bound.
-    __device__ __forceinline__ float monotone(float T, int lane) {
-        const float m = fminf(warp_scan_min(T, lane), carry_t);
-        carry_t = __shfl_sync(0xffffffffu, m, 31);
-        return m;
-    }
+    // after step(), on every lane of the chunk: the running minimum of T along the ray (monotone_trans)
+    __device__ __forceinline__ float monotone(float T, int lane) { return monotone_trans(T, carry_t, lane); }
 
     // on every lane after the last chunk: opacity clamped to [1e-6, 1], depth = sum w*mid / opacity, median depth
     __device__ __forceinline__ void finish(float& op, float& depth, float& median) {

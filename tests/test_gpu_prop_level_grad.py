@@ -360,11 +360,12 @@ def test_level_backward_vs_fp64(case, restore_sinks):
 
 
 # ------------------------------------------------------------------------------------------------- the production step
-def _interlevel(s, cdf, prop_s, prop_cdf, r, dtype=torch.float64, chunk=1024):
+def _interlevel(s, cdf, prop_s, prop_cdf, r, dtype=torch.float64, chunk=1024, reduce=True):
     """One level's anti-aliased interlevel term in ``dtype`` (the restatement of test_gpu_kernels.py::
     test_interlevel_loss_value_and_gradient_vs_oracle, nerfacc_prop_net.py:22-60,182-240 of the reference): blur the
     final histogram, integrate it, interpolate at the level's edges, hinge against the level's weights.  Only
-    ``prop_cdf`` carries gradient; the dense bracketing masks are built ``chunk`` rays at a time."""
+    ``prop_cdf`` carries gradient; the dense bracketing masks are built ``chunk`` rays at a time.  ``reduce=False``:
+    the [R, n] terms instead of their mean."""
     with torch.no_grad():
         s_, ps_, cdf_ = s.to(dtype), prop_s.to(dtype), cdf.to(dtype)
         w_n = (cdf_[:, 1:] - cdf_[:, :-1]) / (s_[:, 1:] - s_[:, :-1])
@@ -375,7 +376,8 @@ def _interlevel(s, cdf, prop_s, prop_cdf, r, dtype=torch.float64, chunk=1024):
                                                                cd[i:i + chunk]), dim=-1)
                          for i in range(0, s.shape[0], chunk)])
     wp = prop_cdf[:, 1:] - prop_cdf[:, :-1]
-    return ((w_s - wp).clamp_min(0) ** 2 / (wp + 1e-5)).mean()
+    terms = (w_s - wp).clamp_min(0) ** 2 / (wp + 1e-5)
+    return terms.mean() if reduce else terms
 
 
 # Sinks against the fp64 gradient of the whole loss.  Measured on an NVIDIA H100 80GB HBM3 at 700 W: table 2.9e-5,
