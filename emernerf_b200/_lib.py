@@ -169,6 +169,9 @@ _SIGNATURES = {
                         POINTER(EmerVoxelGrid), _P],
     "emer_voxel_compact": [POINTER(EmerVoxelGrid), c_int, _P, _P, _P, _P],
     "emer_voxel_select": [_P, _P, _P, c_int, c_float, _P, _P, c_int64, c_int, _P, _P, _P, c_int64, _P, _P, _P, _P, _P],
+    "emer_flow_vis_select": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, _P,
+                             c_int, c_float, c_float, _P, _P, _P, _P, _P, _P, _P],
+    "emer_flow_vis_color": [_P, c_int64, _P, c_float, c_int64, c_int, c_float, _P, c_int, _P, c_int64, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])
@@ -263,6 +266,10 @@ def tag_of(name: str, args) -> str:
             return f"G{args[1]}" + ("_write" if args[3].value else "_count")
         if name == "emer_voxel_select":
             return f"K{args[3]}_C{args[8]}_N{args[12]}"
+        if name == "emer_flow_vis_select":
+            return f"N{args[12]}_C{args[14]}"
+        if name == "emer_flow_vis_color":
+            return f"N{args[4]}" + ("_G" if args[2].value else "") + ("" if args[9].value else "_radius")
         if name == "emer_flow_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("" if args[18].value else "_density")
         if name == "emer_flow_field_bwd":

@@ -8,13 +8,14 @@
 //   that takes the last ticket scans them per grid and writes the totals; the write pass turns each block's bits into
 //   coordinates at its scanned offset.  Integer arithmetic only.
 // emer_voxel_select: tiles of EMER_VOXEL_SELECT_TILE rows taken in ticket order; each tile waits for the previous
-//   tile's inclusive count (a chained scan), so the kept rows land in row order behind the running count.  A tile is
-//   only ever taken by a running CTA and every earlier tile by an earlier one, so the wait always ends.
+//   tile's inclusive count (the chained scan of ordered_scan.cuh), so the kept rows land in row order behind the
+//   running count.
 //
 // The arithmetic is the reference's fp32 with one rounding per torch op; the file is compiled with -fmad=false and
 // spells every rounding with an intrinsic anyway.
 #include "common.cuh"
 #include "cta_reduce.cuh"
+#include "ordered_scan.cuh"
 
 namespace emer {
 
@@ -88,27 +89,6 @@ __device__ __forceinline__ int grid_of_block(const CompactParams& p, int64_t b) 
     return g;
 }
 
-// Exclusive block scan of one value per thread (VX_THREADS threads); returns this thread's prefix, *total the sum.
-__device__ __forceinline__ long long block_exclusive_scan(long long v, long long* sh, long long* total) {
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    long long incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const long long t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    __syncthreads();
-    if (lane == 31) sh[wid] = incl;
-    __syncthreads();
-    long long before = 0, all = 0;
-    for (int w = 0; w < VX_THREADS / 32; ++w) {
-        if (w < wid) before += sh[w];
-        all += sh[w];
-    }
-    *total = all;
-    return before + incl - v;
-}
-
 __global__ void __launch_bounds__(VX_THREADS) voxel_count_kernel(const CompactParams p) {
     __shared__ long long sh[VX_THREADS / 32];
     for (int64_t b = blockIdx.x; b < p.block0[p.n]; b += gridDim.x) {
@@ -121,7 +101,7 @@ __global__ void __launch_bounds__(VX_THREADS) voxel_count_kernel(const CompactPa
             if (w < p.words[g]) c += __popc(__ldg(p.g[g].bits + w));
         }
         long long total;
-        block_exclusive_scan(c, sh, &total);
+        block_exclusive_scan<VX_THREADS>(c, sh, &total);
         if (threadIdx.x == 0) p.blocks[b] = total;
     }
     if (!take_last_ticket(p.ticket)) return;
@@ -132,7 +112,7 @@ __global__ void __launch_bounds__(VX_THREADS) voxel_count_kernel(const CompactPa
             const int64_t b = b0 + threadIdx.x;
             const long long v = b < p.block0[g + 1] ? __ldcg(p.blocks + b) : 0;
             long long total;
-            const long long ex = block_exclusive_scan(v, sh, &total);
+            const long long ex = block_exclusive_scan<VX_THREADS>(v, sh, &total);
             if (b < p.block0[g + 1]) p.blocks[b] = carry + ex;
             carry += total;
         }
@@ -156,7 +136,7 @@ __global__ void __launch_bounds__(VX_THREADS) voxel_write_kernel(const CompactPa
             c += __popc(bits[i]);
         }
         long long total;
-        long long row = p.first_row[g] + __ldcg(p.blocks + b) + block_exclusive_scan(c, sh, &total);
+        long long row = p.first_row[g] + __ldcg(p.blocks + b) + block_exclusive_scan<VX_THREADS>(c, sh, &total);
         const int64_t yz = G.res[1] * G.res[2];
 #pragma unroll
         for (int i = 0; i < VX_WORDS_PER_THREAD; ++i) {
@@ -207,7 +187,7 @@ __global__ void __launch_bounds__(VX_THREADS) voxel_select_kernel(const SelectPa
     __shared__ long long round_base[VX_ROWS_PER_THREAD + 1];
     __shared__ long long tile_base;
     __shared__ int64_t tile_s;
-    if (threadIdx.x == 0) tile_s = atomicAdd(p.ticket, 1u);
+    if (threadIdx.x == 0) tile_s = take_tile(p.ticket);
     __syncthreads();
     const int64_t tile = tile_s;
     const int64_t r0 = tile * EMER_VOXEL_SELECT_TILE;
@@ -223,30 +203,11 @@ __global__ void __launch_bounds__(VX_THREADS) voxel_select_kernel(const SelectPa
 #pragma unroll
     for (int i = 0; i < VX_ROWS_PER_THREAD; ++i) {
         long long total;
-        mine[i] = (int)block_exclusive_scan((keep >> i) & 1u, sh, &total);
+        mine[i] = (int)block_exclusive_scan<VX_THREADS>((keep >> i) & 1u, sh, &total);
         if (threadIdx.x == 0) round_base[i] = acc;
         acc += total;
     }
-    if (threadIdx.x == 0) {
-        long long before;
-        if (tile == 0) {
-            before = *(volatile long long*)p.count;
-        } else {
-            unsigned long long f;
-            while ((f = atomicAdd(p.flags + tile - 1, 0ull)) == 0ull) __nanosleep(32);
-            p.flags[tile - 1] = 0ull;                 // only this tile reads it: left zeroed for the next call
-            before = (long long)(f - 1ull);
-        }
-        tile_base = before;
-        const long long after = before + acc;
-        if (tile + 1 < p.tiles) {
-            __threadfence();
-            atomicExch(p.flags + tile, (unsigned long long)after + 1ull);
-        } else {
-            *p.count = after;
-            *p.ticket = 0u;                           // every tile has been taken: ready for the next call
-        }
-    }
+    if (threadIdx.x == 0) tile_base = chain_tile(tile, p.tiles, acc, p.count, p.ticket, p.flags);
     __syncthreads();
     const int c4 = p.c >> 2;
 #pragma unroll

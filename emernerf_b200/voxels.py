@@ -67,15 +67,27 @@ SELECT_WORKSPACE_BYTES = 65600   # EMER_VOXEL_SELECT_WORKSPACE_BYTES
 _WS: Dict[object, Tensor] = {}
 
 
+def grown_box(aabb: Tensor) -> Tuple[Tensor, Tensor]:
+    """The reference's figure box on ``aabb``'s device, fp32: (vis_aabb [6], its extent [3]).  The box grows by 1 on
+    y_min, z_min and every maximum, not on x_min.  No host sync."""
+    vis_aabb = aabb.detach().reshape(-1).to(torch.float32).clone()
+    vis_aabb[1:3] -= 1
+    vis_aabb[3:] += 1
+    aabb_min, aabb_max = torch.split(vis_aabb, 3, dim=-1)
+    return vis_aabb, aabb_max - aabb_min
+
+
+def box_ratios(length) -> Tuple[float, float, float]:
+    """The figure's x, y and z ratios: 1 and the fp32 quotients of the box's extents, as the reference's ``.item()``."""
+    l0, l1, l2 = np.asarray(length, np.float32)
+    return 1, float(l1 / l0), float(l2 / l0)
+
+
 class VoxelGeometry:
     """The box, resolutions and voxel sizes of the reference, computed on ``device`` with its torch ops (one sync)."""
 
     def __init__(self, aabb: Tensor, vis_voxel_size: float):
-        vis_aabb = aabb.detach().reshape(-1).to(torch.float32).clone()
-        vis_aabb[1:3] -= 1
-        vis_aabb[3:] += 1
-        aabb_min, aabb_max = torch.split(vis_aabb, 3, dim=-1)
-        length = aabb_max - aabb_min
+        vis_aabb, length = grown_box(aabb)
         res_s = torch.ceil(length / vis_voxel_size).long()
         res_d = torch.ceil(length / vis_voxel_size * 0.8).long()
         packed = torch.cat([vis_aabb, length, length / res_s, length / res_d]).double()
@@ -91,8 +103,7 @@ class VoxelGeometry:
                 raise ValueError(f"voxel lifting: a {res[0]} x {res[1]} x {res[2]} grid (1 to 2^32 voxels)")
 
     def ratios(self) -> Tuple[float, float, float]:
-        l0, l1, l2 = self.length
-        return 1, float(l1 / l0), float(l2 / l0)
+        return box_ratios(self.length)
 
 
 class BitGrid:

@@ -769,6 +769,41 @@ int emer_voxel_select(const float* d0, const float* d1, const float* d2, int k, 
                       const float* color_min, const float* color_max, int64_t n, float* out_points,
                       float* out_colors, int64_t* count, void* workspace, void* stream);
 
+/* ---- scene-flow figure (csrc/flow_vis.cu; replaces utils/visualization_tools.py:729-821, visualize_scene_flow, with
+ *      its boolean indexes, per-camera inverse() syncs and masked assignments per frame, and scene_flow_to_rgb).
+ *      The colour is scene_flow_to_rgb's, restated once in csrc/flow_color.cuh with one rounding per torch op. ---- */
+#define EMER_FLOW_VIS_TILE 1024                   /* points per emer_flow_vis_select tile */
+#define EMER_FLOW_VIS_MAX_ROWS (1 << 24)          /* points per emer_flow_vis_select call */
+#define EMER_FLOW_VIS_WORKSPACE_BYTES 131080      /* ticket + one flag per tile */
+#define EMER_FLOW_VIS_MAX_CAMS 16
+enum { EMER_FLOW_SCALE_NONE = 0, EMER_FLOW_SCALE_HOST = 1, EMER_FLOW_SCALE_DEVICE = 2 };
+/* One lidar frame of n points (n <= EMER_FLOW_VIS_MAX_ROWS): origins, viewdirs and flows rows of 3 floats, ranges,
+ * times and int64 flow classes, each with its row stride (read in place).  A point is labelled when its class is not
+ * -1.  A labelled point p = origin + range * viewdir (two fp32 roundings) is kept when, for any of the num_cams
+ * (<= EMER_FLOW_VIS_MAX_CAMS) dense 4x4 lidar2img matrices M (device), d = M[:3, :3] p + M[:3, 3] (a k-ordered fma
+ * chain, then the translation added) has d[2] > 0 and u, v = d[0] / (d[2] + 1e-6f), d[1] / (d[2] + 1e-6f) with
+ * 0 <= u < width and 0 <= v < height.  Kept points are appended in point order at *count (int64, device), which is
+ * advanced: p to points (dense [., 3]), the time to out_times, and to rows9 (dense [., 9]) p in columns 0..2 and the
+ * flow's colour (scene_flow_to_rgb, flow_max_radius 2, "bright") in columns 6..8.  frame_counts (int64 [2], device)
+ * += (labelled, kept), with integer atomics.  workspace: EMER_FLOW_VIS_WORKSPACE_BYTES, zeroed once by its owner and
+ * left zeroed by every call.  The output is deterministic. */
+int emer_flow_vis_select(const float* origins, int64_t ld_origins, const float* viewdirs, int64_t ld_viewdirs,
+                         const float* ranges, int64_t ld_ranges, const float* times, int64_t ld_times,
+                         const float* flows, int64_t ld_flows, const int64_t* classes, int64_t ld_classes, int64_t n,
+                         const float* lidar2img, int num_cams, float width, float height, float* points,
+                         float* out_times, float* rows9, int64_t* count, int64_t* frame_counts, void* workspace,
+                         void* stream);
+/* scene_flow_to_rgb of n flows (rows of at least 2 floats, x and y first, row stride ld_flow, read in place).  With
+ * density (dense, device) the flow is first gated as pred[density < threshold] *= 0 (NaN is not gated).  scale_mode
+ * EMER_FLOW_SCALE_HOST: the radius is divided by radius_scale as torch's CUDA division by a host scalar does it (times
+ * 1.0f / radius_scale; the reference's radius_scale > 0 test is the caller's); EMER_FLOW_SCALE_DEVICE: by
+ * *device_radius when it is > 0 (a true division); EMER_FLOW_SCALE_NONE: not at all.  bright selects the "bright" background, else "dark".  colors (rows of
+ * 3 floats, row stride ld_colors) receive the colours; a NaN radius or angle gives NaN in all three channels.  With
+ * colors NULL, radius (dense) receives the unscaled radii of the gated flows instead.  One launch, no host sync. */
+int emer_flow_vis_color(const float* flow, int64_t ld_flow, const float* density, float threshold, int64_t n,
+                        int scale_mode, float radius_scale, const float* device_radius, int bright, float* colors,
+                        int64_t ld_colors, float* radius, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
