@@ -85,6 +85,14 @@ __device__ __forceinline__ void stage_weight_t(uint8_t* hi, uint8_t* lo, const f
     }
 }
 
+// ReLU that keeps NaN, as the reference's torch.relu does: fmaxf(NaN, 0) is 0, which would turn a NaN encoding row
+// into a plausible finite density and colour.  One FMNMX with the NaN flag, the cost of fmaxf.
+__device__ __forceinline__ float relu(float x) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(x), "f"(0.0f));
+    return r;
+}
+
 __device__ __forceinline__ float2 ld2(const float* p, bool ok) {
     return ok ? __ldg(reinterpret_cast<const float2*>(p)) : make_float2(0.f, 0.f);
 }
@@ -211,8 +219,8 @@ __device__ __forceinline__ void field_fwd_body(const FwdParams& p) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int c = 8 * j + 2 * q;
-                const float v0 = fmaxf(acc[4 * j] + bb0_s[c], 0.0f), v1 = fmaxf(acc[4 * j + 1] + bb0_s[c + 1], 0.0f);
-                const float v2 = fmaxf(acc[4 * j + 2] + bb0_s[c], 0.0f), v3 = fmaxf(acc[4 * j + 3] + bb0_s[c + 1], 0.0f);
+                const float v0 = relu(acc[4 * j] + bb0_s[c]), v1 = relu(acc[4 * j + 1] + bb0_s[c + 1]);
+                const float v2 = relu(acc[4 * j + 2] + bb0_s[c]), v3 = relu(acc[4 * j + 3] + bb0_s[c + 1]);
                 if (p.save_hb) {
                     st2(p.save_hb + (qo + row0) * H + c, v0, v1, ok0);
                     st2(p.save_hb + (qo + row1) * H + c, v2, v3, ok1);
@@ -295,8 +303,8 @@ __device__ __forceinline__ void field_fwd_body(const FwdParams& p) {
         for (int j = 0; j < 8; ++j) {
             const int c = 8 * j + 2 * q;
             const float2 b0 = __ldg(reinterpret_cast<const float2*>(rb0 + c)), b1 = __ldg(reinterpret_cast<const float2*>(rb1 + c));
-            const float v0 = fmaxf(d0[4 * j] + b0.x, 0.0f), v1 = fmaxf(d0[4 * j + 1] + b0.y, 0.0f);
-            const float v2 = fmaxf(d0[4 * j + 2] + b1.x, 0.0f), v3 = fmaxf(d0[4 * j + 3] + b1.y, 0.0f);
+            const float v0 = relu(d0[4 * j] + b0.x), v1 = relu(d0[4 * j + 1] + b0.y);
+            const float v2 = relu(d0[4 * j + 2] + b1.x), v3 = relu(d0[4 * j + 3] + b1.y);
             if (p.save_hg) {
                 st2(p.save_hg + row0 * 128 + c, v0, v1, ok0);
                 st2(p.save_hg + row1 * 128 + c, v2, v3, ok1);
@@ -316,8 +324,8 @@ __device__ __forceinline__ void field_fwd_body(const FwdParams& p) {
             const int c = 8 * j + 2 * q;
             const float2 b0 = __ldg(reinterpret_cast<const float2*>(rb0 + H + c));
             const float2 b1 = __ldg(reinterpret_cast<const float2*>(rb1 + H + c));
-            const float v0 = fmaxf(d1[4 * j] + b0.x, 0.0f), v1 = fmaxf(d1[4 * j + 1] + b0.y, 0.0f);
-            const float v2 = fmaxf(d1[4 * j + 2] + b1.x, 0.0f), v3 = fmaxf(d1[4 * j + 3] + b1.y, 0.0f);
+            const float v0 = relu(d1[4 * j] + b0.x), v1 = relu(d1[4 * j + 1] + b0.y);
+            const float v2 = relu(d1[4 * j + 2] + b1.x), v3 = relu(d1[4 * j + 3] + b1.y);
             if (p.save_h1) {
                 st2(p.save_h1 + row0 * H + c, v0, v1, ok0);
                 st2(p.save_h1 + row1 * H + c, v2, v3, ok1);
