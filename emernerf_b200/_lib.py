@@ -95,6 +95,12 @@ class EmerVoxelGrid(ctypes.Structure):
     _fields_ = [("min", c_float * 3), ("voxel_size", c_float * 3), ("res", c_int64 * 3), ("bits", _P),
                 ("first_row", c_int64)]
 
+
+# host struct of emer_video_compose (include/emer_b200.h): field names and order as there
+class EmerVideoTile(ctypes.Structure):
+    _fields_ = [("inputs", _P * 3), ("kind", c_int32), ("row", c_int32), ("invert", c_int32), ("f64", c_int32)]
+
+
 # number of kernels this library launched through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = 0
 
@@ -172,6 +178,7 @@ _SIGNATURES = {
     "emer_flow_vis_select": [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, _P,
                              c_int, c_float, c_float, _P, _P, _P, _P, _P, _P, _P],
     "emer_flow_vis_color": [_P, c_int64, _P, c_float, c_int64, c_int, c_float, _P, c_int, _P, c_int64, _P, _P],
+    "emer_video_compose": [_P, c_int64, POINTER(EmerVideoTile), c_int, c_int64, c_int64, c_int, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGNATURES) + ["emer_last_error", "emer_version"])
@@ -270,6 +277,8 @@ def tag_of(name: str, args) -> str:
             return f"N{args[12]}_C{args[14]}"
         if name == "emer_flow_vis_color":
             return f"N{args[4]}" + ("_G" if args[2].value else "") + ("" if args[9].value else "_radius")
+        if name == "emer_video_compose":
+            return f"T{args[3]}_H{args[4]}_W{args[5]}"
         if name == "emer_flow_field_fwd":
             return f"k{args[2]}_f{args[7]}_N{args[23]}" + ("" if args[18].value else "_density")
         if name == "emer_flow_field_bwd":

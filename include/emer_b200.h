@@ -804,6 +804,36 @@ int emer_flow_vis_color(const float* flow, int64_t ld_flow, const float* density
                         int scale_mode, float radius_scale, const float* device_radius, int bright, float* colors,
                         int64_t ld_colors, float* radius, void* stream);
 
+/* ---- evaluation video frames (csrc/video.cu; replaces the host side of radiance_fields/video_utils.py:471-627,
+ *      save_videos: visualize_depth's turbo colouring, the two numpy blends, the sky-mask tiles, np.concatenate and
+ *      to8b).  The formulas are stated once, in csrc/video.cuh. ---- */
+#define EMER_VIDEO_MAX_TILES 32                   /* rows of one frame, one tile each per emer_video_compose call */
+#define EMER_VIDEO_MAX_PIXELS (1 << 26)           /* H * W of one tile */
+enum { EMER_VIDEO_RGB = 0, EMER_VIDEO_DEPTH = 1, EMER_VIDEO_BLEND = 2, EMER_VIDEO_GRAY = 3 };
+/* One tile of a frame: an [H, W] image of one product, written at frame row `row` (rows of H pixels).  Inputs are
+ * dense float32 [H * W, C] on the device:
+ *   EMER_VIDEO_RGB    in[0] [., 3]: to8b of the pixel;
+ *   EMER_VIDEO_DEPTH  in[0] depth [., 1], in[1] opacity [., 1]: visualize_depth(lo=4, hi=120, curve -log(x + 1e-6)),
+ *                     i.e. the turbo entry of clip((curve(d) - curve(hi)) / |curve(hi) - curve(lo)|, 0, 1) (NaN to 0)
+ *                     times the opacity, by matplotlib's rule min(int(v * 256), 255), 0 below 0, black for NaN;
+ *   EMER_VIDEO_BLEND  in[0] a [., 3], in[1] alpha [., 1], in[2] b [., 3]: np.clip(a * alpha + b * (1 - alpha), 0, 1)
+ *                     in float32, one rounding per operation;
+ *   EMER_VIDEO_GRAY   in[0] [., 1]: the value in all three channels, 1 - value when invert is set.
+ * f64: the product reaches to8b as float64 (its frame holds a depth row), so 255 * x is a float64 product; otherwise
+ * a float32 one.  Either is truncated to uint8 after np.clip(x, 0, 1); NaN gives 0. */
+typedef struct emer_video_tile {
+    const float* in[3];
+    int32_t kind;
+    int32_t row;
+    int32_t invert;
+    int32_t f64;
+} emer_video_tile;
+/* Writes n_tiles (1..EMER_VIDEO_MAX_TILES) tiles of one image into the uint8 frame [rows * H, frame_w, 3] (device),
+ * at pixel column col * W of their rows; the caller owns the frame's height.  lut: the turbo table, 256 x 3 uint8
+ * (device), trunc(255 * colour) in float64, read by EMER_VIDEO_DEPTH tiles.  One launch, no host sync. */
+int emer_video_compose(uint8_t* frame, int64_t frame_w, const emer_video_tile* tiles, int n_tiles, int64_t height,
+                       int64_t width, int col, const uint8_t* lut, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
